@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- Bit-Swap encode+decode throughput on B200 (BASELINE.json metric).
+"""bench.py -- Bit-Swap encode+decode throughput on H100 (BASELINE.json metric).
 
 A "step" = one pass of the hot path over one batch: Bit-Swap ENCODE of B images (one per ANS stream)
 followed by Bit-Swap DECODE of the same B images, CIFAR-shaped 32x32x3 uint8, 8-latent VAE
@@ -16,7 +16,7 @@ state, so steps repeat without re-initialisation.
                to host, all copies inside the timed region.
   roofline     dominant kernel category, from CUDA events around every launch in a replay of the
                timed steps with the SAME launch shapes (the lanes run back to back instead of
-               concurrently); traffic / FP64 instruction counts from the tracked ncu summary.
+               concurrently).
   cpu_baseline the oracle port of the reference path (torch-CPU nets + float64 tables + Python-loop
                ANS) on this box's host cores: latency mode with the 5-way time split and
                throughput mode (cores/16 processes of 16 threads, one chain each), bounded samples.
@@ -24,6 +24,11 @@ state, so steps repeat without re-initialisation.
 `--impl reference` times that CPU path as its own arm (the reference is pure Python and cannot be
 pip-installed/travel; DESIGN.md).  `--config crop` is BASELINE configs[4]: 100 variable-size images as
 chained 32x32 block streams over the GPUs, next to gzip/bz2/lzma/PNG/WebP on the host.
+
+`--dump-outputs DIR` writes what the timed path returned in its last step as DIR/<name>.npy (float32 / float64, the
+inputs are seeded, so two builds can be compared output for output): the trimmed bitstreams the encode produced
+(the words above each stream's lowest depth, per-stream lengths, bases and 64-bit heads split into 32-bit halves) and
+the pixels the decode restored.  Above 1024 streams a fixed seeded sample of 1024 streams is written.
 """
 import argparse
 import hashlib
@@ -53,14 +58,8 @@ def measured_peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"], bf16_tflops_sustained=d["bf16_tflops_sustained"],
                     source="MEASURED_PEAKS.json")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
-
-
-def ncu_facts():
-    """Per-kernel facts taken from the tracked ncu captures (profiles/ncu_facts_r2.json, written by
-    scripts/ncu_summary.py facts): dram bytes per launch, FP64-pipe instructions per launch, streams per launch."""
-    p = os.path.join(ROOT, "profiles", "ncu_facts_r2.json")
-    return json.load(open(p)) if os.path.exists(p) else {}
+    # NVIDIA's H100 SXM data sheet (dense bf16, 700 W board): a ceiling to divide by, not a rate this card reached
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source="H100 SXM data sheet")
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -194,9 +193,7 @@ def _tp_init(config, threads):
 class ThroughputPool:
     """All host cores on the reference's CPU path (BASELINE.md 3, throughput mode): `procs` worker processes of `threads`
     torch threads each, procs x threads = cores, every worker its own chain.  16 threads per chain is where the path's torch
-    ops stop scaling for one chain.  One single-threaded process per core was measured too and is the stronger aggregate
-    (profiles/bench_r2_reference_arm_1thread.json: 0.0026 against 0.0018 Mpixel/s on 128 cores) but needs 48 s per image,
-    i.e. 20 minutes for the 25-step arm the driver launches; the line says so (`single_thread_per_core`)."""
+    ops stop scaling for one chain."""
 
     def __init__(self, config, procs, threads):
         import multiprocessing as mp
@@ -258,9 +255,7 @@ def run_reference_arm(args, cfg, rank, world):
             "latency_mode": {"threads": threads, "encode_s_per_image": e / 2, "decode_s_per_image": d / 2,
                              "Mpixel_s": 2 * 1024 / (e + d) / 1e6, "time_split": split,
                              "sample": "one 2-image chain alone on the box"},
-            "cpu_baseline": {"value": val, "unit": UNIT, "cores": procs * threads, "kind": "port", "sample": sample,
-                             "single_thread_per_core": "measured once on this pool's 128-core host: 0.0026 Mpixel/s, 48 s per step "
-                                                       "(profiles/bench_r2_reference_arm_1thread.json) -- 1.45x this arm's rate"},
+            "cpu_baseline": {"value": val, "unit": UNIT, "cores": procs * threads, "kind": "port", "sample": sample},
             "e2e": {"value": val, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     print(json.dumps(line))
 
@@ -283,8 +278,6 @@ def cpu_baseline_block(config, images, tp_steps):
         wall += w; imgs += n
     pool.close()
     out.update(value=imgs * 1024 / wall / 1e6, cores=procs * threads,
-               single_thread_per_core="measured once on this pool's 128-core host: 0.0026 Mpixel/s "
-                                      "(profiles/bench_r2_reference_arm_1thread.json)",
                sample=f"throughput mode: {procs} processes x {threads} torch threads x {tp_steps} image(s) each, encode + decode "
                       f"({os.cpu_count()} host cores); latency mode beside it")
     return out
@@ -301,6 +294,27 @@ def states_digest(ss, first=0, count=None):
     return h.hexdigest()[:16]
 
 
+def dump_outputs(d, pixels, words, offs, heads, base, max_streams=1024):
+    """The timed path's outputs as DIR/<name>.npy in float32 / float64 (exact for uint8 pixels and 32-bit words), at most
+    `max_streams` streams (a fixed seeded sample above that): well under 64 MB at any batch."""
+    B = pixels.shape[0]
+    idx = np.arange(B) if B <= max_streams else np.sort(np.random.RandomState(0).choice(B, max_streams, replace=False))
+    words, heads = words.view(np.uint32), heads.view(np.uint64)
+    sel = [words[offs[i]:offs[i + 1]] for i in idx]
+    out = {"decoded_pixels": pixels[idx].astype(np.float32),
+           "stream_index": idx.astype(np.float64),
+           "encoded_words": np.concatenate(sel).astype(np.float64),
+           "encoded_lengths": np.array([len(v) for v in sel], dtype=np.float64),
+           "encoded_base": base[idx].astype(np.float64),
+           "encoded_head_hi": (heads[idx] >> np.uint64(32)).astype(np.float64),
+           "encoded_head_lo": (heads[idx] & np.uint64(0xffffffff)).astype(np.float64)}
+    total = sum(a.nbytes for a in out.values())
+    assert total <= 64 << 20, f"dump of {total} bytes exceeds 64 MB"
+    os.makedirs(d, exist_ok=True)
+    for k, a in out.items():
+        np.save(os.path.join(d, k + ".npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -309,7 +323,7 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", default="cifar8", help="cifar8 (BASELINE configs[1], default), imagenet4, mnist2, ..., or crop (configs[4])")
     ap.add_argument("--batch", type=int, default=0, help="streams (= images per step) PER GPU (default 1024; imagenet4: 4096)")
-    ap.add_argument("--tensor-cores", type=int, default=-1, help="-1 auto, 0 SIMT fp32 convs, 1 tcgen05")
+    ap.add_argument("--tensor-cores", type=int, default=-1, help="-1 auto, 0 SIMT fp32 convs, 1 wgmma tensor-core convs")
     ap.add_argument("--ref-procs", type=int, default=0, help="worker processes (of 16 threads) of the CPU reference arm (0 = cores / 16)")
     ap.add_argument("--cpu-baseline-images", type=int, default=4)
     ap.add_argument("--no-cpu-baseline", action="store_true")
@@ -321,6 +335,8 @@ def main():
     ap.add_argument("--fused-coder", action="store_true", help="one-warp-per-stream fused coder kernels instead of the two-phase coder")
     ap.add_argument("--crop-images", type=int, default=100)
     ap.add_argument("--hwc-quirk", action="store_true", help="crop: feed blocks as imagenetcrop_compress.py:130 does")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's bitstreams and decoded pixels as DIR/<name>.npy (rank 0's shard)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -348,7 +364,6 @@ def main():
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     dev = torch.device("cuda", local)
     peaks = measured_peaks()
-    facts = ncu_facts()
 
     B = args.batch or (4096 if args.config == "imagenet4" else 1024)
     use_tc = args.tensor_cores
@@ -419,9 +434,14 @@ def main():
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(3 * args.steps + 1)]
     ev[0].record()
     gathered_words = 0
+    snap = None
     for i in range(args.steps):
         codec.encode(ss, x_dev)
         ev[3 * i + 1].record()
+        if args.dump_outputs and i == args.steps - 1:        # the encoded bitstreams, before the decode consumes them
+            if free_running:
+                codec.join()
+            snap = [t.clone() for t in ss.pack_device(trim=True)]
         if world > 1:
             W, M, counts = gather_step()
         ev[3 * i + 2].record()
@@ -431,6 +451,9 @@ def main():
         ev[3 * i + 3].record()
     torch.cuda.synchronize()
     codec.free_running = False
+    if snap is not None and rank == 0:
+        words_d, offs_d, heads_d, base_d = (t.cpu().numpy() for t in snap)
+        dump_outputs(args.dump_outputs, out_dev.cpu().numpy(), words_d, offs_d, heads_d, base_d)
     total_ms = ev[0].elapsed_time(ev[-1])
     enc_ms = sum(ev[3 * i].elapsed_time(ev[3 * i + 1]) for i in range(args.steps))
     gat_ms = sum(ev[3 * i + 1].elapsed_time(ev[3 * i + 2]) for i in range(args.steps))
@@ -536,21 +559,11 @@ def main():
             bound, work = per_launch[k]
             sec = ms / n * 1e-3
             if bound == "tensor":
-                rec.update(bound="tensor", achieved=work / sec / 1e12, peak=peaks["bf16_tflops_sustained"], unit="TFLOP/s",
+                rec.update(bound="tensor", achieved=work / sec / 1e12, peak=peaks["bf16_tflops"], unit="TFLOP/s",
                            mma_tflops_issued=3 * work * (256 / cfg.reswidth) ** 2 / sec / 1e12 if use_tc else None)
             else:
                 rec.update(bound="hbm", achieved=work / sec / 1e9, peak=peaks["hbm_gbs"], unit="GB/s", algorithmic_bytes_per_launch=work)
             rec["frac"] = rec["achieved"] / rec["peak"]
-            fk = facts.get(k)
-            if fk and fk.get("streams_per_launch"):
-                scale = Bl / fk["streams_per_launch"]
-                rec["traffic"] = fk["dram_bytes_per_launch"] * scale
-                rec["traffic_source"] = fk.get("source")
-                if fk.get("fp64_inst_per_launch"):
-                    lanes_per_s = 32.0 * fk["fp64_inst_per_launch"] * scale / sec
-                    rec["fp64"] = {"warp_instructions_per_launch": fk["fp64_inst_per_launch"] * scale, "achieved_lanes_per_s": lanes_per_s,
-                                   "peak_measured_dfma_lanes_per_s": fp64_peak, "frac": lanes_per_s / fp64_peak,
-                                   "source": "sm__inst_executed_pipe_fp64 of " + str(fk.get("source"))}
         kernels[k] = rec
     # dominant kernel: among the THROUGHPUT kernels (tables, convs).  The serial coder kernels are latency-bound -- their
     # duration does not depend on the stream count, so the lane-by-lane replay counts them once per lane although in the
@@ -558,19 +571,15 @@ def main():
     dom = max((k for k in kernels if "bound" in kernels[k] and (k.startswith("conv") or k.startswith("rows"))),
               key=lambda k: kernels[k]["ms_per_step"])
     roofline = {"kernel": dom, "bound": kernels[dom]["bound"], "achieved": kernels[dom]["achieved"], "peak": kernels[dom]["peak"],
-                "unit": kernels[dom]["unit"], "frac": kernels[dom]["frac"], "traffic": kernels[dom].get("traffic"),
-                "traffic_source": kernels[dom].get("traffic_source"),
-                "peak_source": peaks["source"] + (" bf16_tflops_sustained" if kernels[dom]["bound"] == "tensor" else " hbm_gbs"),
-                "share_of_step": kernels[dom]["share"], "streams_per_launch": Bl}
-    if "fp64" in kernels[dom]:
-        roofline["fp64"] = kernels[dom]["fp64"]
+                "unit": kernels[dom]["unit"], "frac": kernels[dom]["frac"],
+                "peak_source": peaks["source"] + (" bf16_tflops" if kernels[dom]["bound"] == "tensor" else " hbm_gbs"),
+                "share_of_step": kernels[dom]["share"], "streams_per_launch": Bl, "fp64_peak_measured_dfma_lanes_per_s": fp64_peak}
     if kernels[dom]["bound"] == "hbm":
         roofline["note"] = ("the coder's table kernel is bound by float64 arithmetic, not HBM ((S-1) float64 logistic values per "
-                            "symbol-op, SURVEY.md 8d/H2): the hbm fraction is the contract's figure; `fp64` is the FP64-pipe "
-                            "instruction count of the tracked ncu capture against the measured DFMA peak")
+                            "symbol-op, SURVEY.md 8d/H2): the hbm fraction only shows how far it is from being bandwidth bound")
     line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
             "ms_per_step": total_ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": "f64 tables / int64 coder / " + ("bf16x3 split tcgen05" if use_tc else "f32 SIMT") + " convs",
+            "dtype": "f64 tables / int64 coder / " + ("bf16x3 split wgmma" if use_tc else "f32 SIMT") + " convs",
             "coder": "two-phase (parallel f64 row tables + serial integer coder)" if two_phase else "fused one-warp-per-stream",
             "lanes": codec.lanes,
             "data": "synthetic",
@@ -579,7 +588,7 @@ def main():
                                    + (" + NCCL gather of the produced bitstreams" if world > 1 else "") + " + decode",
                        "streams_per_gpu": B, "global_batch": B * world, "weights": "seeded random init (reference default-init distribution)",
                        "bins": "synthetic uniform grids + float32 equal-mass top level", "images": "iid uniform uint8",
-                       "l2": "per-step working set (3 x 268 MB activations + streams) >> 126 MB L2: no explicit flush needed",
+                       "l2": "per-step working set (3 x 268 MB activations + streams) >> 50 MB L2: no explicit flush needed",
                        "parallelism": f"streams sharded over {world} GPU(s); within a GPU {codec.lanes} sub-batches of {Bl} on separate CUDA streams"},
             "encode_Mpixel_s": None if free_running else px_job / (enc_ms * 1e-3) / 1e6,
             "decode_Mpixel_s": None if free_running else px_job / (dec_ms * 1e-3) / 1e6,

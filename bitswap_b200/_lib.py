@@ -1,4 +1,4 @@
-"""Builds (nvcc, sm_100a) and loads the C-ABI library declared in include/bitswap_b200.h.
+"""Builds (nvcc, sm_90a) and loads the C-ABI library declared in include/bitswap_b200.h.
 
 There is deliberately no CPU fallback: if the shared library is missing or fails to
 load, every product entry point raises."""
@@ -10,7 +10,7 @@ import subprocess
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 SO_PATH = os.path.join(_HERE, "libbitswap_b200.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC"]
 
 _lib = None
@@ -44,7 +44,7 @@ def build(force=False, verbose=False):
             print(out)
         if p.returncode:
             raise RuntimeError(f"nvcc failed on {s}:\n{out}")
-    link = [_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", SO_PATH] + objs
+    link = [_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", SO_PATH] + objs
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode:
         raise RuntimeError("link failed:\n" + r.stdout)

@@ -123,8 +123,7 @@ class PipelinedCodec:
 
     The coder's row-table kernel is FP64-pipe bound and the dense convs are tensor-pipe bound; chains of
     different sub-batches drift apart in phase, so their kernels share SMs and the two pipes overlap
-    (measured on B200, C8, 1024 streams: 379 -> 345 ms per encode+decode step with 4 lanes; more lanes do not
-    help).  Results are identical to a single BitSwapCodec: every stream is independent and every kernel is
+    (4 lanes by default).  Results are identical to a single BitSwapCodec: every stream is independent and every kernel is
     batch-invariant.  Each lane owns a model replica (activations are per-lane anyway)."""
 
     def __init__(self, cfg: CodecConfig, state_dict, bins: Bins, max_batch: int, lanes: int = 4, use_tensor_cores=True, lane_size: int = 0,

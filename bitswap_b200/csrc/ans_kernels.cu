@@ -1,4 +1,4 @@
-// rANS coder kernels + stream sets + bin tables (sm_100a).
+// rANS coder kernels + stream sets + bin tables (sm_90a).
 //
 // Reference being replaced (fhkingma/bitswap @ dfe0bf7d): class ANS, cifar_compress.py:12-67, and the
 // float64 logistic table construction around it, cifar_compress.py:182-187,197-202,245-250.

@@ -1,7 +1,7 @@
-// Two-phase logistic coder (sm_100a): the throughput path of the device-resident codec.
+// Two-phase logistic coder (sm_90a): the throughput path of the device-resident codec.
 //
 // The fused kernels of ans_kernels.cu keep one warp per stream busy with the whole row table, which leaves
-// the FP64 pipe 27 % utilised at 1024 streams (profiles/r1_ncu_logistic_pop_v1.md: 7 warps per SM, long
+// the FP64 pipe 27 % utilised at 1024 streams (7 warps per SM, long
 // dependent DFMA chains).  The table of a row does not depend on the ANS head, only the *search* does, so:
 //
 //   phase A  (k_rows_push / k_rows_pop)   one warp per (stream,row), fully parallel over count x L rows:
@@ -86,7 +86,7 @@ struct WarpStream2 {          // same state handling as ans_kernels.cu's WarpStr
 };
 
 constexpr int RW = 16;       // warps per CTA in phase A: 512 threads x <=64 registers = half an SM's register file, so two
-                             // of these CTAs fill an SM, or one of them sits beside one k_conv_tc CTA (codec.cu overlap)
+                             // of these CTAs fill an SM, or one of them sits beside one k_conv_wg CTA (codec.cu overlap)
 
 // ---- phase A ----------------------------------------------------------------------------------------------------
 // One CTA = one row index for RW (=16) streams, one warp per stream.  The row's endpoints (shared by every stream) are
@@ -332,7 +332,7 @@ __global__ void __launch_bounds__(BW * 32) k_pop_coarse(bsw_streams sv, int firs
     }
     // coarse cdf rows are independent of the head: keep the loads two rows ahead of their use.  (They are issued AFTER
     // the per-row shuffles below: the first version issued the load first and ncu showed every row stalling ~700 cycles
-    // on that load's scoreboard at the first shuffle, profiles/r1_ncu_popcoarse.md.)
+    // on that load's scoreboard at the first shuffle.)
     uint32_t base_n1 = (lane < NB) ? __ldg(cb + (L - 1) * NB + lane) : 0xffffffffu;
     uint32_t base_n2 = (lane < NB && L > 1) ? __ldg(cb + (L - 2) * NB + lane) : 0xffffffffu;
     for (int64_t i = L - 1; i >= 0; --i) {

@@ -1,4 +1,4 @@
-// Affine-row two-phase logistic coder (sm_100a): the throughput path for every table the reference builds over a UNIFORM
+// Affine-row two-phase logistic coder (sm_90a): the throughput path for every table the reference builds over a UNIFORM
 // endpoint grid -- all latent levels below the top one (discretization.py:105-118, KBinsDiscretizer 'uniform') and the
 // pixel level (utils/torch/rand.py:146-147).  Same contract and the same integers as k_rows / k_pop_coarse in ans_rows.cu
 // (ANS.__init__, cifar_compress.py:25-39; ANS.encode/decode :48-67); what differs is how the float64 work is organised:

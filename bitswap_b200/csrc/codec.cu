@@ -1,4 +1,4 @@
-// The bits-back recursions, device resident (sm_100a).
+// The bits-back recursions, device resident (sm_90a).
 //
 // Reference being replaced (fhkingma/bitswap @ dfe0bf7d):
 //   Bit-Swap sender   cifar_compress.py:175-204, 244-250      receiver  :283-317

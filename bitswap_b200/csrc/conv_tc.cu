@@ -1,25 +1,27 @@
-// tcgen05 implicit-GEMM convolution for the dense W->W layers (sm_100a).
+// wgmma implicit-GEMM convolution for the dense W->W layers, the in-convs and the mu/sigma heads (sm_90a).
 //
 // Replaces F.conv2d inside WnConv2d._forward for the 3x3 / 5x5 W->W convolutions of the ResNet blocks
 // (utils/torch/modules.py:98-106 called from ResNetLayer.forward :229-241), which are 98 % of the
 // model's FLOPs (SURVEY.md 6.3).
 //
 // GEMM view (per image):  D[p, o] = sum_{tap, c} A_tap[p, c] * W[tap][o, c]
-//     M = 256 pixels of one 16x16 image (two UMMA M=128 halves), N = 128 output channels per CTA
-//     (grid = images x 2), K = taps x 256 input channels, walked as (tap, 32-channel chunk) k-blocks.
+//     one tile = 128 pixels (8 image rows of a 16x16 image) x N output channels (N = 128 for the W->W convs and the
+//     in-convs, 32 for the heads), K = taps x input channels, walked as (tap, 32-channel chunk) k-blocks.
 //   * A_tap is never materialised (no im2col): the activation tensor is NHWC bf16 and one 4-D TMA box
-//     {32 ch, 16 w, 16 h, 1 img} at coordinates (c0, dx-r, dy-r, img) IS the shifted tile; TMA's
+//     {32 ch, 16 w, 8 h, 1 img} at coordinates (c0, dx-r, dy-r+8*half, img) IS the shifted tile; TMA's
 //     out-of-bounds zero fill supplies the "same" padding.
 //   * float32 accuracy on bf16 tensor cores: every operand is split x = hi + lo (two bf16 planes) and
-//     each k-block issues three MMAs: hi*hi into a MAIN float32 TMEM accumulator, hi*lo and lo*hi into a
-//     separate CROSS accumulator.  The tensor core truncates (RZ) on every accumulate; keeping the 2^-8
-//     smaller cross terms out of the main accumulator cuts its truncating adds 3x (measured: one shared
-//     accumulator gave 1.9e-4 max error through the deepest stack, above the 1e-4 bar).
-//   * accumulators = {main, cross} x 2 halves x (128 lanes x 128 columns) = all 512 TMEM columns.
-//   * warp roles: warp 0 = TMA producer (one elected lane), warp 1 = MMA issuer (one elected lane) and
-//     TMEM allocator, warps 2..9 = epilogue (tcgen05.ld -> bias / residual / ELU / bf16 split -> HBM).
-//   * fixed k order, no split-K, no atomics: results are bit-identical for any batch size or position
-//     in the batch (the decoder must regenerate the encoder's tables exactly, SURVEY.md H3).
+//     each k-block issues three MMAs: hi*hi into a MAIN float32 accumulator, hi*lo and lo*hi into a
+//     separate CROSS accumulator.  The tensor core truncates on every accumulate; keeping the 2^-8 smaller
+//     cross terms out of the main accumulator cuts its truncating adds 3x.
+//   * warp roles: warps 0..7 = two consumer warpgroups, each owning 64 of the tile's 128 pixels and issuing
+//     wgmma.m64nNk16 from shared memory into register accumulators ({main, cross} x N/2 floats per thread),
+//     then running the epilogue (bias / residual / ELU / bf16 split -> HBM) straight from those registers;
+//     warp 8 = TMA producer (one elected lane) feeding an NSTAGE ring of mbarrier-guarded stages.
+//   * a CTA walks tiles t = blockIdx.x, + gridDim.x, ...: with one CTA per tile (per-tile grid) or one per SM
+//     (persistent grid, the producer then prefetches the next tile's k-blocks while the consumers run the epilogue).
+//   * fixed k order, no split-K, no atomics: results are bit-identical for any batch size, position in the batch
+//     or grid (the decoder must regenerate the encoder's tables exactly, SURVEY.md H3).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdlib.h>
@@ -32,28 +34,28 @@ extern "C" int bsw_has_tensor_cores(void) { return 1; }
 namespace {
 
 constexpr int BK = 32;                      // channels per k-block (64-byte rows, SWIZZLE_64B)
-constexpr int NSTAGE = 4;
-constexpr int BN = 128;                     // output channels per CTA
-constexpr int TILE_BYTES = 256 * BK * 2;    // one 256-row x 32-col bf16 A tile = 16 KB
-constexpr int WTILE_BYTES = BN * BK * 2;    // one 128-row weight tile = 8 KB
-constexpr int STAGE_BYTES = 2 * TILE_BYTES + 2 * WTILE_BYTES; // A_hi, A_lo, B_hi, B_lo = 48 KB
-constexpr int TC_THREADS = 320;             // 10 warps
-constexpr int SMEM_BYTES = NSTAGE * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-// half-image variant (k_conv_tc_h): M = 128 pixels per CTA, 256 TMEM columns, 3 x 32 KB stages -> two CTAs per SM
-constexpr int H_TILE_BYTES = 128 * BK * 2;  // 8 KB
-constexpr int H_STAGE_BYTES = 2 * H_TILE_BYTES + 2 * WTILE_BYTES;   // 32 KB
-constexpr int H_NSTAGE = 3;
-constexpr int H_SMEM_BYTES = H_NSTAGE * H_STAGE_BYTES + 1024 + 256;
+constexpr int MT = 128;                     // pixels per tile: two warpgroups x 64
+constexpr int BN = 128;                     // output channels per tile of the W->W convs and in-convs
+constexpr int HD_N = 32;                    // output channels of the heads (n_mu + n_sc <= 32, zero padded)
+constexpr int A_BYTES = MT * BK * 2;        // one 128-row x 32-col bf16 activation tile = 8 KB
+constexpr int WG_THREADS = 288;             // two consumer warpgroups + one producer warp
+constexpr int PRODUCER_WARP = 8;
+
+template <int N> struct TileCfg {
+    static constexpr int W_BYTES = N * BK * 2;                       // one N-row weight tile
+    static constexpr int STAGE = 2 * A_BYTES + 2 * W_BYTES;          // A_hi, A_lo, B_hi, B_lo
+    static constexpr int NSTAGE = 6;                                 // 192 KB (N = 128) / 120 KB (N = 32) of stages
+    static constexpr int SMEM = NSTAGE * STAGE + 1024 /*align*/ + 256 /*barriers*/;
+};
+static_assert(TileCfg<BN>::SMEM <= 227 * 1024, "stages must fit one H100 SM's shared memory");
 
 struct TcState {
     // bf16 hi/lo activation planes, ping-pong: [max_batch, 256 px, 256 ch]
     __nv_bfloat16 *act[2][2];
-    CUtensorMap act_map[2][2];
-    CUtensorMap act_map_h[2][2];   // same planes, box = 8 image rows (k_conv_tc_h)
+    CUtensorMap act_map[2][2];     // box = 8 image rows (one tile's 128 pixels)
     // in-conv input: the flat `given` re-laid as NHWC bf16 hi/lo planes with the (1..12) input channels padded to 32
     __nv_bfloat16 *inp[2];
     CUtensorMap inp_map[2];
-    CUtensorMap inp_map_h[2];
     std::vector<void *> wbufs;
 };
 
@@ -65,6 +67,9 @@ __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(uint64_t *bar, uint32_t parity) {
     uint32_t ok;
@@ -99,55 +104,71 @@ __device__ __forceinline__ void tma_load_3d(void *dst, const CUtensorMap *map, u
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                  ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// K-major, SWIZZLE_64B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
+// K-major, SWIZZLE_64B wgmma shared-memory matrix descriptor:
 //   [0,14) start address >> 4 | [16,30) LBO >> 4 (unused for swizzled K-major, 1) | [32,46) SBO >> 4 = 512 B
-//   (8 rows x 64 B) | [46,48) version = 1 | [61,64) layout type 4 = SWIZZLE_64B
+//   (8 rows x 64 B) | [62,64) layout type 2 = SWIZZLE_64B.  The k16 slices of a 64-byte row start 32 B apart.
 __device__ __forceinline__ uint64_t make_desc_sw64(uint32_t saddr) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3fff);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)(512 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)4 << 61;
+    d |= (uint64_t)2 << 62;
     return d;
 }
-// kind::f16 instruction descriptor: D=F32 (bits 4-5 = 1), A=B=BF16 (bits 7-9, 10-12 = 1), K-major both,
-// N>>3 at [17,23), M>>4 at [24,29)
-constexpr uint32_t IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((128u >> 4) << 24);
 
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(IDESC), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, bf16 operands from shared memory, float32 accumulators in registers.
+// Accumulator layout (per warpgroup thread, warp w, lane l): d[4j + 2h + e] = D[16w + l/4 + 8h][8j + 2(l%4) + e].
+template <int N> struct Wgmma;
+template <> struct Wgmma<128> {
+    static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) {
+        asm volatile(
+            "{\n"
+            ".reg .pred p;\n"
+            "setp.ne.b32 p, %66, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+            "%64, %65, p, 1, 1, 0, 0;\n"
+            "}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "l"(da), "l"(db), "r"(1));
+    }
+};
+template <> struct Wgmma<32> {
+    static __device__ __forceinline__ void mma(float (&d)[16], uint64_t da, uint64_t db) {
+        asm volatile(
+            "{\n"
+            ".reg .pred p;\n"
+            "setp.ne.b32 p, %18, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+            "%16, %17, p, 1, 1, 0, 0;\n"
+            "}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(da), "l"(db), "r"(1));
+    }
+};
+
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int K> __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(K) : "memory"); }
+// The accumulators are written asynchronously: pin every read of them after the wait that retires the writes.
+template <int R> __device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 // ELU(x) = x > 0 ? x : exp(x) - 1 (utils/torch/modules.py:229-241 F.elu).  exp by the hardware ex2 (2 ulp of the result,
 // |error| <= 2.4e-7 absolute after the subtraction): far inside the 1e-4 bar on mu/sigma (measured in the P3 tests) and
-// a third of expm1f's instructions -- the epilogue's ALU work, not its bytes, is what the convs wait for.
+// a third of expm1f's instructions.
 __device__ __forceinline__ float elu1(float x) { return x > 0.f ? x : __expf(x) - 1.0f; }
 
+__device__ __forceinline__ uint32_t pack_bf16x2(__nv_bfloat16 a, __nv_bfloat16 b) {
+    return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
+}
+
 struct TcArgs {
+    static constexpr int kN = BN, kCoBlocks = 256 / BN;
     int taps, ks;
     int cchunks;             // 32-channel chunks per tap: 8 for the dense W->W convs, 1 for the in-convs
     const float *bias;       // [256]
@@ -158,760 +179,53 @@ struct TcArgs {
     int A_elu;
 };
 
-__device__ __forceinline__ void conv_tc_body(const CUtensorMap &amap_hi, const CUtensorMap &amap_lo, const CUtensorMap &wmap_hi,
-                                             const CUtensorMap &wmap_lo, const TcArgs &a) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t *full_bar = (uint64_t *)(smem + NSTAGE * STAGE_BYTES);
-    uint64_t *empty_bar = full_bar + NSTAGE;
-    uint64_t *acc_bar = empty_bar + NSTAGE;
-    uint32_t *tmem_ptr = (uint32_t *)(acc_bar + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int img = blockIdx.x, co0 = blockIdx.y * BN;
-    const int nkb = a.taps * a.cchunks;
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&amap_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&amap_lo) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap_lo) : "memory");
-        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(acc_bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {     // TMEM: all 512 columns (2 accumulators of 256 fp32 columns)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_ptr)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-
-    if (warp == 0) {
-        // ===== TMA producer =====
-        if (lane == 0) {
-            const int r = a.ks / 2;
-            int stage = 0, phase = 0;
-            for (int kb = 0; kb < nkb; ++kb) {
-                int tap = kb / a.cchunks, c0 = (kb - tap * a.cchunks) * BK;
-                int dy = tap / a.ks, dx = tap - dy * a.ks;
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                uint8_t *st = smem + stage * STAGE_BYTES;
-                mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
-                tma_load_4d(st, &amap_hi, &full_bar[stage], c0, dx - r, dy - r, img);
-                tma_load_4d(st + TILE_BYTES, &amap_lo, &full_bar[stage], c0, dx - r, dy - r, img);
-                tma_load_3d(st + 2 * TILE_BYTES, &wmap_hi, &full_bar[stage], c0, co0, tap);
-                tma_load_3d(st + 2 * TILE_BYTES + WTILE_BYTES, &wmap_lo, &full_bar[stage], c0, co0, tap);
-                if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        if (lane == 0) {
-            int stage = 0, phase = 0;
-            for (int kb = 0; kb < nkb; ++kb) {
-                mbar_wait(&full_bar[stage], phase);
-                tc_fence_after();
-                uint32_t sbase = smem_u32(smem + stage * STAGE_BYTES);
+// Dense / in-conv epilogue from the accumulators: (main + cross) + bias (+ residual) (-> ELU) -> trunk; (-> ELU) -> bf16
+// hi/lo planes of the next conv.  A quad of lanes covers 8 consecutive channels (32 B of the trunk row): every store
+// instruction writes whole sectors.  The residual is the trunk itself (updated in place: resid == T), so its loads are
+// issued explicitly four column groups ahead of the stores that could alias them.  A thread re-reads nothing it has
+// written, so the in-place update stays exact.
+__device__ __forceinline__ void epilogue(const TcArgs &a, const float (&dm)[64], const float (&dc)[64], int img, int prow0,
+                                         int co0, int lane) {
+    const int cl = 2 * (lane & 3);
+    const int64_t base = ((int64_t)img * 256 + prow0) * 256 + co0 + cl;     // + 8h * 256 + 8j
 #pragma unroll
-                for (int kk = 0; kk < BK / 16; ++kk) {
+    for (int jb = 0; jb < 16; jb += 4) {
+        float2 q[4][2];
 #pragma unroll
-                    for (int half = 0; half < 2; ++half) {
-                        uint32_t aoff = half * (128 * BK * 2) + kk * 32;           // 128 rows x 64 B ; +32 B per UMMA_K
-                        uint64_t a_hi = make_desc_sw64(sbase + aoff);
-                        uint64_t a_lo = make_desc_sw64(sbase + TILE_BYTES + aoff);
-                        uint64_t b_hi = make_desc_sw64(sbase + 2 * TILE_BYTES + kk * 32);
-                        uint64_t b_lo = make_desc_sw64(sbase + 2 * TILE_BYTES + WTILE_BYTES + kk * 32);
-                        uint32_t d_main = tmem_base + half * BN, d_cross = tmem_base + 256 + half * BN;
-                        umma_bf16(d_main, a_hi, b_hi, (kb | kk) != 0);
-                        umma_bf16(d_cross, a_lo, b_hi, (kb | kk) != 0);
-                        umma_bf16(d_cross, a_hi, b_lo, 1);
-                    }
-                }
-                umma_commit(&empty_bar[stage]);
-                if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
-            }
-            umma_commit(acc_bar);                        // accumulators complete
-        }
-    } else {
-        // ===== epilogue: 8 warps; warp w reads TMEM lanes 32*(w%4).., columns of accumulator (w-2)/4 =====
-        // Coalesced through shared memory (see k_conv_tc_h): once acc_bar has fired every pipeline stage is idle, so each
-        // warp transposes its 32 px x 32 ch chunks through a private padded tile in the stage memory and moves whole
-        // 128-byte lines (tcgen05.ld hands a lane one pixel's 32 channels: written directly that is 32 scattered 16-byte
-        // pieces per store instruction).  Same arithmetic, same order -> same bits as the direct epilogue.
-        const int ew = warp - 2;
-        const int half = ew >> 2;
-        const int quad = warp & 3;                       // TMEM lane quadrant this warp may access
-        float *tile = reinterpret_cast<float *>(smem) + ew * (32 * 36);          // 32 rows x 36 floats (144 B stride)
-        const int rsub = lane >> 3, col4 = (lane & 7) * 4;
-        const int64_t pbase = ((int64_t)img * 256 + half * 128 + quad * 32 + rsub) * 256 + co0 + col4;   // + (4 k) * 256 + cc
-        // The residual is the trunk itself (updated in place: resid == T), so the compiler may not move its loads above the
-        // stores of an earlier row -- left alone, every row's HBM latency is paid in series (ncu: the conv2 launches ran
-        // 0.98 ms against 0.75 ms for conv1, long_scoreboard on the residual loads).  The loads are therefore issued
-        // explicitly one 32-channel chunk ahead: chunk 0's before the accumulator is even ready (they do not depend on
-        // it), chunk c+1's before chunk c's arithmetic and stores.  A thread re-reads nothing it has written (chunks are
-        // disjoint channel ranges of its own rows), so the in-place update stays exact.
-        float4 q[8], qn[8];
-        auto load_resid = [&](float4 (&dst)[8], int cc) {
+        for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
-            for (int k = 0; k < 8; ++k)
-                dst[k] = a.resid ? *reinterpret_cast<const float4 *>(a.resid + pbase + (int64_t)(4 * k) * 256 + cc) : make_float4(0.f, 0.f, 0.f, 0.f);
-        };
-        load_resid(q, 0);
-        mbar_wait(acc_bar, 0);
-        tc_fence_after();
-#pragma unroll 1
-        for (int cc = 0; cc < BN; cc += 32) {
-            const int c0 = co0 + cc;
-            {
-                uint32_t rr[32], rc[32];
-                tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + half * BN + cc, rr);
-                tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + 256 + half * BN + cc, rc);
-                float4 *trow = reinterpret_cast<float4 *>(tile + lane * 36);
+            for (int h = 0; h < 2; ++h)
+                q[jj][h] = a.resid ? *reinterpret_cast<const float2 *>(a.resid + base + h * 8 * 256 + 8 * (jb + jj)) : make_float2(0.f, 0.f);
 #pragma unroll
-                for (int i = 0; i < 8; ++i)
-                    trow[i] = make_float4(__uint_as_float(rr[4 * i]) + __uint_as_float(rc[4 * i]),
-                                          __uint_as_float(rr[4 * i + 1]) + __uint_as_float(rc[4 * i + 1]),
-                                          __uint_as_float(rr[4 * i + 2]) + __uint_as_float(rc[4 * i + 2]),
-                                          __uint_as_float(rr[4 * i + 3]) + __uint_as_float(rc[4 * i + 3]));
-            }
-            __syncwarp();
-            if (cc + 32 < BN) load_resid(qn, cc + 32);
-            const float4 bq = __ldg(reinterpret_cast<const float4 *>(a.bias + c0 + col4));
+        for (int jj = 0; jj < 4; ++jj) {
+            const int j = jb + jj;
+            const float2 bq = __ldg(reinterpret_cast<const float2 *>(a.bias + co0 + cl + 8 * j));
 #pragma unroll
-            for (int k = 0; k < 8; ++k) {
-                const int r = 4 * k + rsub;
-                const int64_t prow = pbase + (int64_t)(4 * k) * 256 + cc;
-                float4 x = *reinterpret_cast<const float4 *>(tile + r * 36 + col4);
-                x.x += bq.x; x.y += bq.y; x.z += bq.z; x.w += bq.w;      // (main+cross)+bias
-                if (a.resid) { x.x += q[k].x; x.y += q[k].y; x.z += q[k].z; x.w += q[k].w; }
-                if (a.T_elu) { x.x = elu1(x.x); x.y = elu1(x.y); x.z = elu1(x.z); x.w = elu1(x.w); }
-                if (a.T) *reinterpret_cast<float4 *>(a.T + prow) = x;
+            for (int h = 0; h < 2; ++h) {
+                const int i = 4 * j + 2 * h;
+                const int64_t off = base + h * 8 * 256 + 8 * j;
+                float x0 = (dm[i] + dc[i]) + bq.x, x1 = (dm[i + 1] + dc[i + 1]) + bq.y;
+                if (a.resid) { x0 += q[jj][h].x; x1 += q[jj][h].y; }
+                if (a.T_elu) { x0 = elu1(x0); x1 = elu1(x1); }
+                if (a.T) *reinterpret_cast<float2 *>(a.T + off) = make_float2(x0, x1);
                 if (a.A_hi) {
-                    float y[4] = {x.x, x.y, x.z, x.w};
-                    uint32_t hi[2], lo[2];
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        float x0 = a.A_elu ? elu1(y[2 * i]) : y[2 * i], x1 = a.A_elu ? elu1(y[2 * i + 1]) : y[2 * i + 1];
-                        __nv_bfloat16 h0 = __float2bfloat16_rn(x0), h1 = __float2bfloat16_rn(x1);
-                        __nv_bfloat16 l0 = __float2bfloat16_rn(x0 - __bfloat162float(h0)), l1 = __float2bfloat16_rn(x1 - __bfloat162float(h1));
-                        hi[i] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-                        lo[i] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-                    }
-                    *reinterpret_cast<uint2 *>(a.A_hi + prow) = make_uint2(hi[0], hi[1]);
-                    *reinterpret_cast<uint2 *>(a.A_lo + prow) = make_uint2(lo[0], lo[1]);
-                }
-            }
-#pragma unroll
-            for (int k = 0; k < 8; ++k) q[k] = qn[k];
-            __syncwarp();                                 // the tile is rewritten by the next chunk
-        }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        __syncwarp();
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
-    }
-}
-
-// One CTA per SM (shared memory); ~150 registers per thread for the epilogue's two residual chunks in flight.  That leaves
-// 17 K registers per SM: room for the serial coder CTAs of another lane (11 K), not for a 32 K-register table CTA -- by
-// measurement nothing is lost: the convs run at the board's power cap, so FP64 work beside them only lowers the clock
-// (DESIGN.md 5.3).
-__global__ void __launch_bounds__(TC_THREADS, 1)
-k_conv_tc(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ CUtensorMap amap_lo,
-          const __grid_constant__ CUtensorMap wmap_hi, const __grid_constant__ CUtensorMap wmap_lo, TcArgs a) {
-    conv_tc_body(amap_hi, amap_lo, wmap_hi, wmap_lo, a);
-}
-// Half-image variant: the default for the in-convs (0.555 -> 0.416 ms per launch at B=1024), optional for the dense convs.
-// k_conv_tc above owns the SM (192 KB of stages, all 512 TMEM columns), so the tensor
-// pipe idles while its eight epilogue warps drain the accumulators to HBM -- about half of a 3x3 launch and nearly all
-// of an in-conv launch (13.8 waves x ~40 us per CTA with nine k-blocks of work).  Here a CTA owns 128 pixels (8 image
-// rows) x 128 output channels: {main, cross} x 128 columns = 256 TMEM columns and 3 x 32 KB stages, so TWO CTAs are
-// resident per SM and one's epilogue runs under the other's MMAs.  Price: the weight tile is fetched per half image
-// (L2->SM bytes per k-block and MMA row 48 KB/256 rows -> 32 KB/128 rows); the order of the k-blocks and of the MMAs
-// into each accumulator is unchanged, so results are bit-identical to the full-tile kernel.
-__global__ void __launch_bounds__(TC_THREADS, 2)
-k_conv_tc_h(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ CUtensorMap amap_lo,
-            const __grid_constant__ CUtensorMap wmap_hi, const __grid_constant__ CUtensorMap wmap_lo, TcArgs a) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t *full_bar = (uint64_t *)(smem + H_NSTAGE * H_STAGE_BYTES);
-    uint64_t *empty_bar = full_bar + H_NSTAGE;
-    uint64_t *acc_bar = empty_bar + H_NSTAGE;
-    uint32_t *tmem_ptr = (uint32_t *)(acc_bar + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int img = blockIdx.x, co0 = blockIdx.y * BN, mh = blockIdx.z;
-    const int nkb = a.taps * a.cchunks;
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&amap_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&amap_lo) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap_lo) : "memory");
-        for (int s = 0; s < H_NSTAGE; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(acc_bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {     // TMEM: 256 columns = main [0,128) + cross [128,256); the co-resident CTA takes the other 256
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" ::"r"(smem_u32(tmem_ptr)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-
-    if (warp == 0) {
-        if (lane == 0) {     // ===== TMA producer =====
-            const int r = a.ks / 2;
-            int stage = 0, phase = 0;
-            for (int kb = 0; kb < nkb; ++kb) {
-                int tap = kb / a.cchunks, c0 = (kb - tap * a.cchunks) * BK;
-                int dy = tap / a.ks, dx = tap - dy * a.ks;
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                uint8_t *st = smem + stage * H_STAGE_BYTES;
-                mbar_expect_tx(&full_bar[stage], H_STAGE_BYTES);
-                tma_load_4d(st, &amap_hi, &full_bar[stage], c0, dx - r, dy - r + 8 * mh, img);
-                tma_load_4d(st + H_TILE_BYTES, &amap_lo, &full_bar[stage], c0, dx - r, dy - r + 8 * mh, img);
-                tma_load_3d(st + 2 * H_TILE_BYTES, &wmap_hi, &full_bar[stage], c0, co0, tap);
-                tma_load_3d(st + 2 * H_TILE_BYTES + WTILE_BYTES, &wmap_lo, &full_bar[stage], c0, co0, tap);
-                if (++stage == H_NSTAGE) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {     // ===== MMA issuer =====
-            int stage = 0, phase = 0;
-            const uint32_t d_main = tmem_base, d_cross = tmem_base + BN;
-            for (int kb = 0; kb < nkb; ++kb) {
-                mbar_wait(&full_bar[stage], phase);
-                tc_fence_after();
-                uint32_t sbase = smem_u32(smem + stage * H_STAGE_BYTES);
-#pragma unroll
-                for (int kk = 0; kk < BK / 16; ++kk) {
-                    uint64_t a_hi = make_desc_sw64(sbase + kk * 32);
-                    uint64_t a_lo = make_desc_sw64(sbase + H_TILE_BYTES + kk * 32);
-                    uint64_t b_hi = make_desc_sw64(sbase + 2 * H_TILE_BYTES + kk * 32);
-                    uint64_t b_lo = make_desc_sw64(sbase + 2 * H_TILE_BYTES + WTILE_BYTES + kk * 32);
-                    umma_bf16(d_main, a_hi, b_hi, (kb | kk) != 0);
-                    umma_bf16(d_cross, a_lo, b_hi, (kb | kk) != 0);
-                    umma_bf16(d_cross, a_hi, b_lo, 1);
-                }
-                umma_commit(&empty_bar[stage]);
-                if (++stage == H_NSTAGE) { stage = 0; phase ^= 1; }
-            }
-            umma_commit(acc_bar);
-        }
-    } else {
-        // ===== epilogue: warp w may read TMEM lanes 32*(w%4)..; the two warps of a quadrant split the 128 columns =====
-        const int ew = warp - 2;
-        const int chalf = ew >> 2;
-        const int quad = warp & 3;
-        mbar_wait(acc_bar, 0);
-        tc_fence_after();
-        // Coalesced epilogue.  tcgen05.ld hands every lane one pixel's 32 consecutive channels; written straight to
-        // HBM that is 32 scattered 16-byte pieces per store instruction (the LSU, not HBM, bounds the direct epilogue:
-        // ncu shows lg_throttle on every STG).  Instead the warp transposes each 32 px x 32 ch chunk through a private
-        // padded tile in the (now idle) pipeline stages, so that 8 consecutive lanes hold 128 contiguous bytes of one
-        // pixel row: residual loads, trunk stores and plane stores become 4 full lines per instruction.
-        float *tile = reinterpret_cast<float *>(smem) + ew * (32 * 36);          // 32 rows x 36 floats (144 B stride)
-        const int rsub = lane >> 3, col4 = (lane & 7) * 4;
-#pragma unroll 1
-        for (int cc = chalf * 64; cc < chalf * 64 + 64; cc += 32) {
-            const int c0 = co0 + cc;
-            {
-                uint32_t rr[32], rc[32];
-                tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + cc, rr);
-                tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + BN + cc, rc);
-                float4 *trow = reinterpret_cast<float4 *>(tile + lane * 36);
-#pragma unroll
-                for (int i = 0; i < 8; ++i)
-                    trow[i] = make_float4(__uint_as_float(rr[4 * i]) + __uint_as_float(rc[4 * i]),
-                                          __uint_as_float(rr[4 * i + 1]) + __uint_as_float(rc[4 * i + 1]),
-                                          __uint_as_float(rr[4 * i + 2]) + __uint_as_float(rc[4 * i + 2]),
-                                          __uint_as_float(rr[4 * i + 3]) + __uint_as_float(rc[4 * i + 3]));
-            }
-            __syncwarp();
-            const float4 bq = __ldg(reinterpret_cast<const float4 *>(a.bias + c0 + col4));
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-                const int r = 4 * k + rsub;
-                const int64_t prow = ((int64_t)img * 256 + mh * 128 + quad * 32 + r) * 256 + c0 + col4;
-                float4 x = *reinterpret_cast<const float4 *>(tile + r * 36 + col4);
-                x.x += bq.x; x.y += bq.y; x.z += bq.z; x.w += bq.w;      // same order as the direct path: (main+cross)+bias
-                if (a.resid) {
-                    const float4 q = *reinterpret_cast<const float4 *>(a.resid + prow);
-                    x.x += q.x; x.y += q.y; x.z += q.z; x.w += q.w;
-                }
-                if (a.T_elu) { x.x = elu1(x.x); x.y = elu1(x.y); x.z = elu1(x.z); x.w = elu1(x.w); }
-                if (a.T) *reinterpret_cast<float4 *>(a.T + prow) = x;
-                if (a.A_hi) {
-                    float y[4] = {x.x, x.y, x.z, x.w};
-                    uint32_t hi[2], lo[2];
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        float x0 = a.A_elu ? elu1(y[2 * i]) : y[2 * i], x1 = a.A_elu ? elu1(y[2 * i + 1]) : y[2 * i + 1];
-                        __nv_bfloat16 h0 = __float2bfloat16_rn(x0), h1 = __float2bfloat16_rn(x1);
-                        __nv_bfloat16 l0 = __float2bfloat16_rn(x0 - __bfloat162float(h0)), l1 = __float2bfloat16_rn(x1 - __bfloat162float(h1));
-                        hi[i] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-                        lo[i] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-                    }
-                    *reinterpret_cast<uint2 *>(a.A_hi + prow) = make_uint2(hi[0], hi[1]);
-                    *reinterpret_cast<uint2 *>(a.A_lo + prow) = make_uint2(lo[0], lo[1]);
-                }
-            }
-            __syncwarp();                             // the tile is rewritten by the next chunk
-        }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        __syncwarp();
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" ::"r"(tmem_base) : "memory");
-    }
-}
-
-// Persistent variant: ONE CTA per SM walks half-image tiles (128 pixels x 128 output channels) of the whole batch.
-//   * TMEM ping-pong: tile i accumulates into columns [256*(i&1), +256) (main 128 + cross 128) while the eight epilogue
-//     warps drain tile i-1 from the other 256 -- the epilogue (a third of k_conv_tc's CTA life on the 3x3 convs, nearly
-//     all of it on the in-convs) disappears under the next tile's MMAs, and the TMA ring keeps prefetching across tile
-//     boundaries, so the per-CTA start-up latency (allocation, tensormap fetch, first TMA round trip) is paid once per SM
-//     instead of once per tile.
-//   * Because the grid is at most one CTA per SM and every CTA is resident from the start, the block scheduler is free
-//     to place other streams' kernels (the FP64-bound coder kernels of another lane: 32 K registers, no shared memory)
-//     on the same SMs while the convolution runs -- with per-tile grids the queue of conv CTAs keeps them out.
-//   * k-block order, MMA order per accumulator and the epilogue arithmetic are those of k_conv_tc / k_conv_tc_h: results
-//     are bit-identical to both.
-constexpr int P_NSTAGE = 5;
-constexpr int P_SCRATCH = 8 * 32 * 36 * 4;   // one 32 x 36 float transposition tile per epilogue warp
-constexpr int P_SMEM_BYTES = P_NSTAGE * H_STAGE_BYTES + P_SCRATCH + 1024 + 256;
-
-// (min-blocks 2 only caps the registers at 96 per thread so that a 32 K-register coder CTA fits beside this one)
-__global__ void __launch_bounds__(TC_THREADS, 2)
-k_conv_tc_p(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ CUtensorMap amap_lo,
-            const __grid_constant__ CUtensorMap wmap_hi, const __grid_constant__ CUtensorMap wmap_lo, TcArgs a, int ntiles) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    float *scratch = reinterpret_cast<float *>(smem + P_NSTAGE * H_STAGE_BYTES);
-    uint64_t *full_bar = (uint64_t *)(smem + P_NSTAGE * H_STAGE_BYTES + P_SCRATCH);
-    uint64_t *empty_bar = full_bar + P_NSTAGE;
-    uint64_t *accf_bar = empty_bar + P_NSTAGE;           // [2] accumulator buffer complete (MMA -> epilogue)
-    uint64_t *acce_bar = accf_bar + 2;                   // [2] accumulator buffer drained  (epilogue -> MMA)
-    uint32_t *tmem_ptr = (uint32_t *)(acce_bar + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int nkb = a.taps * a.cchunks;
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&amap_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&amap_lo) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap_lo) : "memory");
-        for (int s = 0; s < P_NSTAGE; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&accf_bar[b], 1); mbar_init(&acce_bar[b], 8); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {     // all 512 TMEM columns: two {main, cross} accumulator pairs
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_ptr)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-
-    // tile t -> image t>>2, output-channel half (t>>1)&1, pixel half t&1: the four tiles of an image run on neighbouring
-    // SMs at about the same time, so the activation planes they share come out of L2.
-    if (warp == 0) {
-        if (lane == 0) {     // ===== TMA producer =====
-            const int r = a.ks / 2;
-            int stage = 0, phase = 0;
-            for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
-                const int img = t >> 2, co0 = ((t >> 1) & 1) * BN, mh = t & 1;
-                for (int kb = 0; kb < nkb; ++kb) {
-                    int tap = kb / a.cchunks, c0 = (kb - tap * a.cchunks) * BK;
-                    int dy = tap / a.ks, dx = tap - dy * a.ks;
-                    mbar_wait(&empty_bar[stage], phase ^ 1);
-                    uint8_t *st = smem + stage * H_STAGE_BYTES;
-                    mbar_expect_tx(&full_bar[stage], H_STAGE_BYTES);
-                    tma_load_4d(st, &amap_hi, &full_bar[stage], c0, dx - r, dy - r + 8 * mh, img);
-                    tma_load_4d(st + H_TILE_BYTES, &amap_lo, &full_bar[stage], c0, dx - r, dy - r + 8 * mh, img);
-                    tma_load_3d(st + 2 * H_TILE_BYTES, &wmap_hi, &full_bar[stage], c0, co0, tap);
-                    tma_load_3d(st + 2 * H_TILE_BYTES + WTILE_BYTES, &wmap_lo, &full_bar[stage], c0, co0, tap);
-                    if (++stage == P_NSTAGE) { stage = 0; phase ^= 1; }
+                    const float y0 = a.A_elu ? elu1(x0) : x0, y1 = a.A_elu ? elu1(x1) : x1;
+                    const __nv_bfloat16 h0 = __float2bfloat16_rn(y0), h1 = __float2bfloat16_rn(y1);
+                    const __nv_bfloat16 l0 = __float2bfloat16_rn(y0 - __bfloat162float(h0)), l1 = __float2bfloat16_rn(y1 - __bfloat162float(h1));
+                    *reinterpret_cast<uint32_t *>(a.A_hi + off) = pack_bf16x2(h0, h1);
+                    *reinterpret_cast<uint32_t *>(a.A_lo + off) = pack_bf16x2(l0, l1);
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {     // ===== MMA issuer =====
-            int stage = 0, phase = 0, it = 0;
-            for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++it) {
-                const int buf = it & 1;
-                mbar_wait(&acce_bar[buf], ((it >> 1) & 1) ^ 1);      // the epilogue has drained this buffer (first use: passes)
-                tc_fence_after();
-                const uint32_t d_main = tmem_base + buf * 256, d_cross = d_main + BN;
-                for (int kb = 0; kb < nkb; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    uint32_t sbase = smem_u32(smem + stage * H_STAGE_BYTES);
-#pragma unroll
-                    for (int kk = 0; kk < BK / 16; ++kk) {
-                        uint64_t a_hi = make_desc_sw64(sbase + kk * 32);
-                        uint64_t a_lo = make_desc_sw64(sbase + H_TILE_BYTES + kk * 32);
-                        uint64_t b_hi = make_desc_sw64(sbase + 2 * H_TILE_BYTES + kk * 32);
-                        uint64_t b_lo = make_desc_sw64(sbase + 2 * H_TILE_BYTES + WTILE_BYTES + kk * 32);
-                        umma_bf16(d_main, a_hi, b_hi, (kb | kk) != 0);
-                        umma_bf16(d_cross, a_lo, b_hi, (kb | kk) != 0);
-                        umma_bf16(d_cross, a_hi, b_lo, 1);
-                    }
-                    umma_commit(&empty_bar[stage]);
-                    if (++stage == P_NSTAGE) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(&accf_bar[buf]);
-            }
-        }
-    } else {
-        // ===== epilogue (the coalesced one of k_conv_tc_h): warp w may read TMEM lanes 32*(w%4)..; the two warps of a
-        // quadrant split the 128 columns =====
-        const int ew = warp - 2;
-        const int chalf = ew >> 2;
-        const int quad = warp & 3;
-        float *tile = scratch + ew * (32 * 36);
-        const int rsub = lane >> 3, col4 = (lane & 7) * 4;
-        int it = 0;
-        for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++it) {
-            const int img = t >> 2, co0 = ((t >> 1) & 1) * BN, mh = t & 1;
-            const int buf = it & 1;
-            mbar_wait(&accf_bar[buf], (it >> 1) & 1);
-            tc_fence_after();
-            const uint32_t tb = tmem_base + buf * 256 + ((uint32_t)(quad * 32) << 16);
-#pragma unroll 1
-            for (int cc = chalf * 64; cc < chalf * 64 + 64; cc += 32) {
-                const int c0 = co0 + cc;
-                {
-                    uint32_t rr[32], rc[32];
-                    tmem_ld32(tb + cc, rr);
-                    tmem_ld32(tb + BN + cc, rc);
-                    if (cc == chalf * 64 + 32) {          // my last TMEM read of this tile: hand the buffer back to the MMA warp
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&acce_bar[buf])) : "memory");
-                    }
-                    float4 *trow = reinterpret_cast<float4 *>(tile + lane * 36);
-#pragma unroll
-                    for (int i = 0; i < 8; ++i)
-                        trow[i] = make_float4(__uint_as_float(rr[4 * i]) + __uint_as_float(rc[4 * i]),
-                                              __uint_as_float(rr[4 * i + 1]) + __uint_as_float(rc[4 * i + 1]),
-                                              __uint_as_float(rr[4 * i + 2]) + __uint_as_float(rc[4 * i + 2]),
-                                              __uint_as_float(rr[4 * i + 3]) + __uint_as_float(rc[4 * i + 3]));
-                }
-                __syncwarp();
-                const float4 bq = __ldg(reinterpret_cast<const float4 *>(a.bias + c0 + col4));
-#pragma unroll
-                for (int k = 0; k < 8; ++k) {
-                    const int r = 4 * k + rsub;
-                    const int64_t prow = ((int64_t)img * 256 + mh * 128 + quad * 32 + r) * 256 + c0 + col4;
-                    float4 x = *reinterpret_cast<const float4 *>(tile + r * 36 + col4);
-                    x.x += bq.x; x.y += bq.y; x.z += bq.z; x.w += bq.w;      // same order as the direct path: (main+cross)+bias
-                    if (a.resid) {
-                        const float4 q = *reinterpret_cast<const float4 *>(a.resid + prow);
-                        x.x += q.x; x.y += q.y; x.z += q.z; x.w += q.w;
-                    }
-                    if (a.T_elu) { x.x = elu1(x.x); x.y = elu1(x.y); x.z = elu1(x.z); x.w = elu1(x.w); }
-                    if (a.T) *reinterpret_cast<float4 *>(a.T + prow) = x;
-                    if (a.A_hi) {
-                        float y[4] = {x.x, x.y, x.z, x.w};
-                        uint32_t hi[2], lo[2];
-#pragma unroll
-                        for (int i = 0; i < 2; ++i) {
-                            float x0 = a.A_elu ? elu1(y[2 * i]) : y[2 * i], x1 = a.A_elu ? elu1(y[2 * i + 1]) : y[2 * i + 1];
-                            __nv_bfloat16 h0 = __float2bfloat16_rn(x0), h1 = __float2bfloat16_rn(x1);
-                            __nv_bfloat16 l0 = __float2bfloat16_rn(x0 - __bfloat162float(h0)), l1 = __float2bfloat16_rn(x1 - __bfloat162float(h1));
-                            hi[i] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-                            lo[i] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-                        }
-                        *reinterpret_cast<uint2 *>(a.A_hi + prow) = make_uint2(hi[0], hi[1]);
-                        *reinterpret_cast<uint2 *>(a.A_lo + prow) = make_uint2(lo[0], lo[1]);
-                    }
-                }
-                __syncwarp();                             // the tile is rewritten by the next chunk
-            }
-        }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        __syncwarp();
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
     }
 }
 
-// Pair-tile variant: a 2-CTA cluster (one SM pair) owns one IMAGE and issues cta_group::2 MMAs with M = 256, N = 256.
-//   * Why: the convs are bound by L2 -> SM delivery, ~6300 B/clk chip-wide = 42.6 B/clk/SM (B300_MICROARCH.md, "LTS
-//     throughput cap", the same for TMA and LDG).  k_conv_tc fills 48 KB per k-block of twelve 64-cycle MMAs: 48 KB / 42.6 =
-//     1154 cycles against a tensor floor of 768 -- measured 1170.  The half-image tiles fill 32 KB per six MMAs: 769 against
-//     384 -- measured 768.  With N = 256 the activation tile is fetched once per 256 output channels, and with cta_group::2
-//     the weight tile is SPLIT across the pair (128 of its 256 rows each): 32 KB per CTA and k-block of six 128-cycle MMAs
-//     = 769 cycles of L2 against 768 of tensor pipe -- balanced; measured 855 (38 B/clk/SM, 0.90 of either bound).
-//   * CTA r holds image rows 8r..8r+7 (its 128 pixels) of the A tile and weight rows 128r..128r+127 of the B tile; its
-//     accumulators are 128 lanes x {main, cross} x 256 columns = all 512 TMEM columns: no ping-pong, so the epilogue
-//     first empties TMEM into shared memory and registers, hands it back, and does its global traffic under the next tile.
-//   * Leader (cluster rank 0) issues the MMAs and owns the `full` barriers (both CTAs' TMA loads signal them:
-//     cp.async.bulk.tensor ... cta_group::2 with the barrier address' peer bit cleared); tcgen05.commit multicasts to both CTAs'
-//     `empty` and `accf` barriers; the epilogue warps of both CTAs arrive on the leader's `acce` barrier.
-//   * k order, MMA order per accumulator and the epilogue arithmetic are those of the other kernels: bit-identical results.
-constexpr int P2_WTILE = 128 * BK * 2;                         // my 128 of the tile's 256 weight rows: 8 KB per plane
-constexpr int P2_STAGE = 2 * H_TILE_BYTES + 2 * P2_WTILE;      // 32 KB
-constexpr int P2_NSTAGE = 4;
-constexpr int P2_NE = 8;                                       // epilogue warps per CTA: 2 per TMEM lane quadrant, 128 columns each
-constexpr int P2_SCRATCH = P2_NE * 3 * 32 * 32 * 4;            // three 32 x 32 float tiles per epilogue warp (96 KB): see the epilogue
-constexpr int P2_SMEM_BYTES = P2_NSTAGE * P2_STAGE + P2_SCRATCH + 1024 + 256;
-constexpr uint32_t IDESC_2SM = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(256 >> 3) << 17) | ((256u >> 4) << 24);   // M = 256, N = 256
-constexpr uint32_t PEER_MASK = 0xFEFFFFFFu;                    // clears the bit that tells the pair's two shared windows apart
-
-__device__ __forceinline__ uint32_t cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA loads of the pair: data into MY shared memory, completion bytes onto the LEADER's mbarrier
-__device__ __forceinline__ void tma2_load_4d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, int c2, int c3) {
-    asm volatile("cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5, %6}], [%2], %7;"
-                 ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar) & PEER_MASK), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(0x1000000000000000ull) : "memory");
-}
-__device__ __forceinline__ void tma2_load_3d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, int c2) {
-    asm volatile("cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5}], [%2], %6;"
-                 ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar) & PEER_MASK), "r"(c0), "r"(c1), "r"(c2), "l"(0x1000000000000000ull) : "memory");
-}
-__device__ __forceinline__ void umma2_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(IDESC_2SM), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma2_commit(uint64_t *bar) {       // arrives on BOTH CTAs' barrier at this offset
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t *bar) { // arrive on the leader CTA's barrier at this offset
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & PEER_MASK) : "memory");
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__((2 + P2_NE) * 32, 1)
-k_conv_tc_2sm(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ CUtensorMap amap_lo,
-              const __grid_constant__ CUtensorMap wmap_hi, const __grid_constant__ CUtensorMap wmap_lo, TcArgs a, int ntiles) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    float *scratch = reinterpret_cast<float *>(smem + P2_NSTAGE * P2_STAGE);
-    uint64_t *full_bar = (uint64_t *)(smem + P2_NSTAGE * P2_STAGE + P2_SCRATCH);
-    uint64_t *empty_bar = full_bar + P2_NSTAGE;
-    uint64_t *accf_bar = empty_bar + P2_NSTAGE;          // [2] accumulator buffer complete (leader's MMAs -> both epilogues)
-    uint64_t *acce_bar = accf_bar + 2;                   // [2] accumulator buffer drained  (both epilogues -> leader's MMA thread)
-    uint32_t *tmem_ptr = (uint32_t *)(acce_bar + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int rank = (int)cluster_rank();                // 0 = leader
-    const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-    const int nkb = a.taps * a.cchunks;
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&amap_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&amap_lo) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap_lo) : "memory");
-        for (int s = 0; s < P2_NSTAGE; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(&accf_bar[0], 1); mbar_init(&acce_bar[0], 2 * P2_NE);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {     // the pair's TMEM: 512 columns in both CTAs (same warp in both CTAs, same shared offset)
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_ptr)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    cluster_sync_all();                                  // the peer's barriers exist before anything signals them
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-
-    if (warp == 0) {
-        if (lane == 0) {     // ===== TMA producer (both CTAs): my half of A, my 64 weight rows =====
-            const int r = a.ks / 2;
-            int stage = 0, phase = 0;
-            for (int t = pair; t < ntiles; t += npairs) {
-                const int img = t;
-                for (int kb = 0; kb < nkb; ++kb) {
-                    int tap = kb / a.cchunks, c0 = (kb - tap * a.cchunks) * BK;
-                    int dy = tap / a.ks, dx = tap - dy * a.ks;
-                    mbar_wait(&empty_bar[stage], phase ^ 1);
-                    uint8_t *st = smem + stage * P2_STAGE;
-                    if (rank == 0) mbar_expect_tx(&full_bar[stage], 2 * P2_STAGE);       // both CTAs' bytes land on the leader's barrier
-                    tma2_load_4d(st, &amap_hi, &full_bar[stage], c0, dx - r, dy - r + 8 * rank, img);
-                    tma2_load_4d(st + H_TILE_BYTES, &amap_lo, &full_bar[stage], c0, dx - r, dy - r + 8 * rank, img);
-                    tma2_load_3d(st + 2 * H_TILE_BYTES, &wmap_hi, &full_bar[stage], c0, 128 * rank, tap);
-                    tma2_load_3d(st + 2 * H_TILE_BYTES + P2_WTILE, &wmap_lo, &full_bar[stage], c0, 128 * rank, tap);
-                    if (++stage == P2_NSTAGE) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0 && rank == 0) {     // ===== MMA issuer: the leader, for the pair =====
-            int stage = 0, phase = 0, it = 0;
-            for (int t = pair; t < ntiles; t += npairs, ++it) {
-                mbar_wait(&acce_bar[0], (it & 1) ^ 1);               // both CTAs' epilogues have drained the accumulators (first tile: passes)
-                tc_fence_after();
-                const uint32_t d_main = tmem_base, d_cross = tmem_base + 256;
-                for (int kb = 0; kb < nkb; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    uint32_t sbase = smem_u32(smem + stage * P2_STAGE);
-#pragma unroll
-                    for (int kk = 0; kk < BK / 16; ++kk) {
-                        uint64_t a_hi = make_desc_sw64(sbase + kk * 32);
-                        uint64_t a_lo = make_desc_sw64(sbase + H_TILE_BYTES + kk * 32);
-                        uint64_t b_hi = make_desc_sw64(sbase + 2 * H_TILE_BYTES + kk * 32);
-                        uint64_t b_lo = make_desc_sw64(sbase + 2 * H_TILE_BYTES + P2_WTILE + kk * 32);
-                        umma2_bf16(d_main, a_hi, b_hi, (kb | kk) != 0);
-                        umma2_bf16(d_cross, a_lo, b_hi, (kb | kk) != 0);
-                        umma2_bf16(d_cross, a_hi, b_lo, 1);
-                    }
-                    umma2_commit(&empty_bar[stage]);                 // frees the stage in both CTAs when these MMAs retire
-                    if (++stage == P2_NSTAGE) { stage = 0; phase ^= 1; }
-                }
-                umma2_commit(&accf_bar[0]);
-            }
-        }
-    } else {
-        // ===== epilogue (both CTAs, my 128 pixels x 256 channels) =====
-        // Phase 1 (exposed, short): main + cross summed out of TMEM -- three of my four 32-channel chunks into my shared
-        // tiles, the fourth kept in registers -- then the accumulators go back to the leader's MMA thread.
-        // Phase 2 (under the next tile's MMAs): bias, residual (loaded one chunk ahead), ELU, bf16 hi/lo split and the
-        // coalesced global stores, chunk by chunk out of shared memory; the register chunk goes through tile 0 once that is done.
-        // float4 i of row r sits at slot i ^ (r & 7) of its 128-byte row: conflict-free both ways without padding, which is
-        // what lets 96 KB of tiles sit next to four 32 KB stages.  (With the whole 128 KB output tile in shared memory only
-        // three stages fit, and the main loop slowed by more than the epilogue saved: profiles/r2_ab_runs.md.)
-        constexpr int CW = 256 / (P2_NE / 4);            // columns per warp: 128 = four chunks
-        static_assert(CW == 128, "epilogue written for four chunks per warp");
-        const int ew = warp - 2;
-        const int cpart = ew >> 2;                       // which CW of the 256 columns
-        const int quad = warp & 3;
-        float *slice = scratch + ew * (3 * 32 * 32);
-        const int rsub = lane >> 3, col4 = (lane & 7) * 4;
-        int it = 0;
-        for (int t = pair; t < ntiles; t += npairs, ++it) {
-            const int img = t;
-            const int64_t pbase = ((int64_t)img * 256 + rank * 128 + quad * 32 + rsub) * 256 + cpart * CW + col4;   // + (4 k) * 256 + cc
-            float4 q[8], qn[8];
-            float s3[32];
-            auto load_resid = [&](float4 (&dst)[8], int cc) {
-#pragma unroll
-                for (int k = 0; k < 8; ++k)
-                    dst[k] = a.resid ? *reinterpret_cast<const float4 *>(a.resid + pbase + (int64_t)(4 * k) * 256 + cc) : make_float4(0.f, 0.f, 0.f, 0.f);
-            };
-            load_resid(q, 0);
-            mbar_wait(&accf_bar[0], it & 1);
-            tc_fence_after();
-            const uint32_t tb = tmem_base + ((uint32_t)(quad * 32) << 16) + cpart * CW;
-#pragma unroll 1
-            for (int c = 0; c < 3; ++c) {
-                uint32_t rr[32], rc[32];
-                tmem_ld32(tb + c * 32, rr);
-                tmem_ld32(tb + 256 + c * 32, rc);
-                float *trow = slice + c * 1024 + lane * 32;
-#pragma unroll
-                for (int i = 0; i < 8; ++i)
-                    *reinterpret_cast<float4 *>(trow + ((i ^ (lane & 7)) << 2)) =
-                        make_float4(__uint_as_float(rr[4 * i]) + __uint_as_float(rc[4 * i]),
-                                    __uint_as_float(rr[4 * i + 1]) + __uint_as_float(rc[4 * i + 1]),
-                                    __uint_as_float(rr[4 * i + 2]) + __uint_as_float(rc[4 * i + 2]),
-                                    __uint_as_float(rr[4 * i + 3]) + __uint_as_float(rc[4 * i + 3]));
-            }
-            {
-                uint32_t rr[32], rc[32];
-                tmem_ld32(tb + 96, rr);
-                tmem_ld32(tb + 256 + 96, rc);
-#pragma unroll
-                for (int i = 0; i < 32; ++i) s3[i] = __uint_as_float(rr[i]) + __uint_as_float(rc[i]);
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_leader(&acce_bar[0]);     // the pair's next tile may start
-#pragma unroll 1
-            for (int c = 0; c < 4; ++c) {
-                const int cc = c * 32, c0 = cpart * CW + cc;
-                const float *tl = slice + (c < 3 ? c : 0) * 1024;
-                if (c == 3) {                             // the register chunk takes over tile 0 (its readers are done: same warp)
-                    __syncwarp();
-                    float *trow = slice + lane * 32;
-#pragma unroll
-                    for (int i = 0; i < 8; ++i)
-                        *reinterpret_cast<float4 *>(trow + ((i ^ (lane & 7)) << 2)) = make_float4(s3[4 * i], s3[4 * i + 1], s3[4 * i + 2], s3[4 * i + 3]);
-                    __syncwarp();
-                }
-                if (c < 3) load_resid(qn, cc + 32);
-                const float4 bq = __ldg(reinterpret_cast<const float4 *>(a.bias + c0 + col4));
-#pragma unroll
-                for (int k = 0; k < 8; ++k) {
-                    const int r = 4 * k + rsub;
-                    const int64_t prow = pbase + (int64_t)(4 * k) * 256 + cc;
-                    float4 x = *reinterpret_cast<const float4 *>(tl + r * 32 + (((lane & 7) ^ (r & 7)) << 2));
-                    x.x += bq.x; x.y += bq.y; x.z += bq.z; x.w += bq.w;      // (main+cross)+bias
-                    if (a.resid) { x.x += q[k].x; x.y += q[k].y; x.z += q[k].z; x.w += q[k].w; }
-                    if (a.T_elu) { x.x = elu1(x.x); x.y = elu1(x.y); x.z = elu1(x.z); x.w = elu1(x.w); }
-                    if (a.T) *reinterpret_cast<float4 *>(a.T + prow) = x;
-                    if (a.A_hi) {
-                        float y[4] = {x.x, x.y, x.z, x.w};
-                        uint32_t hi[2], lo[2];
-#pragma unroll
-                        for (int i = 0; i < 2; ++i) {
-                            float x0 = a.A_elu ? elu1(y[2 * i]) : y[2 * i], x1 = a.A_elu ? elu1(y[2 * i + 1]) : y[2 * i + 1];
-                            __nv_bfloat16 h0 = __float2bfloat16_rn(x0), h1 = __float2bfloat16_rn(x1);
-                            __nv_bfloat16 l0 = __float2bfloat16_rn(x0 - __bfloat162float(h0)), l1 = __float2bfloat16_rn(x1 - __bfloat162float(h1));
-                            hi[i] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-                            lo[i] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-                        }
-                        *reinterpret_cast<uint2 *>(a.A_hi + prow) = make_uint2(hi[0], hi[1]);
-                        *reinterpret_cast<uint2 *>(a.A_lo + prow) = make_uint2(lo[0], lo[1]);
-                    }
-                }
-#pragma unroll
-                for (int k = 0; k < 8; ++k) q[k] = qn[k];
-            }
-            __syncwarp();                                 // the tiles are rewritten by my next tile
-        }
-        tc_fence_before();
-    }
-    __syncthreads();
-    cluster_sync_all();                                  // the peer may signal my barriers / read my shared memory until here
-    if (warp == 1) {
-        __syncwarp();
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
-    }
-}
-
-// mu/sigma heads on the tensor cores: the 3x3 W -> (n_mu + n_sc <= 32) convolution that ends every net
-// (cifar_train.py:349,368,411,426), with the scale transforms and the UnSqueeze2d index map of the x head in the epilogue.
-// GEMM per image: M = 256 pixels (two UMMA M=128 halves), N = 32 (output channels zero-padded), K = taps x 256.
-// {main, cross} x 2 halves x 32 columns = 128 TMEM columns and 3 x 36 KB stages, so two CTAs share an SM and one's
-// epilogue / start-up runs under the other's MMAs.  Narrow-N MMAs are bound by the A-operand bytes (shared memory reads
-// and L2 -> SM), not by the tensor pipe: the point is to stop spending 16 ms per step in FP32 FMAs (k_conv_simt).
-constexpr int HD_N = 32;
-constexpr int HD_WTILE = HD_N * BK * 2;                       // 2 KB
-constexpr int HD_STAGE = 2 * TILE_BYTES + 2 * HD_WTILE;        // 36 KB
-constexpr int HD_NSTAGE = 3;
-constexpr int HD_SMEM_BYTES = HD_NSTAGE * HD_STAGE + 1024 + 256;
-constexpr uint32_t IDESC_HD = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(HD_N >> 3) << 17) | ((128u >> 4) << 24);
-
+// mu/sigma heads: the 3x3 W -> (n_mu + n_sc <= 32) convolution that ends every net (cifar_train.py:349,368,411,426),
+// with the scale transforms and the UnSqueeze2d index map of the x head in the epilogue.
 struct HeadArgs {
+    static constexpr int kN = HD_N, kCoBlocks = 1;
     int taps, ks;
+    int cchunks;             // 8: K = taps x 256
     const float *bias;       // [>= n_mu + n_sc]
     float *mu, *scale;
     int n_mu, n_sc, scale_kind, out_mode, out_dim;
@@ -928,119 +242,114 @@ __device__ __forceinline__ float hd_scale(float r, int kind) {      // same expr
     return r;
 }
 
-__global__ void __launch_bounds__(TC_THREADS, 2)
-k_conv_tc_head(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ CUtensorMap amap_lo,
-               const __grid_constant__ CUtensorMap wmap_hi, const __grid_constant__ CUtensorMap wmap_lo, HeadArgs a) {
+__device__ __forceinline__ void epilogue(const HeadArgs &a, const float (&dm)[16], const float (&dc)[16], int img, int prow0,
+                                         int co0, int lane) {
+    float *mu_row = a.mu + (int64_t)img * a.out_dim;
+    float *sc_row = a.scale ? a.scale + (int64_t)img * a.out_dim : nullptr;
+#pragma unroll
+    for (int j = 0; j < HD_N / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int c = 8 * j + 2 * (lane & 3) + e;
+                if (c >= a.n_mu + a.n_sc) continue;
+                const int p = prow0 + 8 * h, y = p >> 4, x = p & 15;
+                const int i = 4 * j + 2 * h + e;
+                const bool is_mu = c < a.n_mu;
+                const int o = is_mu ? c : c - a.n_mu;
+                float r = (dm[i] + dc[i]) + __ldg(a.bias + co0 + c);
+                if (!is_mu) r = hd_scale(r, a.scale_kind);
+                float *dst = is_mu ? mu_row : sc_row;
+                if (a.out_mode == OUT_HEAD_Z) dst[o * 256 + p] = r;
+                else dst[(o >> 2) * 1024 + (2 * y + ((o >> 1) & 1)) * 32 + 2 * x + (o & 1)] = r;      // UnSqueeze2d, modules.py:205-207
+            }
+}
+
+// Tile t -> image t / (2 * kCoBlocks), output-channel block, pixel half (t & 1): the tiles of one image run on
+// neighbouring SMs at about the same time, so the activation planes they share come out of L2.
+template <class Args>
+__global__ void __launch_bounds__(WG_THREADS, 1)
+k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ CUtensorMap amap_lo,
+          const __grid_constant__ CUtensorMap wmap_hi, const __grid_constant__ CUtensorMap wmap_lo, const Args a, int ntiles) {
+    constexpr int N = Args::kN;
+    using C = TileCfg<N>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t *full_bar = (uint64_t *)(smem + HD_NSTAGE * HD_STAGE);
-    uint64_t *empty_bar = full_bar + HD_NSTAGE;
-    uint64_t *acc_bar = empty_bar + HD_NSTAGE;
-    uint32_t *tmem_ptr = (uint32_t *)(acc_bar + 1);
+    uint64_t *full_bar = (uint64_t *)(smem + C::NSTAGE * C::STAGE);
+    uint64_t *empty_bar = full_bar + C::NSTAGE;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int img = blockIdx.x;
-    const int nkb = a.taps * 8;
+    const int nkb = a.taps * a.cchunks;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == PRODUCER_WARP && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&amap_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&amap_lo) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap_lo) : "memory");
-        for (int s = 0; s < HD_NSTAGE; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(acc_bar, 1);
+        for (int s = 0; s < C::NSTAGE; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {     // 128 columns: main [0,64) = two halves x 32, cross [64,128)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 128;" ::"r"(smem_u32(tmem_ptr)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
-    if (warp == 0) {
+    if (warp == PRODUCER_WARP) {
         if (lane == 0) {     // ===== TMA producer =====
             const int r = a.ks / 2;
             int stage = 0, phase = 0;
-            for (int kb = 0; kb < nkb; ++kb) {
-                int tap = kb >> 3, c0 = (kb & 7) * BK;
-                int dy = tap / a.ks, dx = tap - dy * a.ks;
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                uint8_t *st = smem + stage * HD_STAGE;
-                mbar_expect_tx(&full_bar[stage], HD_STAGE);
-                tma_load_4d(st, &amap_hi, &full_bar[stage], c0, dx - r, dy - r, img);
-                tma_load_4d(st + TILE_BYTES, &amap_lo, &full_bar[stage], c0, dx - r, dy - r, img);
-                tma_load_3d(st + 2 * TILE_BYTES, &wmap_hi, &full_bar[stage], c0, 0, tap);
-                tma_load_3d(st + 2 * TILE_BYTES + HD_WTILE, &wmap_lo, &full_bar[stage], c0, 0, tap);
-                if (++stage == HD_NSTAGE) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {     // ===== MMA issuer =====
-            int stage = 0, phase = 0;
-            for (int kb = 0; kb < nkb; ++kb) {
-                mbar_wait(&full_bar[stage], phase);
-                tc_fence_after();
-                uint32_t sbase = smem_u32(smem + stage * HD_STAGE);
-#pragma unroll
-                for (int kk = 0; kk < BK / 16; ++kk) {
-#pragma unroll
-                    for (int half = 0; half < 2; ++half) {
-                        uint32_t aoff = half * (128 * BK * 2) + kk * 32;
-                        uint64_t a_hi = make_desc_sw64(sbase + aoff);
-                        uint64_t a_lo = make_desc_sw64(sbase + TILE_BYTES + aoff);
-                        uint64_t b_hi = make_desc_sw64(sbase + 2 * TILE_BYTES + kk * 32);
-                        uint64_t b_lo = make_desc_sw64(sbase + 2 * TILE_BYTES + HD_WTILE + kk * 32);
-                        uint32_t d_main = tmem_base + half * HD_N, d_cross = tmem_base + 64 + half * HD_N;
-                        const uint32_t acc = (kb | kk) != 0;
-                        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n"
-                                     ::"r"(d_main), "l"(a_hi), "l"(b_hi), "r"(IDESC_HD), "r"(acc) : "memory");
-                        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n"
-                                     ::"r"(d_cross), "l"(a_lo), "l"(b_hi), "r"(IDESC_HD), "r"(acc) : "memory");
-                        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n"
-                                     ::"r"(d_cross), "l"(a_hi), "l"(b_lo), "r"(IDESC_HD), "r"(1u) : "memory");
-                    }
+            for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+                const int img = t / (2 * Args::kCoBlocks), co0 = ((t >> 1) % Args::kCoBlocks) * N, mh = t & 1;
+                for (int kb = 0; kb < nkb; ++kb) {
+                    const int tap = kb / a.cchunks, c0 = (kb - tap * a.cchunks) * BK;
+                    const int dy = tap / a.ks, dx = tap - dy * a.ks;
+                    mbar_wait(&empty_bar[stage], phase ^ 1);
+                    uint8_t *st = smem + stage * C::STAGE;
+                    mbar_expect_tx(&full_bar[stage], C::STAGE);
+                    tma_load_4d(st, &amap_hi, &full_bar[stage], c0, dx - r, dy - r + 8 * mh, img);
+                    tma_load_4d(st + A_BYTES, &amap_lo, &full_bar[stage], c0, dx - r, dy - r + 8 * mh, img);
+                    tma_load_3d(st + 2 * A_BYTES, &wmap_hi, &full_bar[stage], c0, co0, tap);
+                    tma_load_3d(st + 2 * A_BYTES + C::W_BYTES, &wmap_lo, &full_bar[stage], c0, co0, tap);
+                    if (++stage == C::NSTAGE) { stage = 0; phase ^= 1; }
                 }
-                umma_commit(&empty_bar[stage]);
-                if (++stage == HD_NSTAGE) { stage = 0; phase ^= 1; }
             }
-            umma_commit(acc_bar);
         }
-    } else {
-        // ===== epilogue: warp -> (pixel half, TMEM lane quadrant); a lane owns one pixel and all 32 output channels.
-        // For a fixed channel the 32 lanes write 32 consecutive pixels of the flat CHW mu / sigma rows: whole lines. =====
-        const int ew = warp - 2;
-        const int half = ew >> 2;
-        const int quad = warp & 3;
-        const int p = half * 128 + quad * 32 + lane;
-        const int y = p >> 4, x = p & 15;
-        mbar_wait(acc_bar, 0);
-        tc_fence_after();
-        uint32_t rr[32], rc[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + half * HD_N, rr);
-        tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + 64 + half * HD_N, rc);
-        float *mu_row = a.mu + (int64_t)img * a.out_dim;
-        float *sc_row = a.scale ? a.scale + (int64_t)img * a.out_dim : nullptr;
-#pragma unroll
-        for (int c = 0; c < HD_N; ++c) {
-            if (c >= a.n_mu + a.n_sc) break;
-            const bool is_mu = c < a.n_mu;
-            const int o = is_mu ? c : c - a.n_mu;
-            float r = (__uint_as_float(rr[c]) + __uint_as_float(rc[c])) + __ldg(a.bias + c);
-            if (!is_mu) r = hd_scale(r, a.scale_kind);
-            float *dst = is_mu ? mu_row : sc_row;
-            if (a.out_mode == OUT_HEAD_Z) dst[o * 256 + p] = r;
-            else dst[(o >> 2) * 1024 + (2 * y + ((o >> 1) & 1)) * 32 + 2 * x + (o & 1)] = r;      // UnSqueeze2d, modules.py:205-207
-        }
-        tc_fence_before();
+        return;
     }
-    __syncthreads();
-    if (warp == 1) {
-        __syncwarp();
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 128;" ::"r"(tmem_base) : "memory");
+
+    // ===== consumers: warpgroup wg owns tile rows [64 wg, 64 wg + 64) =====
+    const int wg = warp >> 2;
+    const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);          // this thread's first accumulator row
+    int stage = 0, phase = 0;
+    for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const int img = t / (2 * Args::kCoBlocks), co0 = ((t >> 1) % Args::kCoBlocks) * N, mh = t & 1;
+        float dm[N / 2], dc[N / 2];
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) { dm[i] = 0.f; dc[i] = 0.f; }
+        int prev = -1;
+        for (int kb = 0; kb < nkb; ++kb) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t sbase = smem_u32(smem + stage * C::STAGE);
+            wg_fence();
+#pragma unroll
+            for (int kk = 0; kk < BK / 16; ++kk) {
+                const uint64_t a_hi = make_desc_sw64(sbase + wg * (64 * BK * 2) + kk * 32);
+                const uint64_t a_lo = make_desc_sw64(sbase + A_BYTES + wg * (64 * BK * 2) + kk * 32);
+                const uint64_t b_hi = make_desc_sw64(sbase + 2 * A_BYTES + kk * 32);
+                const uint64_t b_lo = make_desc_sw64(sbase + 2 * A_BYTES + C::W_BYTES + kk * 32);
+                Wgmma<N>::mma(dm, a_hi, b_hi);
+                Wgmma<N>::mma(dc, a_lo, b_hi);
+                Wgmma<N>::mma(dc, a_hi, b_lo);
+            }
+            wg_commit();
+            wg_wait<1>();                                  // the previous k-block's MMAs have read their stage
+            if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+            prev = stage;
+            if (++stage == C::NSTAGE) { stage = 0; phase ^= 1; }
+        }
+        wg_wait<0>();
+        fence_regs(dm);
+        fence_regs(dc);
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+        epilogue(a, dm, dc, img, mh * 128 + row0, co0, lane);
     }
 }
 
@@ -1110,7 +419,7 @@ int encode_map(CUtensorMap *m, void *base, int rank, const cuuint64_t *dims, con
 struct TcSlot { CUtensorMap map_hi, map_lo; };
 
 int bsw_model_tc_prepare(bsw_model *m) {
-    BSW_REQUIRE(m->Wp == 256, "tcgen05 conv path needs a padded width of 256 (reswidth 193..256)");
+    BSW_REQUIRE(m->Wp == 256, "tensor-core conv path needs a padded width of 256 (reswidth 193..256)");
     TcState *ts = new TcState();
     m->tc_state = ts;
     const size_t act_elems = (size_t)m->d.max_batch * 256 * 256;
@@ -1120,20 +429,16 @@ int bsw_model_tc_prepare(bsw_model *m) {
             BSW_CUDA(cudaMemset(ts->act[b][pl], 0, act_elems * sizeof(__nv_bfloat16)));
             cuuint64_t dims[4] = {256, 16, 16, (cuuint64_t)m->d.max_batch};
             cuuint64_t str[3] = {256 * 2, 16 * 256 * 2, 256 * 256 * 2};
-            cuuint32_t box[4] = {BK, 16, 16, 1};
+            cuuint32_t box[4] = {BK, 16, 8, 1};
             if (int rc = encode_map(&ts->act_map[b][pl], ts->act[b][pl], 4, dims, str, box)) return rc;
-            cuuint32_t boxh[4] = {BK, 16, 8, 1};
-            if (int rc = encode_map(&ts->act_map_h[b][pl], ts->act[b][pl], 4, dims, str, boxh)) return rc;
         }
     for (int pl = 0; pl < 2; ++pl) {
         size_t elems = (size_t)m->d.max_batch * 256 * 32;
         BSW_CUDA(cudaMalloc(&ts->inp[pl], elems * sizeof(__nv_bfloat16)));
         cuuint64_t dims[4] = {32, 16, 16, (cuuint64_t)m->d.max_batch};
         cuuint64_t str[3] = {32 * 2, 16 * 32 * 2, 256 * 32 * 2};
-        cuuint32_t box[4] = {BK, 16, 16, 1};
+        cuuint32_t box[4] = {BK, 16, 8, 1};
         if (int rc = encode_map(&ts->inp_map[pl], ts->inp[pl], 4, dims, str, box)) return rc;
-        cuuint32_t boxh[4] = {BK, 16, 8, 1};
-        if (int rc = encode_map(&ts->inp_map_h[pl], ts->inp[pl], 4, dims, str, boxh)) return rc;
     }
     // weights: [tap][o=256][c=Kc] bf16 hi/lo planes, K (=c) innermost; Kc = 256 for the dense convs, 32 for the in-convs
     std::vector<TcSlot> *slots = new std::vector<TcSlot>();
@@ -1176,16 +481,11 @@ int bsw_model_tc_prepare(bsw_model *m) {
         slots->push_back(s);
     }
     m->tc_slots = slots;
-    BSW_CUDA(cudaFuncSetAttribute(k_conv_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    BSW_CUDA(cudaFuncSetAttribute(k_conv_tc_h, cudaFuncAttributeMaxDynamicSharedMemorySize, H_SMEM_BYTES));
-    BSW_CUDA(cudaFuncSetAttribute(k_conv_tc_p, cudaFuncAttributeMaxDynamicSharedMemorySize, P_SMEM_BYTES));
-    BSW_CUDA(cudaFuncSetAttribute(k_conv_tc_2sm, cudaFuncAttributeMaxDynamicSharedMemorySize, P2_SMEM_BYTES));
-    bsw_prefer_max_shared(k_conv_tc_2sm);
-    BSW_CUDA(cudaFuncSetAttribute(k_conv_tc_head, cudaFuncAttributeMaxDynamicSharedMemorySize, HD_SMEM_BYTES));
-    bsw_prefer_max_shared(k_conv_tc_head);
+    BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<TcArgs>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<BN>::SMEM));
+    BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<HeadArgs>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<HD_N>::SMEM));
     // one SM-wide L1/shared split for every kernel of the path (see bsw_prefer_max_shared)
-    bsw_prefer_max_shared(k_conv_tc); bsw_prefer_max_shared(k_conv_tc_h);
-    bsw_prefer_max_shared(k_conv_tc_p); bsw_prefer_max_shared(k_given_to_planes);
+    bsw_prefer_max_shared(k_conv_wg<TcArgs>); bsw_prefer_max_shared(k_conv_wg<HeadArgs>);
+    bsw_prefer_max_shared(k_given_to_planes);
     m->tc_ready = true;
     return BSW_OK;
 }
@@ -1218,31 +518,29 @@ int bsw_tc_split(bsw_model *m, const float *in, int which, int64_t n, cudaStream
     return BSW_OK;
 }
 
-// Which kernel the dense convs and in-convs run on: a bit mask -- 8 / 16 = dense 3x3 / 5x5 on the pair-tile kernel
-// k_conv_tc_2sm, 1 / 2 = dense 3x3 / 5x5 on the persistent half-image kernel k_conv_tc_p, 4 = in-convs on k_conv_tc_p; a
-// clear bit means the per-tile grid (k_conv_tc / k_conv_tc_h).  Default 24 (BSW_TC_PERSIST overrides): measured on B200 at
-// 1024 images the pair tiles win (3x3 0.83 -> 0.68 ms, 5x5 1.94 -> 1.55 ms) because the convs are bound by L2 -> SM bytes
-// per MMA, which N = 256 and the weight-tile split halve; the half-image tiles of k_conv_tc_p lose to the per-tile grids
-// for the same reason.  Results are bit-identical in every mode.
+// Which grid the convolutions run on: a bit mask -- 1 / 2 = dense 3x3 / 5x5, 4 = in-convs and heads on a persistent grid
+// (one CTA per SM walking the tiles, the TMA ring prefetching across tile boundaries); a clear bit means one CTA per tile.
+// Default 7 (BSW_TC_PERSIST overrides).  Same kernel, same k order per tile: results are bit-identical in every mode.
 static int g_tc_mode = -1;
 static bool tc_persistent(int which) {
-    static const int env = getenv("BSW_TC_PERSIST") ? atoi(getenv("BSW_TC_PERSIST")) : 24;
+    static const int env = getenv("BSW_TC_PERSIST") ? atoi(getenv("BSW_TC_PERSIST")) : 7;
     return (((g_tc_mode < 0) ? env : g_tc_mode) & which) != 0;
 }
 extern "C" int bsw_set_conv_mode(int mode) {
-    BSW_REQUIRE(mode >= -1 && mode <= 31, "bsw_set_conv_mode: -1 (default) or a mask of 1 | 2 | 4 (persistent: dense 3x3, 5x5, in-convs) | 8 | 16 (pair tiles: dense 3x3, 5x5)");
+    BSW_REQUIRE(mode >= -1 && mode <= 7, "bsw_set_conv_mode: -1 (default) or a mask of 1 | 2 | 4 (persistent grid: dense 3x3, 5x5, in-convs and heads)");
     g_tc_mode = mode;
     return BSW_OK;
 }
-static unsigned tc_pgrid(int ntiles) {             // one CTA per SM of the current device, at most one per tile
+static unsigned tc_grid(int ntiles, bool persistent) {   // one CTA per tile, or one per SM of the current device
     static int sms[64] = {0};
+    if (!persistent) return (unsigned)ntiles;
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) dev = 0;
     if (!sms[dev]) {
         int v = 0;
         cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-        sms[dev] = v > 0 ? v : 148;
+        sms[dev] = v > 0 ? v : 132;
     }
     return (unsigned)(ntiles < sms[dev] ? ntiles : sms[dev]);
 }
@@ -1259,20 +557,9 @@ int bsw_conv_tc(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t n, c
     t.A_hi = a.A_planes >= 0 ? ts->act[a.A_planes][0] : nullptr;
     t.A_lo = a.A_planes >= 0 ? ts->act[a.A_planes][1] : nullptr;
     t.A_elu = a.A_elu;
-    // Kernel choice by measurement (B200, 1024 images), see the mode mask above.  A 2-CTA cluster with multicast activation
-    // tiles but M = 128 MMAs (r1) measured no gain (0.897 vs 0.880 ms) and is gone; so is a pair kernel with N = 128 and a
-    // TMEM ping-pong (0.92 / 2.4 ms).
-    if (tc_persistent(c.ks <= 3 ? 8 : 16)) {
-        const int ntiles = (int)n;                                        // one pair tile per image
-        const unsigned pairs = tc_pgrid(ntiles * 2) / 2;                 // one cluster per SM pair, at most one per tile
-        k_conv_tc_2sm<<<2 * pairs, (2 + P2_NE) * 32, P2_SMEM_BYTES, st>>>(ts->act_map_h[a.in_planes][0], ts->act_map_h[a.in_planes][1],
-                                                                           s.map_hi, s.map_lo, t, ntiles);
-    } else if (tc_persistent(c.ks <= 3 ? 1 : 2))
-        k_conv_tc_p<<<tc_pgrid((int)n * 4), TC_THREADS, P_SMEM_BYTES, st>>>(ts->act_map_h[a.in_planes][0], ts->act_map_h[a.in_planes][1],
-                                                                           s.map_hi, s.map_lo, t, (int)n * 4);
-    else
-        k_conv_tc<<<dim3((unsigned)n, 256 / BN), TC_THREADS, SMEM_BYTES, st>>>(ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1],
-                                                                           s.map_hi, s.map_lo, t);
+    const int ntiles = (int)n * 2 * TcArgs::kCoBlocks;
+    k_conv_wg<TcArgs><<<tc_grid(ntiles, tc_persistent(c.ks <= 3 ? 1 : 2)), WG_THREADS, TileCfg<BN>::SMEM, st>>>(
+        ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1], s.map_hi, s.map_lo, t, ntiles);
     BSW_LAUNCH_CHECK();
     return BSW_OK;
 }
@@ -1288,14 +575,16 @@ int bsw_conv_tc_head(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t
     BSW_REQUIRE(ts && c.tc_index >= 0 && a.n_mu + a.n_sc <= HD_N, "bsw_conv_tc_head: conv has no tensor-core head weights");
     const TcSlot &s = (*(std::vector<TcSlot> *)m->tc_slots)[c.tc_index];
     HeadArgs h;
-    h.taps = c.ks * c.ks; h.ks = c.ks; h.bias = c.bias; h.mu = a.mu; h.scale = a.scale; h.n_mu = a.n_mu; h.n_sc = a.n_sc;
+    h.taps = c.ks * c.ks; h.ks = c.ks; h.cchunks = 8; h.bias = c.bias; h.mu = a.mu; h.scale = a.scale; h.n_mu = a.n_mu; h.n_sc = a.n_sc;
     h.scale_kind = a.scale_kind; h.out_mode = a.out_mode; h.out_dim = a.out_dim;
-    k_conv_tc_head<<<(unsigned)n, TC_THREADS, HD_SMEM_BYTES, st>>>(ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1], s.map_hi, s.map_lo, h);
+    const int ntiles = (int)n * 2;
+    k_conv_wg<HeadArgs><<<tc_grid(ntiles, tc_persistent(4)), WG_THREADS, TileCfg<HD_N>::SMEM, st>>>(
+        ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1], s.map_hi, s.map_lo, h, ntiles);
     BSW_LAUNCH_CHECK();
     return BSW_OK;
 }
 
-// In-conv on the tensor cores: `given` (flat CHW float32) -> 32-channel bf16 planes -> k_conv_tc with one channel chunk
+// In-conv on the tensor cores: `given` (flat CHW float32) -> 32-channel bf16 planes -> k_conv_wg with one channel chunk
 // per tap.  Epilogue as for every conv: T = ELU(raw) (the trunk), A planes = ELU(T) for the first ResNet layer.
 int bsw_conv_tc_in(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t n, cudaStream_t st, int *launches) {
     TcState *ts = (TcState *)m->tc_state;
@@ -1311,12 +600,9 @@ int bsw_conv_tc_in(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t n
     t.A_hi = a.A_planes >= 0 ? ts->act[a.A_planes][0] : nullptr;
     t.A_lo = a.A_planes >= 0 ? ts->act[a.A_planes][1] : nullptr;
     t.A_elu = a.A_elu;
-    // in-convs: nine or twenty-five tiny k-blocks, all epilogue -> half-image tiles, two CTAs per SM (0.26 ms per launch at
-    // 1024 images against 0.55 ms on the full tile)
-    if (tc_persistent(4))
-        k_conv_tc_p<<<tc_pgrid((int)n * 4), TC_THREADS, P_SMEM_BYTES, st>>>(ts->inp_map_h[0], ts->inp_map_h[1], s.map_hi, s.map_lo, t, (int)n * 4);
-    else
-        k_conv_tc_h<<<dim3((unsigned)n, 256 / BN, 2), TC_THREADS, H_SMEM_BYTES, st>>>(ts->inp_map_h[0], ts->inp_map_h[1], s.map_hi, s.map_lo, t);
+    const int ntiles = (int)n * 2 * TcArgs::kCoBlocks;
+    k_conv_wg<TcArgs><<<tc_grid(ntiles, tc_persistent(4)), WG_THREADS, TileCfg<BN>::SMEM, st>>>(
+        ts->inp_map[0], ts->inp_map[1], s.map_hi, s.map_lo, t, ntiles);
     BSW_LAUNCH_CHECK();
     *launches += 2;
     return BSW_OK;

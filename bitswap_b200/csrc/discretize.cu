@@ -1,4 +1,4 @@
-// Sampling epilogue and bin fit of the latent-space discretisation (sm_100a).
+// Sampling epilogue and bin fit of the latent-space discretisation (sm_90a).
 //
 // Reference: discretize() / discretize_kbins(), discretization.py:30-118.  Per latent level it draws 30 * 2^q samples per
 // dimension from the generative chain and as many from the inference chain,

@@ -1,4 +1,4 @@
-// The inference-time hierarchical VAE (sm_100a): weight-norm folding, conv stacks, mu/sigma heads.
+// The inference-time hierarchical VAE (sm_90a): weight-norm folding, conv stacks, mu/sigma heads.
 //
 // Reference being replaced (fhkingma/bitswap @ dfe0bf7d):
 //   Model.infer(i)(given) / Model.generate(i)(given), compressing mode   model/cifar_train.py:315-438
@@ -16,7 +16,7 @@
 //
 // This file holds the float32 SIMT implicit-GEMM conv (k_conv_simt): the permanent path for the
 // small-contraction convs (in-convs with 1..12 input channels, mu/sigma heads with <= 32 outputs) and
-// the fallback-free baseline for the dense W->W convs; conv_tc.cu adds the tcgen05 path for those.
+// the fallback-free baseline for the dense W->W convs; conv_tc.cu adds the wgmma tensor-core path for those.
 #include <math.h>
 #include <map>
 #include <string>

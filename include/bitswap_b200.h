@@ -1,5 +1,5 @@
 /*
- * bitswap_b200.h -- C ABI of the B200-native Bit-Swap hot path.
+ * bitswap_b200.h -- C ABI of the H100-native Bit-Swap hot path.
  *
  * The reference (fhkingma/bitswap @ dfe0bf7d) is pure Python and has no FFI: its
  * "plugin interface" for this path is a handful of Python call signatures
@@ -36,7 +36,7 @@ typedef enum {
 
 const char *bsw_last_error(void);
 int         bsw_version(void);
-/* 1 if this build contains the tcgen05 conv path (bsw_model_desc.use_tensor_cores may be set). */
+/* 1 if this build contains the tensor-core (wgmma) conv path (bsw_model_desc.use_tensor_cores may be set). */
 int         bsw_has_tensor_cores(void);
 /* Measures this GPU's peak float64 FMA rate (DFMA/s, lanes) with a register-resident kernel: the roofline
  * denominator of the float64 row-table kernel (the driver's MEASURED_PEAKS.json has no FP64 figure). */
@@ -182,10 +182,9 @@ int bsw_rows6_set_verify(int on);
 /* Mapping of the affine-row table kernel: lanes of a warp that share one row (2, 4, 8 or 32; 0 = default 4, i.e. eight
  * rows per warp).  Every setting emits the same integers; exposed for A/B timing and the parity test. */
 int bsw_rows6_set_lanes_per_row(int lpr);
-/* Launch shape of the tcgen05 convolutions, a bit mask: 8 / 16 = dense 3x3 / dense 5x5 on the pair-tile kernel (2-CTA
- * clusters issuing cta_group::2 M = 256, N = 256 MMAs, one image per pair, weight tile split across the pair), 1 / 2 / 4 =
- * dense 3x3 / dense 5x5 / in-convs on the persistent kernel (one CTA per SM walking half-image tiles with a TMEM
- * ping-pong); a clear bit = one CTA per tile.  -1 = default (BSW_TC_PERSIST if set, else 24).  Bit-identical results. */
+/* Launch shape of the tensor-core convolutions, a bit mask: 1 / 2 / 4 = dense 3x3 / dense 5x5 / in-convs and heads on a
+ * persistent grid (one CTA per SM walking half-image tiles); a clear bit = one CTA per tile.  -1 = default
+ * (BSW_TC_PERSIST if set, else 7).  Bit-identical results. */
 int bsw_set_conv_mode(int mode);
 int bsw_rows6_verify_read(uint64_t *out4_host);
 int bsw_logistic_push_2p(bsw_streams *s, int first, int count, const float *mu_dev, int64_t mu_stream_stride,
@@ -252,7 +251,7 @@ typedef struct {
     int32_t reswidth;
     int32_t cond_xscale;   /* imagenetcrop: x-scale from a conv head */
     int32_t max_batch;     /* activations are preallocated for this many images */
-    int32_t use_tensor_cores; /* 1: tcgen05 path for the W->W convs (needs padded width 256); 0: fp32 SIMT */
+    int32_t use_tensor_cores; /* 1: wgmma tensor-core path for the W->W convs (needs padded width 256); 0: fp32 SIMT */
 } bsw_model_desc;
 
 int bsw_model_create(bsw_model **out, const bsw_model_desc *desc);
@@ -295,7 +294,7 @@ int bsw_codec_decode(bsw_codec *c, bsw_streams *s, int first, int count, uint8_t
 int64_t bsw_codec_last_launches(const bsw_codec *c);
 /* Stream placement inside one encode/decode call: 0 (default) = every kernel on the caller's stream; 1 = conv kernels
  * on a high-priority internal stream, coder kernels on a low-priority one, chained with events and joined back into
- * `stream` at the end (an experiment in co-scheduling tensor-bound and FP64-bound CTAs; measured no gain on B200). */
+ * `stream` at the end (an experiment in co-scheduling tensor-bound and FP64-bound CTAs). */
 int bsw_codec_set_dual_stream(bsw_codec *c, int on);
 /* Coder variant: 1 (default) = two-phase (ans_rows.cu: fully parallel float64 row tables, then the serial integer
  * coder), 0 = fused one-warp-per-stream kernels (bsw_logistic_push/pop).  Bit-identical results. */

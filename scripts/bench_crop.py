@@ -152,7 +152,7 @@ def run_crop(args, rank, world, local):
         line = {"metric": "Mpixels/sec encode+decode (Bit-Swap, variable-size images as chained 32x32 block streams)", "value": value,
                 "unit": "Mpixel/s", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 1),
                 "ms_per_step": 1e3 * (enc + gat + dec) / args.steps, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
-                "dtype": "f64 tables / int64 coder / bf16x3 split tcgen05 convs", "data": "synthetic",
+                "dtype": "f64 tables / int64 coder / bf16x3 split wgmma convs", "data": "synthetic",
                 "config": {"workload": f"BASELINE configs[4]: {n} variable-size images (H, W ~ U{{224..512}}, {sum(costs)} blocks of 32x32x3), each "
                                        f"image ONE chain over its blocks, imagenetcrop model (nz=4, W=256, conditional x-scale), chains dealt to "
                                        f"{world} GPU(s) by block count; step = compress every chain + gather the containers on rank 0 + decompress",

@@ -1,6 +1,6 @@
-"""Do the FP64-bound table kernel (k_rows6) and the tensor-bound convs (k_conv_tc) actually run TOGETHER on an SM?
+"""Do the FP64-bound table kernel (k_rows6) and the tensor-bound convs (k_conv_wg) actually run TOGETHER on an SM?
 
-VERDICT r1 weak #10: "FP64 || tensor overlap is asserted, not shown".  This probe times, on one B200,
+VERDICT r1 weak #10: "FP64 || tensor overlap is asserted, not shown".  This probe times, on one GPU,
   A  a loop of Model.infer(0) calls (in-conv + 8 dense 5x5 + 2 dense 3x3 + head; tensor pipe) alone,
   B  a loop of two-phase logistic pushes (k_rows6 + k_push_pairs; FP64 pipe) alone,
   C  both loops at once on two CUDA streams of equal priority,

@@ -1,4 +1,4 @@
-"""CPU-only checks of the drop-in boundary: the C-ABI library builds for sm_100a, loads, and exports
+"""CPU-only checks of the drop-in boundary: the C-ABI library builds for sm_90a, loads, and exports
 every symbol include/bitswap_b200.h declares (no compute calls without a GPU)."""
 import ctypes
 import os
@@ -27,11 +27,11 @@ def test_header_symbols_are_exported(so):
     assert sorted(_lib.EXPORTS) == declared
 
 
-def test_library_is_sm100a_only(so):
+def test_library_is_sm90a_only(so):
     import subprocess
     out = subprocess.run(["cuobjdump", "-lelf", so], stdout=subprocess.PIPE, text=True).stdout
     archs = set(re.findall(r"sm_\d+a?", out))
-    assert archs == {"sm_100a"}, archs
+    assert archs == {"sm_90a"}, archs
 
 
 def test_product_does_not_import_the_oracle():

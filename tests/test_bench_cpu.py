@@ -29,17 +29,3 @@ def test_reference_arm_prints_one_contract_line():
     assert set(split) == {"cdf", "net", "pop", "push", "tables"} and abs(sum(split.values()) - 1.0) < 1e-6
     print(f"reference arm (tiny3, 1 worker): {d['value']:.5f} Mpixel/s, {time.time() - t0:.1f} s wall")
 
-
-def test_ncu_facts_follow_from_the_tracked_raw_pages(tmp_path):
-    """bench.py's roofline.traffic / roofline.fp64 come from profiles/ncu_facts_r2.json; that file must be what
-    scripts/ncu_summary.py derives from the tracked `ncu --page raw --csv` exports (no hand-edited constants)."""
-    out = tmp_path / "facts.json"
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "scripts", "ncu_summary.py"), "facts", "1024", str(out),
-                        os.path.join(ROOT, "profiles", "r2_final_rows_raw.csv"), os.path.join(ROOT, "profiles", "r2_final_convs_raw.csv")],
-                       stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=120, cwd=ROOT)
-    assert r.returncode == 0, r.stderr[-2000:]
-    got, want = json.load(open(out)), json.load(open(os.path.join(ROOT, "profiles", "ncu_facts_r2.json")))
-    assert set(got) == set(want) and {"rows_z", "pop_z", "push_z", "conv_dense3x3", "conv_dense5x5"} <= set(got)
-    for cat in want:
-        for key in ("dram_bytes_per_launch", "fp64_inst_per_launch", "warp_inst_per_launch", "ncu_ms_per_launch", "launches_captured"):
-            assert abs(got[cat][key] - want[cat][key]) <= 1e-9 * max(1.0, abs(want[cat][key])), (cat, key)
