@@ -20,6 +20,12 @@
 //     warp 8 = TMA producer (one elected lane) feeding an NSTAGE ring of mbarrier-guarded stages.
 //   * a CTA walks tiles t = blockIdx.x, + gridDim.x, ...: with one CTA per tile (per-tile grid) or one per SM
 //     (persistent grid, the producer then prefetches the next tile's k-blocks while the consumers run the epilogue).
+//   * the dense convs and in-convs run as four-CTA clusters, one image per cluster, CTA rank r = tile t & 3 =
+//     (pixel half r & 1, channel block r >> 1): the two channel blocks of a pixel half read the same A boxes, the two
+//     pixel halves of a channel block the same W boxes.  Each CTA issues two of a stage's four boxes with TMA multicast
+//     to itself and the peer that shares them, so every CTA pulls 16 of its 32 KB per k-block from L2 (the launches are
+//     bound by L2 -> SM bytes, not by their MMAs).  A stage is refilled only after all three CTAs writing into it
+//     released it.
 //   * fixed k order, no split-K, no atomics: results are bit-identical for any batch size, position in the batch
 //     or grid (the decoder must regenerate the encoder's tables exactly, SURVEY.md H3).
 #include <cuda.h>
@@ -71,6 +77,16 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// Arrive on the barrier at the same shared-memory offset in cluster CTA `rank` (this CTA included).  Used to release a
+// stage after wgmma.wait_group has retired the MMAs that read it: no read is left in flight for a fence to order.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t *bar, uint32_t rank) {
+    asm volatile(
+        "{\n"
+        ".reg .b32 ra;\n"
+        "mapa.shared::cluster.u32 ra, %0, %1;\n"
+        "mbarrier.arrive.shared::cluster.b64 _, [ra];\n"
+        "}\n" ::"r"(smem_u32(bar)), "r"(rank) : "memory");
+}
 __device__ __forceinline__ bool mbar_try_wait(uint64_t *bar, uint32_t parity) {
     uint32_t ok;
     asm volatile(
@@ -103,6 +119,32 @@ __device__ __forceinline__ void tma_load_4d(void *dst, const CUtensorMap *map, u
 __device__ __forceinline__ void tma_load_3d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, int c2) {
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                  ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+// Multicast: the box lands at the same shared-memory offset in every cluster CTA of `mask` and completes its bytes on
+// the barrier at `bar`'s offset in each of them.
+__device__ __forceinline__ void tma_load_4d_mc(void *dst, const CUtensorMap *map, uint64_t *bar, uint16_t mask, int c0, int c1, int c2,
+                                               int c3) {
+    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+                 " [%0], [%1, {%4, %5, %6, %7}], [%2], %3;"
+                 ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "h"(mask), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+__device__ __forceinline__ void tma_load_3d_mc(void *dst, const CUtensorMap *map, uint64_t *bar, uint16_t mask, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+                 " [%0], [%1, {%4, %5, %6}], [%2], %3;"
+                 ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "h"(mask), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+__device__ __forceinline__ uint32_t cluster_nctarank() {
+    uint32_t n;
+    asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(n));
+    return n;
+}
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
 // K-major, SWIZZLE_64B wgmma shared-memory matrix descriptor:
@@ -268,6 +310,8 @@ __device__ __forceinline__ void epilogue(const HeadArgs &a, const float (&dm)[16
 
 // Tile t -> image t / (2 * kCoBlocks), output-channel block, pixel half (t & 1): the tiles of one image run on
 // neighbouring SMs at about the same time, so the activation planes they share come out of L2.
+// Launched as four-CTA clusters (TcArgs only, see the file comment), gridDim.x is a multiple of 4: t & 3 is the CTA's
+// cluster rank and the four CTAs of a cluster walk the same images in step.
 template <class Args>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ CUtensorMap amap_lo,
@@ -281,20 +325,26 @@ k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ C
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nkb = a.taps * a.cchunks;
+    const bool mc = Args::kCoBlocks == 2 && cluster_nctarank() == 4;
+    const uint32_t rank = mc ? cluster_ctarank() : 0;
 
     if (warp == PRODUCER_WARP && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&amap_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&amap_lo) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap_lo) : "memory");
-        for (int s = 0; s < C::NSTAGE; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
+        // empty: both consumer warpgroups of this CTA and, with multicast, of the two peers that write into its stages
+        for (int s = 0; s < C::NSTAGE; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], mc ? 6 : 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    __syncthreads();
+    // peers arrive on these barriers and multicast into this CTA's stages: all barriers of the cluster are initialised first
+    if (mc) cluster_sync();
+    else __syncthreads();
 
     if (warp == PRODUCER_WARP) {
         if (lane == 0) {     // ===== TMA producer =====
             const int r = a.ks / 2;
+            const uint16_t amask = (uint16_t)(0x5u << (rank & 1)), wmask = (uint16_t)(0x3u << (rank & 2));
             int stage = 0, phase = 0;
             for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
                 const int img = t / (2 * Args::kCoBlocks), co0 = ((t >> 1) % Args::kCoBlocks) * N, mh = t & 1;
@@ -303,13 +353,28 @@ k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ C
                     const int dy = tap / a.ks, dx = tap - dy * a.ks;
                     mbar_wait(&empty_bar[stage], phase ^ 1);
                     uint8_t *st = smem + stage * C::STAGE;
-                    mbar_expect_tx(&full_bar[stage], C::STAGE);
-                    tma_load_4d(st, &amap_hi, &full_bar[stage], c0, dx - r, dy - r + 8 * mh, img);
-                    tma_load_4d(st + A_BYTES, &amap_lo, &full_bar[stage], c0, dx - r, dy - r + 8 * mh, img);
-                    tma_load_3d(st + 2 * A_BYTES, &wmap_hi, &full_bar[stage], c0, co0, tap);
-                    tma_load_3d(st + 2 * A_BYTES + C::W_BYTES, &wmap_lo, &full_bar[stage], c0, co0, tap);
+                    mbar_expect_tx(&full_bar[stage], C::STAGE);       // whole stage: the peers' boxes complete here too
+                    if (mc) {
+                        // A_hi by channel block 0, A_lo by block 1 of this pixel half; W_hi by pixel half 0, W_lo by half 1
+                        const int ao = (rank & 2) ? A_BYTES : 0, wo = (rank & 1) ? C::W_BYTES : 0;
+                        tma_load_4d_mc(st + ao, (rank & 2) ? &amap_lo : &amap_hi, &full_bar[stage], amask, c0, dx - r,
+                                       dy - r + 8 * mh, img);
+                        tma_load_3d_mc(st + 2 * A_BYTES + wo, (rank & 1) ? &wmap_lo : &wmap_hi, &full_bar[stage], wmask, c0,
+                                       co0, tap);
+                    } else {
+                        tma_load_4d(st, &amap_hi, &full_bar[stage], c0, dx - r, dy - r + 8 * mh, img);
+                        tma_load_4d(st + A_BYTES, &amap_lo, &full_bar[stage], c0, dx - r, dy - r + 8 * mh, img);
+                        tma_load_3d(st + 2 * A_BYTES, &wmap_hi, &full_bar[stage], c0, co0, tap);
+                        tma_load_3d(st + 2 * A_BYTES + C::W_BYTES, &wmap_lo, &full_bar[stage], c0, co0, tap);
+                    }
                     if (++stage == C::NSTAGE) { stage = 0; phase ^= 1; }
                 }
+            }
+            // Drain: wait for the last release of every stage.  With multicast, peers arrive on this CTA's barriers
+            // until then, so the CTA must not exit before (a stage never filled passes at once: parity phase ^ 1).
+            for (int s = 0; s < C::NSTAGE; ++s) {
+                mbar_wait(&empty_bar[stage], phase ^ 1);
+                if (++stage == C::NSTAGE) { stage = 0; phase ^= 1; }
             }
         }
         return;
@@ -318,6 +383,12 @@ k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ C
     // ===== consumers: warpgroup wg owns tile rows [64 wg, 64 wg + 64) =====
     const int wg = warp >> 2;
     const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);          // this thread's first accumulator row
+    // one thread per warpgroup releases a stage: to this CTA's producer and, with multicast, to the two peers writing into it
+    auto release = [&](int s) {
+        if ((threadIdx.x & 127) != 0) return;
+        if (mc) { mbar_arrive_cluster(&empty_bar[s], rank); mbar_arrive_cluster(&empty_bar[s], rank ^ 1); mbar_arrive_cluster(&empty_bar[s], rank ^ 2); }
+        else mbar_arrive(&empty_bar[s]);
+    };
     int stage = 0, phase = 0;
     for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
         const int img = t / (2 * Args::kCoBlocks), co0 = ((t >> 1) % Args::kCoBlocks) * N, mh = t & 1;
@@ -341,14 +412,14 @@ k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ C
             }
             wg_commit();
             wg_wait<1>();                                  // the previous k-block's MMAs have read their stage
-            if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+            if (prev >= 0) release(prev);
             prev = stage;
             if (++stage == C::NSTAGE) { stage = 0; phase ^= 1; }
         }
         wg_wait<0>();
         fence_regs(dm);
         fence_regs(dc);
-        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+        if (prev >= 0) release(prev);
         epilogue(a, dm, dc, img, mh * 128 + row0, co0, lane);
     }
 }
@@ -518,31 +589,70 @@ int bsw_tc_split(bsw_model *m, const float *in, int which, int64_t n, cudaStream
     return BSW_OK;
 }
 
-// Which grid the convolutions run on: a bit mask -- 1 / 2 = dense 3x3 / 5x5, 4 = in-convs and heads on a persistent grid
-// (one CTA per SM walking the tiles, the TMA ring prefetching across tile boundaries); a clear bit means one CTA per tile.
-// Default 7 (BSW_TC_PERSIST overrides).  Same kernel, same k order per tile: results are bit-identical in every mode.
+// Launch shape of the convolutions, a bit mask -- 1 / 2 = dense 3x3 / 5x5, 4 = in-convs and heads on a persistent grid
+// (one CTA or cluster per SM / cluster slot walking the tiles, the TMA ring prefetching across tile boundaries); a clear
+// bit means one CTA per tile.  8 = the dense convs and in-convs without TMA multicast: single CTAs, each loading its whole
+// stage.  Default 7 (BSW_TC_PERSIST overrides).  Same tiles, same k order per tile: results are bit-identical in every mode.
 static int g_tc_mode = -1;
-static bool tc_persistent(int which) {
+static int tc_mode() {
     static const int env = getenv("BSW_TC_PERSIST") ? atoi(getenv("BSW_TC_PERSIST")) : 7;
-    return (((g_tc_mode < 0) ? env : g_tc_mode) & which) != 0;
+    return (g_tc_mode < 0) ? env : g_tc_mode;
 }
+static bool tc_persistent(int which) { return (tc_mode() & which) != 0; }
 extern "C" int bsw_set_conv_mode(int mode) {
-    BSW_REQUIRE(mode >= -1 && mode <= 7, "bsw_set_conv_mode: -1 (default) or a mask of 1 | 2 | 4 (persistent grid: dense 3x3, 5x5, in-convs and heads)");
+    BSW_REQUIRE(mode >= -1 && mode <= 15, "bsw_set_conv_mode: -1 (default) or a mask of 1 | 2 | 4 (persistent grid: dense 3x3, 5x5, "
+                                          "in-convs and heads) | 8 (no TMA multicast)");
     g_tc_mode = mode;
     return BSW_OK;
+}
+static int cur_device() {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    return (dev < 0 || dev >= 64) ? 0 : dev;
 }
 static unsigned tc_grid(int ntiles, bool persistent) {   // one CTA per tile, or one per SM of the current device
     static int sms[64] = {0};
     if (!persistent) return (unsigned)ntiles;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) dev = 0;
+    const int dev = cur_device();
     if (!sms[dev]) {
         int v = 0;
         cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
         sms[dev] = v > 0 ? v : 132;
     }
     return (unsigned)(ntiles < sms[dev] ? ntiles : sms[dev]);
+}
+
+// Dense convs and in-convs: one four-CTA cluster per image (TMA multicast, see k_conv_wg), or single CTAs with mode bit 8.
+// The persistent grid is as many clusters as the device holds at once (GPCs of 16-18 SMs leave some SMs out), cluster c
+// walking images c, c + C, ...
+static int launch_tc(const CUtensorMap &amap_hi, const CUtensorMap &amap_lo, const TcSlot &s, const TcArgs &t, int64_t n,
+                     bool persistent, cudaStream_t st) {
+    static int clusters[64] = {0};
+    const int ntiles = (int)n * 2 * TcArgs::kCoBlocks;
+    const bool mc = (tc_mode() & 8) == 0;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = 4; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)ntiles);
+    cfg.blockDim = dim3(WG_THREADS);
+    cfg.dynamicSmemBytes = TileCfg<BN>::SMEM;
+    cfg.stream = st;
+    cfg.attrs = &attr;
+    cfg.numAttrs = mc ? 1 : 0;
+    if (persistent && !mc) cfg.gridDim = dim3(tc_grid(ntiles, true));
+    if (persistent && mc) {
+        const int dev = cur_device();
+        if (!clusters[dev]) {
+            int v = 0;
+            BSW_CUDA(cudaOccupancyMaxActiveClusters(&v, k_conv_wg<TcArgs>, &cfg));
+            BSW_REQUIRE(v > 0, "launch_tc: a cluster of four conv CTAs does not fit this device");
+            clusters[dev] = v;
+        }
+        cfg.gridDim = dim3(4u * (unsigned)(n < clusters[dev] ? n : clusters[dev]));
+    }
+    BSW_CUDA(cudaLaunchKernelEx(&cfg, k_conv_wg<TcArgs>, amap_hi, amap_lo, s.map_hi, s.map_lo, t, ntiles));
+    return BSW_OK;
 }
 
 // a.in must be one of the plane buffers: a.in_planes = 0/1 selects it; outputs a.A_planes = 0/1/-1.
@@ -557,11 +667,7 @@ int bsw_conv_tc(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t n, c
     t.A_hi = a.A_planes >= 0 ? ts->act[a.A_planes][0] : nullptr;
     t.A_lo = a.A_planes >= 0 ? ts->act[a.A_planes][1] : nullptr;
     t.A_elu = a.A_elu;
-    const int ntiles = (int)n * 2 * TcArgs::kCoBlocks;
-    k_conv_wg<TcArgs><<<tc_grid(ntiles, tc_persistent(c.ks <= 3 ? 1 : 2)), WG_THREADS, TileCfg<BN>::SMEM, st>>>(
-        ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1], s.map_hi, s.map_lo, t, ntiles);
-    BSW_LAUNCH_CHECK();
-    return BSW_OK;
+    return launch_tc(ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1], s, t, n, tc_persistent(c.ks <= 3 ? 1 : 2), st);
 }
 
 // Heads: reads the planes the last ResNet conv wrote (in_planes), writes mu / sigma.  BSW_TC_HEADS=0 keeps the float32 SIMT
@@ -600,10 +706,7 @@ int bsw_conv_tc_in(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t n
     t.A_hi = a.A_planes >= 0 ? ts->act[a.A_planes][0] : nullptr;
     t.A_lo = a.A_planes >= 0 ? ts->act[a.A_planes][1] : nullptr;
     t.A_elu = a.A_elu;
-    const int ntiles = (int)n * 2 * TcArgs::kCoBlocks;
-    k_conv_wg<TcArgs><<<tc_grid(ntiles, tc_persistent(4)), WG_THREADS, TileCfg<BN>::SMEM, st>>>(
-        ts->inp_map[0], ts->inp_map[1], s.map_hi, s.map_lo, t, ntiles);
-    BSW_LAUNCH_CHECK();
+    if (int rc = launch_tc(ts->inp_map[0], ts->inp_map[1], s, t, n, tc_persistent(4), st)) return rc;
     *launches += 2;
     return BSW_OK;
 }

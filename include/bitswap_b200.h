@@ -183,8 +183,10 @@ int bsw_rows6_set_verify(int on);
  * rows per warp).  Every setting emits the same integers; exposed for A/B timing and the parity test. */
 int bsw_rows6_set_lanes_per_row(int lpr);
 /* Launch shape of the tensor-core convolutions, a bit mask: 1 / 2 / 4 = dense 3x3 / dense 5x5 / in-convs and heads on a
- * persistent grid (one CTA per SM walking half-image tiles); a clear bit = one CTA per tile.  -1 = default
- * (BSW_TC_PERSIST if set, else 7).  Bit-identical results. */
+ * persistent grid (one CTA per SM, or one four-CTA cluster per four SMs, walking half-image tiles); a clear bit = one
+ * CTA per tile.  8 = dense convs and in-convs as single CTAs without TMA multicast (by default each image's four tiles
+ * run as one cluster sharing their operand loads).  -1 = default (BSW_TC_PERSIST if set, else 7).  Bit-identical
+ * results. */
 int bsw_set_conv_mode(int mode);
 int bsw_rows6_verify_read(uint64_t *out4_host);
 int bsw_logistic_push_2p(bsw_streams *s, int first, int count, const float *mu_dev, int64_t mu_stream_stride,

@@ -1,0 +1,49 @@
+"""The dense convs and in-convs run as one four-CTA cluster per image that share their operand loads by TMA multicast.
+Every CTA still computes the same tile with the same k order and MMAs, so mu/sigma must be bit-identical to the
+single-CTA launches (conv mode bit 8) on both grids."""
+import numpy as np
+import pytest
+import torch
+
+pytestmark = pytest.mark.gpu
+
+from bitswap_b200 import synthetic                   # noqa: E402
+from bitswap_b200.config import CodecConfig          # noqa: E402
+from bitswap_b200.model import Model                 # noqa: E402
+from bitswap_b200._lib import lib, check             # noqa: E402
+
+NO_MULTICAST = 8
+
+
+@pytest.mark.parametrize("B", [170, 1])
+def test_multicast_clusters_equal_single_cta_convs(B):
+    """Per-tile grid (mode 0) and persistent grid (mode 7), each with and without multicast, over every conv shape on the
+    path: in-convs with 1 and 25 taps, dense 3x3, 5x5 and the heads.  B = 170 leaves some clusters of the persistent grid
+    one image more than others; B = 1 is a single cluster."""
+    cfg = CodecConfig(xs=(3, 32, 32), nz=2, zchannels=8, nprocessing=1, resdepth=1, reswidth=252)
+    sd = synthetic.synthetic_state_dict(cfg, seed=61, varied=True)
+    m = Model.from_config(cfg, max_batch=B, use_tensor_cores=True).load_state_dict(sd)
+    m.compress()
+    rs = np.random.RandomState(5)
+    gx = torch.from_numpy((rs.randint(0, 256, (B, cfg.xdim)) - 127.5) / 127.5).cuda()
+    gz = torch.from_numpy(rs.uniform(-5, 5, (B, cfg.zdim))).cuda()
+    out = {}
+    try:
+        for grid in (0, 7):
+            for mode in (grid, grid | NO_MULTICAST):
+                check(lib().bsw_set_conv_mode(mode))
+                res = []
+                for i in range(cfg.nz):
+                    mu, sc = m.infer(i)(gx if i == 0 else gz)
+                    res += [mu.clone(), sc.clone()]
+                    mu, sc = m.generate(i)(gz)
+                    res += [mu.clone(), sc.clone()]
+                torch.cuda.synchronize()
+                out[mode] = res
+    finally:
+        check(lib().bsw_set_conv_mode(-1))
+    for grid in (0, 7):
+        for a, b in zip(out[grid], out[grid | NO_MULTICAST]):
+            assert torch.equal(a, b), f"conv mode {grid} with and without multicast"
+        assert all(torch.isfinite(t).all() for t in out[grid])
+
