@@ -145,6 +145,7 @@ def _set_argtypes(L):
         "bsw_discretize_edges": [P, I, I, P, L64, P, L64, P],
         "bsw_selftest_cdf": [L64, U64, P, P],
         "bsw_selftest_cdf_apx": [L64, U64, P],
+        "bsw_selftest_conv": [P, ctypes.c_char_p, P, L64, I, P, P, P, P, P, P],
     }
     for name, args in sig.items():
         fn = getattr(L, name, None)
@@ -152,7 +153,7 @@ def _set_argtypes(L):
             fn.argtypes = args
 
 
-EXPORTS = ["bsw_last_error", "bsw_version", "bsw_has_tensor_cores", "bsw_measure_fp64_peak", "bsw_selftest_cdf", "bsw_selftest_cdf_apx", "bsw_streams_create", "bsw_streams_destroy", "bsw_streams_count",
+EXPORTS = ["bsw_last_error", "bsw_version", "bsw_has_tensor_cores", "bsw_measure_fp64_peak", "bsw_selftest_cdf", "bsw_selftest_cdf_apx", "bsw_selftest_conv", "bsw_streams_create", "bsw_streams_destroy", "bsw_streams_count",
            "bsw_streams_capacity", "bsw_streams_import", "bsw_streams_fill", "bsw_streams_sizes", "bsw_streams_min_words", "bsw_streams_rest_words", "bsw_streams_export",
            "bsw_streams_device_ptrs", "bsw_streams_pack", "bsw_streams_unpack", "bsw_streams_pack_trimmed", "bsw_streams_unpack_trimmed", "bsw_streams_total_words", "bsw_ans_tables", "bsw_ans_push", "bsw_ans_pop",
            "bsw_logistic_pmfs", "bsw_logistic_tables", "bsw_logistic_push", "bsw_logistic_pop", "bsw_logistic_scratch_bytes", "bsw_set_rows_mode", "bsw_bins_level_is_uniform", "bsw_rows6_set_verify", "bsw_rows6_verify_read", "bsw_rows6_set_lanes_per_row", "bsw_set_conv_mode", "bsw_logistic_push_2p",

@@ -428,6 +428,46 @@ __global__ void k_broadcast_rows(const float *__restrict__ src, float *__restric
     if (i < n * dim) dst[i] = src[i % dim];
 }
 
+enum { ROLE_IN = 0, ROLE_DENSE = 1, ROLE_HEAD = 2 };
+
+// Which path a net's convs take.  On the tensor-core path the dense convs read and write bf16 hi/lo planes, so the
+// in-conv of a net with ResNet layers writes the first layer's planes (on the tensor cores, or SIMT + split when it has
+// more than 32 input channels).  The head reads the planes the last ResNet conv wrote when it fits the tensor-core head
+// (<= 32 outputs); otherwise it runs SIMT on the float32 trunk.
+static bool net_on_tc(const bsw_model *m) { return m->d.use_tensor_cores && m->tc_ready; }
+static bool in_writes_planes(const bsw_model *m, const NetPlan &np) { return net_on_tc(m) && !np.blocks.empty(); }
+static bool head_on_tc(bsw_model *m, const NetPlan &np) {
+    return in_writes_planes(m, np) && bsw_conv_tc_head_available(m, m->convs[np.head]);
+}
+
+// Runs one conv of net `np` in its role: the one place that picks its kernel(s).  `a` holds the input, the epilogue and,
+// for the tensor-core kernels, the plane buffers read (in_planes) and written (A_planes).
+static int dispatch_conv(bsw_model *m, const NetPlan &np, int role, const ConvSlot &c, ConvArgs a, int64_t n,
+                         cudaStream_t st, int *launches) {
+    if (role == ROLE_IN) {
+        if (in_writes_planes(m, np) && c.tc_index >= 0) {
+            // tensor-core in-conv: the trunk in float32, the first layer's input straight into the bf16 planes
+            a.A = nullptr; a.A_planes = 0;
+            return bsw_conv_tc_in(m, c, a, n, st, launches);
+        }
+        if (int rc = bsw_conv_simt(a, c.ks, n, st)) return rc;
+        ++*launches;
+        if (in_writes_planes(m, np)) {           // conv-input planes for the tensor-core layers: A -> bf16 hi/lo
+            if (int rc = bsw_tc_split(m, a.A, 0, n, st)) return rc;
+            ++*launches;
+        }
+        return BSW_OK;
+    }
+    const bool tc = role == ROLE_DENSE ? net_on_tc(m) : head_on_tc(m, np);
+    int rc;
+    if (!tc) rc = bsw_conv_simt(a, c.ks, n, st);
+    else if (role == ROLE_DENSE) rc = bsw_conv_tc(m, c, a, n, st);
+    else rc = bsw_conv_tc_head(m, c, a, n, st);
+    if (rc) return rc;
+    ++*launches;
+    return BSW_OK;
+}
+
 static int run_net(bsw_model *m, const NetPlan &np, const float *given, int64_t n, float *mu, float *scale,
                    cudaStream_t st, int *launches, BswProf *prof) {
     BswProf noprof;
@@ -436,9 +476,8 @@ static int run_net(bsw_model *m, const NetPlan &np, const float *given, int64_t 
     BSW_REQUIRE(n >= 1 && n <= m->d.max_batch, "batch exceeds the model's max_batch");
     const int Wp = m->Wp;
     const bool has_blocks = !np.blocks.empty();
-    const bool use_tc = m->d.use_tensor_cores && m->tc_ready;
     // heads on the tensor cores: they read the trunk as bf16 planes, which the last ResNet conv then has to write
-    const bool tc_head = use_tc && has_blocks && bsw_conv_tc_head_available(m, m->convs[np.head]);
+    const bool tc_head = head_on_tc(m, np);
     float *T = m->bufT, *A = m->bufA, *B = m->bufB;
     {   // in-conv
         const ConvSlot &c = m->convs[np.in_conv];
@@ -447,18 +486,7 @@ static int run_net(bsw_model *m, const NetPlan &np, const float *given, int64_t 
         a.w = c.w; a.bias = c.bias; a.CoutP = c.CoutP;
         a.out_mode = OUT_NHWC; a.T = T; a.T_elu = 1; a.A = has_blocks ? A : nullptr; a.A_elu = 1;
         prof->begin(CAT_CONV_IN, st);
-        if (use_tc && has_blocks && c.tc_index >= 0) {
-            // tensor-core in-conv: the trunk in float32, the first layer's input straight into the bf16 planes
-            a.A = nullptr; a.A_planes = 0;
-            if (int rc = bsw_conv_tc_in(m, c, a, n, st, launches)) return rc;
-        } else {
-            if (int rc = bsw_conv_simt(a, c.ks, n, st)) return rc;
-            ++*launches;
-            if (use_tc && has_blocks) {          // conv-input planes for the tensor-core layers: A -> bf16 hi/lo
-                if (int rc = bsw_tc_split(m, A, 0, n, st)) return rc;
-                ++*launches;
-            }
-        }
+        if (int rc = dispatch_conv(m, np, ROLE_IN, c, a, n, st, launches)) return rc;
         prof->end(st);
     }
     for (size_t bi = 0; bi < np.blocks.size(); ++bi) {
@@ -480,13 +508,9 @@ static int run_net(bsw_model *m, const NetPlan &np, const float *given, int64_t 
                     a.in_planes = 1; a.A_planes = (last_layer && last_block) ? -1 : 0;
                     if (last_layer && last_block && tc_head) { a.A_planes = 0; a.A_elu = 0; }     // planes = the trunk itself (already ELU'd)
                 }
-                int rc;
                 prof->begin(c.ks == 5 ? CAT_CONV_DENSE5 : CAT_CONV_DENSE3, st);
-                if (use_tc) rc = bsw_conv_tc(m, c, a, n, st);
-                else rc = bsw_conv_simt(a, c.ks, n, st);
-                if (rc) return rc;
+                if (int rc = dispatch_conv(m, np, ROLE_DENSE, c, a, n, st, launches)) return rc;
                 prof->end(st);
-                ++*launches;
             }
         }
     }
@@ -499,10 +523,86 @@ static int run_net(bsw_model *m, const NetPlan &np, const float *given, int64_t 
         a.scale_kind = np.scale_kind; a.out_dim = np.out_dim;
         prof->begin(CAT_CONV_HEAD, st);
         a.in_planes = 0;
-        if (tc_head) { if (int rc = bsw_conv_tc_head(m, c, a, n, st)) return rc; }
-        else if (int rc = bsw_conv_simt(a, c.ks, n, st)) return rc;
+        if (int rc = dispatch_conv(m, np, ROLE_HEAD, c, a, n, st, launches)) return rc;
         prof->end(st);
-        ++*launches;
+    }
+    return BSW_OK;
+}
+
+// Test hook: one conv of a loaded model through dispatch_conv, with the epilogue selected by `flags`.  The conv's role
+// and net come from the model's plans; a head is named by its mu prefix.  Tensor-core dense convs and heads read plane
+// buffer 0, split from in_dev here by the same RNE split the epilogues use; dense convs write plane buffer 1, in-convs
+// plane buffer 0.  The written buffer is filled with 0xffff first and copied whole ([2][max_batch,256,256]) to
+// planes_dev, so rows the conv must not touch can be checked.
+extern "C" int bsw_selftest_conv(bsw_model *m, const char *prefix, const float *in_dev, int64_t n, int flags, float *T_dev,
+                                 float *A_dev, uint16_t *planes_dev, float *mu_dev, float *scale_dev, void *stream) {
+    BSW_REQUIRE(m && prefix && in_dev, "bsw_selftest_conv: null argument");
+    BSW_REQUIRE(m->finalized, "model not finalized");
+    BSW_REQUIRE(n >= 1 && n <= m->d.max_batch, "batch exceeds the model's max_batch");
+    BSW_REQUIRE((flags & ~(BSW_CONV_RESID | BSW_CONV_T | BSW_CONV_T_ELU | BSW_CONV_A | BSW_CONV_A_ELU)) == 0,
+                "bsw_selftest_conv: unknown flags");
+    auto it = m->names.find(prefix);
+    if (it == m->names.end() || it->second.co_off != 0) {
+        bsw_set_error("bsw_selftest_conv: '%s' names no conv of this model (heads go by their mu prefix)", prefix);
+        return BSW_E_INVALID;
+    }
+    const int slot = it->second.slot;
+    const NetPlan *np = nullptr;
+    int role = -1;
+    for (const std::vector<NetPlan> *nets : {&m->infer, &m->gen})
+        for (const NetPlan &p : *nets) {
+            if (p.in_conv == slot) { np = &p; role = ROLE_IN; }
+            if (p.head == slot) { np = &p; role = ROLE_HEAD; }
+            for (const BlockPlan &bp : p.blocks)
+                for (const auto &l : bp.layers)
+                    if (l.first == slot || l.second == slot) { np = &p; role = ROLE_DENSE; }
+        }
+    BSW_REQUIRE(np, "bsw_selftest_conv: the conv is in no net");
+    const ConvSlot &c = m->convs[slot];
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t plane_bytes = (size_t)m->d.max_batch * 256 * 256 * sizeof(uint16_t);
+    ConvArgs a = {};
+    a.Cin = c.Cin; a.CinP = c.CinP; a.w = c.w; a.bias = c.bias; a.CoutP = c.CoutP;
+    a.in = in_dev; a.in_planes = 0; a.A_planes = -1;
+    int out_planes = -1, launches = 0;
+    if (role == ROLE_HEAD) {
+        BSW_REQUIRE(mu_dev && (scale_dev || np->n_sc == 0), "bsw_selftest_conv: head outputs required");
+        a.in_mode = IN_NHWC; a.ld_in = m->Wp;
+        a.out_mode = np->out_mode; a.mu = mu_dev; a.scale = scale_dev; a.n_mu = np->n_mu; a.n_sc = np->n_sc;
+        a.scale_kind = np->scale_kind; a.out_dim = np->out_dim;
+        if (head_on_tc(m, *np))
+            if (int rc = bsw_tc_split(m, in_dev, 0, n, st)) return rc;
+    } else {
+        BSW_REQUIRE(T_dev || !(flags & (BSW_CONV_RESID | BSW_CONV_T)), "bsw_selftest_conv: T_dev required");
+        a.out_mode = OUT_NHWC;
+        a.resid = (flags & BSW_CONV_RESID) ? T_dev : nullptr;           // in place, as run_net does
+        a.T = (flags & BSW_CONV_T) ? T_dev : nullptr; a.T_elu = (flags & BSW_CONV_T_ELU) ? 1 : 0;
+        a.A = (flags & BSW_CONV_A) ? (A_dev ? A_dev : m->bufA) : nullptr; a.A_elu = (flags & BSW_CONV_A_ELU) ? 1 : 0;
+        if (role == ROLE_IN) {
+            a.in_mode = np->in_mode; a.in_dim = np->in_dim; a.ld_in = 0;
+            if (in_writes_planes(m, *np)) {
+                BSW_REQUIRE(flags & BSW_CONV_A, "bsw_selftest_conv: this in-conv writes the first layer's input (BSW_CONV_A)");
+                out_planes = 0;
+            }
+        } else {
+            a.in_mode = IN_NHWC; a.ld_in = m->Wp;
+            if (net_on_tc(m)) {
+                if (int rc = bsw_tc_split(m, in_dev, 0, n, st)) return rc;
+                if (flags & BSW_CONV_A) out_planes = a.A_planes = 1;
+            }
+        }
+    }
+    void *hi = nullptr, *lo = nullptr;
+    if (out_planes >= 0) {
+        BSW_REQUIRE(planes_dev, "bsw_selftest_conv: planes_dev required on the tensor-core path");
+        bsw_tc_planes(m, out_planes, &hi, &lo);
+        BSW_CUDA(cudaMemsetAsync(hi, 0xff, plane_bytes, st));
+        BSW_CUDA(cudaMemsetAsync(lo, 0xff, plane_bytes, st));
+    }
+    if (int rc = dispatch_conv(m, *np, role, c, a, n, st, &launches)) return rc;
+    if (out_planes >= 0) {
+        BSW_CUDA(cudaMemcpyAsync(planes_dev, hi, plane_bytes, cudaMemcpyDeviceToDevice, st));
+        BSW_CUDA(cudaMemcpyAsync((char *)planes_dev + plane_bytes, lo, plane_bytes, cudaMemcpyDeviceToDevice, st));
     }
     return BSW_OK;
 }

@@ -107,4 +107,5 @@ int bsw_conv_tc(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t n, c
 bool bsw_conv_tc_head_available(bsw_model *m, const ConvSlot &c);
 int bsw_conv_tc_head(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t n, cudaStream_t st);
 int bsw_tc_split(bsw_model *m, const float *in, int which, int64_t n, cudaStream_t st);
+void bsw_tc_planes(bsw_model *m, int which, void **hi, void **lo);
 int bsw_conv_tc_in(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t n, cudaStream_t st, int *launches);

@@ -46,6 +46,26 @@ int         bsw_measure_fp64_peak(double *dfma_per_s);
 int         bsw_selftest_cdf(int64_t n, uint64_t seed, int64_t *mismatches_host, double *example_host);
 /* worst |screening cdf - exact cdf| over n random arguments, in units of 2^-51 (the screening window is 64 units) */
 int         bsw_selftest_cdf_apx(int64_t n, uint64_t seed, double *worst_units_host);
+/* Test hook: runs ONE conv of a finalized model -- the one loaded under the state_dict prefix `prefix`; a head goes by
+ * its mu prefix ("infer_mu", "deepgen_mu.0.0", "gen_mu.0") -- for images [0, n), through the same per-conv dispatch
+ * as bsw_vae_*: tensor-core dense conv / in-conv / head, SIMT in-conv followed by the bf16 split, or SIMT head after a
+ * tensor-core trunk.  The role comes from the model's net plans.
+ *   in_dev:  flat CHW `given` [n, dim] for in-convs; float32 NHWC [n,256,Wp] for dense convs and heads (padded
+ *            channels zero).  On the tensor-core path it is split into the input planes as bsw_vae_* splits the trunk.
+ *   flags:   epilogue of in-convs and dense convs, r = conv + bias: BSW_CONV_RESID r += T_dev (the residual, updated in
+ *            place), BSW_CONV_T writes T_dev = (T_ELU ? ELU(r) : r), BSW_CONV_A writes the next conv's input
+ *            (A_ELU ? ELU(T) : T) to A_dev (SIMT; NULL = an internal buffer) or to bf16 hi/lo planes (tensor cores).
+ *   T_dev, A_dev: float32 [n,256,Wp].  planes_dev: uint16 [2][max_batch,256,256] (hi, lo) receives the whole plane
+ *            buffer the conv wrote, pre-filled with 0xffff; tensor-core path with BSW_CONV_A only.
+ *   mu_dev, scale_dev: head outputs [n, dim_out] flat CHW, as bsw_vae_* returns them (scale only with a scale head). */
+#define BSW_CONV_RESID 1
+#define BSW_CONV_T     2
+#define BSW_CONV_T_ELU 4
+#define BSW_CONV_A     8
+#define BSW_CONV_A_ELU 16
+int         bsw_selftest_conv(struct bsw_model *m, const char *prefix, const float *in_dev, int64_t n, int flags,
+                              float *T_dev, float *A_dev, uint16_t *planes_dev, float *mu_dev, float *scale_dev,
+                              void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Stream sets: B device-resident ANS states.

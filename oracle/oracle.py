@@ -244,14 +244,48 @@ def _unsqueeze2(x):    # modules.py:198-208
     return x.view(n, c // 4, 2, 2, h, w).permute(0, 1, 4, 2, 5, 3).reshape(n, c // 4, h * 2, w * 2)
 
 
+def fold_wn(sd, prefix, loggain=True):
+    """The float32 kernel and bias the product folds at load (bsw_model_load_conv): ||v|| summed in float64 and rounded
+    to float32, g = softplus(gain) in float64 rounded to float32, then w = v * (g / (||v|| + 1e-10)) in float32."""
+    v = sd[prefix + ".v"].detach().cpu().numpy().astype(np.float32)
+    gain = sd[prefix + ".gain"].detach().cpu().numpy().astype(np.float32)
+    vnorm = np.sqrt((v.reshape(v.shape[0], -1).astype(np.float64) ** 2).sum(1)).astype(np.float32)
+    g = gain.astype(np.float64)
+    g = (np.maximum(g, 0.0) + np.log1p(np.exp(-np.abs(g)))).astype(np.float32) if loggain else gain
+    scale = g / (vnorm + np.float32(1e-10))
+    w = v * scale.astype(np.float32)[:, None, None, None]
+    return torch.from_numpy(w.astype(np.float32)), sd[prefix + ".b"].detach().cpu().float()
+
+
+def conv_f64(x, w, b=None):
+    """One "same" convolution in float64, and the l2 norm of its products: (y, s) with y = conv(x, w) + b and
+    s = sqrt(sum_k (x_k w_k)^2 + b^2) per output element, the scale a correctly rounded float32-accurate conv is held to
+    (normalising by s rather than |y| keeps outputs where the terms cancel testable)."""
+    x, w = x.double(), w.double().to(x.device)
+    pad = (w.shape[-1] - 1) // 2
+    y = F.conv2d(x, w, None, padding=pad)
+    s2 = F.conv2d(x * x, w * w, None, padding=pad)
+    if b is not None:
+        b = b.double().to(x.device).view(1, -1, 1, 1)
+        y, s2 = y + b, s2 + b * b
+    return y, s2.sqrt()
+
+
 class ModelOracle:
     """infer(i)(given) / generate(i)(given) of the reference Model in
     compressing mode, batched over a leading dimension: given [B, dim] (any
-    float dtype, flat CHW) -> (mu, scale) float64 [B, dim_out]."""
+    float dtype, flat CHW) -> (mu, scale) float64 [B, dim_out].
 
-    def __init__(self, cfg, state_dict):
-        self.cfg = cfg
-        self.sd = {k: v.float() for k, v in state_dict.items()}
+    dtype is the arithmetic: float32 (default, the reference's own) or float64, a reference for the float32 kernels
+    whose own error is far below theirs.  The input is first rounded to float32, as `given.float()` in the reference
+    and the product do.  device places the computation (and the outputs), e.g. "cuda" for large float64 batches."""
+
+    def __init__(self, cfg, state_dict, dtype=torch.float32, device="cpu"):
+        self.cfg, self.dtype, self.device = cfg, dtype, torch.device(device)
+        self.sd = {k: v.float().to(device=self.device, dtype=dtype) for k, v in state_dict.items()}
+
+    def _given(self, given):
+        return given.float().to(device=self.device, dtype=self.dtype)
 
     @torch.no_grad()
     def infer(self, i):
@@ -259,7 +293,7 @@ class ModelOracle:
         rd = cfg.level_resdepth
 
         def distribution(given):
-            h = given.float()
+            h = self._given(given)
             if i == 0:                                           # cifar_train.py:326-349
                 h = h.view((-1,) + tuple(cfg.xs))
                 h = F.elu(_conv(sd, "infer_in.1", _squeeze2(h)))
@@ -286,7 +320,7 @@ class ModelOracle:
         rd = cfg.level_resdepth
 
         def distribution(given):
-            h = given.float().view(-1, cfg.zchannels, 16, 16)    # :391-393
+            h = self._given(given).view(-1, cfg.zchannels, 16, 16)    # :391-393
             if i == 0:                                           # :396-411
                 h = F.elu(_conv(sd, "gen_in.0", h))
                 if rd[0] > 0:

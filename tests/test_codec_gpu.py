@@ -189,12 +189,12 @@ def test_p4_roundtrip_sub_range_and_chain_independence():
 from bitswap_b200.config import CodecConfig          # noqa: E402
 
 
-def _tc_case(cfg, B, seed=4):
+def _tc_case(cfg, B, seed=4, dtype=torch.float32):
     sd = synthetic.synthetic_state_dict(cfg, seed=50, varied=True)
     m_tc = Model.from_config(cfg, max_batch=B, use_tensor_cores=True).load_state_dict(sd)
     m_si = Model.from_config(cfg, max_batch=B, use_tensor_cores=False).load_state_dict(sd)
     m_tc.compress(); m_si.compress()
-    orc = O.ModelOracle(cfg, sd)
+    orc = O.ModelOracle(cfg, sd, dtype=dtype)
     rs = np.random.RandomState(seed)
     worst_o = worst_s = 0.0
     for i in range(cfg.nz):
@@ -221,6 +221,23 @@ def _tc_case(cfg, B, seed=4):
 def test_p3_tc_single_layers(label, cfg):
     worst_o, worst_s = _tc_case(cfg, 3)
     print(f"tensor cores {label}: max |err| vs torch-f32 oracle {worst_o:.2e}, vs SIMT f32 path {worst_s:.2e}")
+    assert worst_o < TOL and worst_s < TOL
+
+
+@pytest.mark.parametrize("label,cfg", [
+    ("zchannels 20: SIMT heads after a tensor-core trunk",
+     CodecConfig(xs=(3, 32, 32), nz=2, zchannels=20, nprocessing=1, resdepth=2, reswidth=252)),
+    ("zchannels 40: SIMT in-conv + k_split_planes, SIMT heads",
+     CodecConfig(xs=(3, 32, 32), nz=2, zchannels=40, nprocessing=1, resdepth=2, reswidth=252)),
+    ("nz 4, resdepth 2: levels without ResNet layers",
+     CodecConfig(xs=(3, 32, 32), nz=4, zchannels=8, nprocessing=1, resdepth=2, reswidth=252)),
+    ("width 193", CodecConfig(xs=(3, 32, 32), nz=2, zchannels=8, nprocessing=1, resdepth=2, reswidth=193)),
+    ("width 255", CodecConfig(xs=(3, 32, 32), nz=2, zchannels=8, nprocessing=1, resdepth=2, reswidth=255, cond_xscale=True)),
+])
+def test_p3_tc_dispatch_seams_vs_f64_oracle(label, cfg):
+    """Whole nets at the dispatch seams of run_net on a tensor-core model, against the float64 oracle."""
+    worst_o, worst_s = _tc_case(cfg, 3, dtype=torch.float64)
+    print(f"tensor cores {label}: max |err| vs torch-f64 oracle {worst_o:.2e}, vs SIMT f32 path {worst_s:.2e}")
     assert worst_o < TOL and worst_s < TOL
 
 
