@@ -14,12 +14,15 @@
 //     each k-block issues three MMAs: hi*hi into a MAIN float32 accumulator, hi*lo and lo*hi into a
 //     separate CROSS accumulator.  The tensor core truncates on every accumulate; keeping the 2^-8 smaller
 //     cross terms out of the main accumulator cuts its truncating adds 3x.
-//   * warp roles: warps 0..7 = two consumer warpgroups, each owning 64 of the tile's 128 pixels and issuing
-//     wgmma.m64nNk16 from shared memory into register accumulators ({main, cross} x N/2 floats per thread),
-//     then running the epilogue (bias / residual / ELU / bf16 split -> HBM) straight from those registers;
-//     warp 8 = TMA producer (one elected lane) feeding an NSTAGE ring of mbarrier-guarded stages.
+//   * warp roles (384 threads): warps 0..7 = two consumer warpgroups, each owning 64 of the tile's 128 pixels and
+//     issuing wgmma.m64nNk16 from shared memory into register accumulators ({main, cross} x N/2 floats per thread);
+//     after the last k-block they write main + cross into an fp32 hand-off tile in shared memory and go on with the
+//     next tile.  Warp 8 = TMA producer (one elected lane) feeding an NSTAGE ring of mbarrier-guarded stages; warps
+//     9..11 = epilogue (bias / residual / ELU / bf16 split -> HBM) from the hand-off tile.  setmaxnreg gives the
+//     consumers 160 registers and the producer / epilogue warpgroup 64.
 //   * a CTA walks tiles t = blockIdx.x, + gridDim.x, ...: with one CTA per tile (per-tile grid) or one per SM
-//     (persistent grid, the producer then prefetches the next tile's k-blocks while the consumers run the epilogue).
+//     (persistent grid: the producer prefetches the next tile's k-blocks and the consumers run its MMAs while the
+//     epilogue warps store the previous tile).
 //   * the dense convs and in-convs run as four-CTA clusters, one image per cluster, CTA rank r = tile t & 3 =
 //     (pixel half r & 1, channel block r >> 1): the two channel blocks of a pixel half read the same A boxes, the two
 //     pixel halves of a channel block the same W boxes.  Each CTA issues two of a stage's four boxes with TMA multicast
@@ -44,16 +47,24 @@ constexpr int MT = 128;                     // pixels per tile: two warpgroups x
 constexpr int BN = 128;                     // output channels per tile of the W->W convs and in-convs
 constexpr int HD_N = 32;                    // output channels of the heads (n_mu + n_sc <= 32, zero padded)
 constexpr int A_BYTES = MT * BK * 2;        // one 128-row x 32-col bf16 activation tile = 8 KB
-constexpr int WG_THREADS = 288;             // two consumer warpgroups + one producer warp
+constexpr int WG_THREADS = 384;             // two consumer warpgroups + the producer / epilogue warpgroup
 constexpr int PRODUCER_WARP = 8;
+constexpr int EPI_WARP0 = 9, EPI_WARPS = 3; // warps 9..11: epilogue
+// Registers per thread: 128 at launch (384 x 128 = 48 K of the SM's 64 K, so a coder CTA fits beside a conv CTA), then
+// setmaxnreg moves them from the producer / epilogue warpgroup to the consumers: 256 x 160 + 128 x 64 = 48 K.  Both
+// sides compile without spills at these counts (ptxas -v).
+constexpr int REGS_CONSUMER = 160, REGS_EPILOGUE = 64;
+constexpr int HD_LD = MT + 4;               // heads' hand-off row stride (floats): bank-conflict free both ways
 
 template <int N> struct TileCfg {
     static constexpr int W_BYTES = N * BK * 2;                       // one N-row weight tile
     static constexpr int STAGE = 2 * A_BYTES + 2 * W_BYTES;          // A_hi, A_lo, B_hi, B_lo
-    static constexpr int NSTAGE = 6;                                 // 192 KB (N = 128) / 120 KB (N = 32) of stages
-    static constexpr int SMEM = NSTAGE * STAGE + 1024 /*align*/ + 256 /*barriers*/;
+    static constexpr int NSTAGE = N == BN ? 4 : 5;                   // 128 KB (N = 128) / 100 KB (N = 32) of stages
+    // fp32 hand-off tile (main + cross) from the consumers to the epilogue warps: 64 KB (N = 128) / 16.5 KB (N = 32)
+    static constexpr int HAND = N == BN ? MT * N * 4 : N * HD_LD * 4;
+    static constexpr int SMEM = NSTAGE * STAGE + HAND + 1024 /*align*/ + 256 /*barriers*/;
 };
-static_assert(TileCfg<BN>::SMEM <= 227 * 1024, "stages must fit one H100 SM's shared memory");
+static_assert(TileCfg<BN>::SMEM <= 227 * 1024, "stages and hand-off must fit one H100 SM's shared memory");
 
 struct TcState {
     // bf16 hi/lo activation planes, ping-pong: [max_batch, 256 px, 256 ch]
@@ -221,42 +232,65 @@ struct TcArgs {
     int A_elu;
 };
 
-// Dense / in-conv epilogue from the accumulators: (main + cross) + bias (+ residual) (-> ELU) -> trunk; (-> ELU) -> bf16
-// hi/lo planes of the next conv.  A quad of lanes covers 8 consecutive channels (32 B of the trunk row): every store
-// instruction writes whole sectors.  The residual is the trunk itself (updated in place: resid == T), so its loads are
-// issued explicitly four column groups ahead of the stores that could alias them.  A thread re-reads nothing it has
-// written, so the in-place update stays exact.
-__device__ __forceinline__ void epilogue(const TcArgs &a, const float (&dm)[64], const float (&dc)[64], int img, int prow0,
-                                         int co0, int lane) {
-    const int cl = 2 * (lane & 3);
-    const int64_t base = ((int64_t)img * 256 + prow0) * 256 + co0 + cl;     // + 8h * 256 + 8j
+// Hand-off tile of the dense convs and in-convs: s = main + cross as fp32 [128 px][128 ch], the 32-byte column chunks
+// of row r XOR-swizzled by r & 3.  The consumers' float2 writes (a half warp covers 4 rows x 4 pairs of one chunk) and
+// the epilogue's float4 row reads (8 lanes read 4 whole chunks of one row) then both hit 32 distinct banks.
+__device__ __forceinline__ int hand_idx(int r, int c) { return r * BN + (((c >> 3) ^ (r & 3)) << 3) + (c & 7); }
+
+__device__ __forceinline__ void hand_store(const TcArgs &, float *hand, const float (&dm)[64], const float (&dc)[64], int row,
+                                           int lane) {
 #pragma unroll
-    for (int jb = 0; jb < 16; jb += 4) {
-        float2 q[4][2];
+    for (int j = 0; j < 16; ++j)
 #pragma unroll
-        for (int jj = 0; jj < 4; ++jj)
+        for (int h = 0; h < 2; ++h) {
+            const int i = 4 * j + 2 * h;
+            *reinterpret_cast<float2 *>(hand + hand_idx(row + 8 * h, 8 * j + 2 * (lane & 3))) =
+                make_float2(dm[i] + dc[i], dm[i + 1] + dc[i + 1]);
+        }
+}
+
+// Dense / in-conv epilogue, run by the epilogue warps from the hand-off tile: s + bias (+ residual) (-> ELU) -> trunk;
+// (-> ELU) -> bf16 hi/lo planes of the next conv.  Warp ew takes tile rows ew, ew + 3, ...; lane l channels co0 + 4l..+3,
+// so a warp stores 512 contiguous bytes of the trunk and 256 of each plane per row.  The residual is the trunk itself
+// (updated in place: resid == T): each element is read and then written by the same thread, and the loads of the next
+// RD rows are issued before the current row's stores.
+__device__ __forceinline__ void epilogue(const TcArgs &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
+    constexpr int RD = 3;
+    const float4 bq = __ldg(reinterpret_cast<const float4 *>(a.bias + co0) + lane);
+    const int64_t base = ((int64_t)img * 256 + mh * 128) * 256 + co0 + 4 * lane;     // + r * 256
+    const int nr = (MT - ew + EPI_WARPS - 1) / EPI_WARPS;
+    auto resid = [&](int k) {
+        return (a.resid && k < nr) ? *reinterpret_cast<const float4 *>(a.resid + base + (ew + EPI_WARPS * k) * 256)
+                                   : make_float4(0.f, 0.f, 0.f, 0.f);
+    };
+    float4 q[RD];
 #pragma unroll
-            for (int h = 0; h < 2; ++h)
-                q[jj][h] = a.resid ? *reinterpret_cast<const float2 *>(a.resid + base + h * 8 * 256 + 8 * (jb + jj)) : make_float2(0.f, 0.f);
+    for (int d = 0; d < RD; ++d) q[d] = resid(d);
+    for (int k0 = 0; k0 < nr; k0 += RD) {
 #pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-            const int j = jb + jj;
-            const float2 bq = __ldg(reinterpret_cast<const float2 *>(a.bias + co0 + cl + 8 * j));
+        for (int d = 0; d < RD; ++d) {
+            const int k = k0 + d, r = ew + EPI_WARPS * k;
+            if (k >= nr) break;
+            const float4 rq = q[d];
+            q[d] = resid(k + RD);
+            const float4 s = *reinterpret_cast<const float4 *>(hand + hand_idx(r, 4 * lane));
+            float x[4] = {s.x + bq.x, s.y + bq.y, s.z + bq.z, s.w + bq.w};
+            if (a.resid) { x[0] += rq.x; x[1] += rq.y; x[2] += rq.z; x[3] += rq.w; }
+            if (a.T_elu)
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int i = 4 * j + 2 * h;
-                const int64_t off = base + h * 8 * 256 + 8 * j;
-                float x0 = (dm[i] + dc[i]) + bq.x, x1 = (dm[i + 1] + dc[i + 1]) + bq.y;
-                if (a.resid) { x0 += q[jj][h].x; x1 += q[jj][h].y; }
-                if (a.T_elu) { x0 = elu1(x0); x1 = elu1(x1); }
-                if (a.T) *reinterpret_cast<float2 *>(a.T + off) = make_float2(x0, x1);
-                if (a.A_hi) {
-                    const float y0 = a.A_elu ? elu1(x0) : x0, y1 = a.A_elu ? elu1(x1) : x1;
-                    const __nv_bfloat16 h0 = __float2bfloat16_rn(y0), h1 = __float2bfloat16_rn(y1);
-                    const __nv_bfloat16 l0 = __float2bfloat16_rn(y0 - __bfloat162float(h0)), l1 = __float2bfloat16_rn(y1 - __bfloat162float(h1));
-                    *reinterpret_cast<uint32_t *>(a.A_hi + off) = pack_bf16x2(h0, h1);
-                    *reinterpret_cast<uint32_t *>(a.A_lo + off) = pack_bf16x2(l0, l1);
+                for (int e = 0; e < 4; ++e) x[e] = elu1(x[e]);
+            const int64_t off = base + r * 256;
+            if (a.T) *reinterpret_cast<float4 *>(a.T + off) = make_float4(x[0], x[1], x[2], x[3]);
+            if (a.A_hi) {
+                __nv_bfloat16 hi[4], lo[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const float y = a.A_elu ? elu1(x[e]) : x[e];
+                    hi[e] = __float2bfloat16_rn(y);
+                    lo[e] = __float2bfloat16_rn(y - __bfloat162float(hi[e]));
                 }
+                *reinterpret_cast<uint2 *>(a.A_hi + off) = make_uint2(pack_bf16x2(hi[0], hi[1]), pack_bf16x2(hi[2], hi[3]));
+                *reinterpret_cast<uint2 *>(a.A_lo + off) = make_uint2(pack_bf16x2(lo[0], lo[1]), pack_bf16x2(lo[2], lo[3]));
             }
         }
     }
@@ -284,44 +318,58 @@ __device__ __forceinline__ float hd_scale(float r, int kind) {      // same expr
     return r;
 }
 
-__device__ __forceinline__ void epilogue(const HeadArgs &a, const float (&dm)[16], const float (&dc)[16], int img, int prow0,
-                                         int co0, int lane) {
-    float *mu_row = a.mu + (int64_t)img * a.out_dim;
-    float *sc_row = a.scale ? a.scale + (int64_t)img * a.out_dim : nullptr;
+// Heads' hand-off tile: channel-major [32 ch][HD_LD], so the epilogue's lanes read consecutive pixels of one channel; the
+// row stride of 132 floats also spreads the consumers' writes (8 rows x 4 channels per register) over 32 banks.
+__device__ __forceinline__ void hand_store(const HeadArgs &, float *hand, const float (&dm)[16], const float (&dc)[16], int row,
+                                           int lane) {
 #pragma unroll
     for (int j = 0; j < HD_N / 8; ++j)
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-                const int c = 8 * j + 2 * (lane & 3) + e;
-                if (c >= a.n_mu + a.n_sc) continue;
-                const int p = prow0 + 8 * h, y = p >> 4, x = p & 15;
                 const int i = 4 * j + 2 * h + e;
-                const bool is_mu = c < a.n_mu;
-                const int o = is_mu ? c : c - a.n_mu;
-                float r = (dm[i] + dc[i]) + __ldg(a.bias + co0 + c);
-                if (!is_mu) r = hd_scale(r, a.scale_kind);
-                float *dst = is_mu ? mu_row : sc_row;
-                if (a.out_mode == OUT_HEAD_Z) dst[o * 256 + p] = r;
-                else dst[(o >> 2) * 1024 + (2 * y + ((o >> 1) & 1)) * 32 + 2 * x + (o & 1)] = r;      // UnSqueeze2d, modules.py:205-207
+                hand[(8 * j + 2 * (lane & 3) + e) * HD_LD + row + 8 * h] = dm[i] + dc[i];
             }
+}
+
+// Heads' epilogue: lane = pixel, so the flat CHW stores dst[o * 256 + p] of a warp are coalesced.
+__device__ __forceinline__ void epilogue(const HeadArgs &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
+    float *mu_row = a.mu + (int64_t)img * a.out_dim;
+    float *sc_row = a.scale ? a.scale + (int64_t)img * a.out_dim : nullptr;
+    for (int r = ew * 32 + lane; r < MT; r += EPI_WARPS * 32) {
+        const int p = mh * 128 + r, y = p >> 4, x = p & 15;
+        for (int c = 0; c < a.n_mu + a.n_sc; ++c) {
+            const bool is_mu = c < a.n_mu;
+            const int o = is_mu ? c : c - a.n_mu;
+            float v = hand[c * HD_LD + r] + __ldg(a.bias + co0 + c);
+            if (!is_mu) v = hd_scale(v, a.scale_kind);
+            float *dst = is_mu ? mu_row : sc_row;
+            if (a.out_mode == OUT_HEAD_Z) dst[o * 256 + p] = v;
+            else dst[(o >> 2) * 1024 + (2 * y + ((o >> 1) & 1)) * 32 + 2 * x + (o & 1)] = v;      // UnSqueeze2d, modules.py:205-207
+        }
+    }
 }
 
 // Tile t -> image t / (2 * kCoBlocks), output-channel block, pixel half (t & 1): the tiles of one image run on
 // neighbouring SMs at about the same time, so the activation planes they share come out of L2.
 // Launched as four-CTA clusters (TcArgs only, see the file comment), gridDim.x is a multiple of 4: t & 3 is the CTA's
 // cluster rank and the four CTAs of a cluster walk the same images in step.
+// Each tile's accumulators go through the shared-memory hand-off tile to the epilogue warps, so the consumers start the
+// next tile's MMAs while its epilogue runs: acc_full (256 consumer threads arrive) publishes the tile, acc_empty (96
+// epilogue threads arrive after their last read of it) frees it.
 template <class Args>
-__global__ void __launch_bounds__(WG_THREADS, 1)
+__global__ void __maxnreg__(128)
 k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ CUtensorMap amap_lo,
           const __grid_constant__ CUtensorMap wmap_hi, const __grid_constant__ CUtensorMap wmap_lo, const Args a, int ntiles) {
     constexpr int N = Args::kN;
     using C = TileCfg<N>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t *full_bar = (uint64_t *)(smem + C::NSTAGE * C::STAGE);
+    float *hand = (float *)(smem + C::NSTAGE * C::STAGE);
+    uint64_t *full_bar = (uint64_t *)(smem + C::NSTAGE * C::STAGE + C::HAND);
     uint64_t *empty_bar = full_bar + C::NSTAGE;
+    uint64_t *acc_full = empty_bar + C::NSTAGE, *acc_empty = acc_full + 1;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nkb = a.taps * a.cchunks;
@@ -335,14 +383,25 @@ k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ C
         asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap_lo) : "memory");
         // empty: both consumer warpgroups of this CTA and, with multicast, of the two peers that write into its stages
         for (int s = 0; s < C::NSTAGE; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], mc ? 6 : 2); }
+        mbar_init(acc_full, 256);
+        mbar_init(acc_empty, EPI_WARPS * 32);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     // peers arrive on these barriers and multicast into this CTA's stages: all barriers of the cluster are initialised first
     if (mc) cluster_sync();
     else __syncthreads();
 
-    if (warp == PRODUCER_WARP) {
-        if (lane == 0) {     // ===== TMA producer =====
+    if (warp >= PRODUCER_WARP) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS_EPILOGUE));
+        if (warp >= EPI_WARP0) {     // ===== epilogue warps =====
+            int it = 0;
+            for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++it) {
+                const int img = t / (2 * Args::kCoBlocks), co0 = ((t >> 1) % Args::kCoBlocks) * N, mh = t & 1;
+                mbar_wait(acc_full, it & 1);
+                epilogue(a, hand, img, mh, co0, warp - EPI_WARP0, lane);
+                mbar_arrive(acc_empty);
+            }
+        } else if (lane == 0) {     // ===== TMA producer =====
             const int r = a.ks / 2;
             const uint16_t amask = (uint16_t)(0x5u << (rank & 1)), wmask = (uint16_t)(0x3u << (rank & 2));
             int stage = 0, phase = 0;
@@ -381,6 +440,7 @@ k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ C
     }
 
     // ===== consumers: warpgroup wg owns tile rows [64 wg, 64 wg + 64) =====
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS_CONSUMER));
     const int wg = warp >> 2;
     const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);          // this thread's first accumulator row
     // one thread per warpgroup releases a stage: to this CTA's producer and, with multicast, to the two peers writing into it
@@ -389,9 +449,8 @@ k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ C
         if (mc) { mbar_arrive_cluster(&empty_bar[s], rank); mbar_arrive_cluster(&empty_bar[s], rank ^ 1); mbar_arrive_cluster(&empty_bar[s], rank ^ 2); }
         else mbar_arrive(&empty_bar[s]);
     };
-    int stage = 0, phase = 0;
-    for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
-        const int img = t / (2 * Args::kCoBlocks), co0 = ((t >> 1) % Args::kCoBlocks) * N, mh = t & 1;
+    int stage = 0, phase = 0, it = 0;
+    for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++it) {
         float dm[N / 2], dc[N / 2];
 #pragma unroll
         for (int i = 0; i < N / 2; ++i) { dm[i] = 0.f; dc[i] = 0.f; }
@@ -420,7 +479,9 @@ k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ C
         fence_regs(dm);
         fence_regs(dc);
         if (prev >= 0) release(prev);
-        epilogue(a, dm, dc, img, mh * 128 + row0, co0, lane);
+        mbar_wait(acc_empty, (it & 1) ^ 1);            // the epilogue has read the previous tile
+        hand_store(a, hand, dm, dc, row0, lane);
+        mbar_arrive(acc_full);
     }
 }
 
