@@ -68,28 +68,49 @@ class BitSwapCodec:
                 pass
             self._h = None
 
-    def encode(self, streams: StreamSet, x: torch.Tensor, first=0, scheme=BITSWAP):
-        """x: uint8 CUDA tensor [count, C, 32, 32]; pushes one image onto each of `count` streams. Async."""
+    def encode(self, streams: StreamSet, x: torch.Tensor, first=0, scheme=BITSWAP, extent=None):
+        """x: uint8 CUDA tensor [count, C, 32, 32]; pushes one image onto each of `count` streams. Async.
+        extent: None (full blocks) or an int16 CUDA tensor [count, 2] of valid block extents (vh, vw) in [1, 32]: only the
+        pixels inside the extent are coded, the rest of the block is ignored (see bsw_codec_encode_ext)."""
         assert x.is_cuda and x.dtype == torch.uint8 and x.is_contiguous()
         self._same_device(streams, x)
         count = x.shape[0]
         with on_device(self.device):
-            check(lib().bsw_codec_encode(self._h, streams.handle, first, count, x.data_ptr(), scheme, cuda_stream_ptr()))
+            if extent is None:
+                check(lib().bsw_codec_encode(self._h, streams.handle, first, count, x.data_ptr(), scheme, cuda_stream_ptr()))
+            else:
+                ext = self._extent(extent, count)
+                check(lib().bsw_codec_encode_ext(self._h, streams.handle, first, count, x.data_ptr(), ext.data_ptr(), scheme,
+                                                 cuda_stream_ptr()))
+
+    def _extent(self, extent, count):
+        if not (torch.is_tensor(extent) and extent.is_cuda and extent.dtype == torch.int16 and extent.is_contiguous()
+                and tuple(extent.shape) == (count, 2)):
+            raise ValueError(f"extent: need a contiguous int16 CUDA tensor of shape ({count}, 2)")
+        if extent.device.index != self.device:
+            raise ValueError(f"codec is on cuda:{self.device}, extents on {extent.device}")
+        return extent
 
     def _same_device(self, streams, x=None):
         if streams.device != self.device or (x is not None and x.device.index != self.device):
             raise ValueError(f"codec is on cuda:{self.device}; streams on cuda:{streams.device}"
                              + (f", pixels on {x.device}" if x is not None else ""))
 
-    def decode(self, streams: StreamSet, count: int, first=0, scheme=BITSWAP, out=None):
-        """Pops one image from each stream; returns uint8 CUDA tensor [count, C, 32, 32]. Async."""
+    def decode(self, streams: StreamSet, count: int, first=0, scheme=BITSWAP, out=None, extent=None):
+        """Pops one image from each stream; returns uint8 CUDA tensor [count, C, 32, 32]. Async.
+        extent: the tensor the images were encoded with (None = full blocks); pixels outside it come back edge-padded."""
         if out is None:
             out = torch.empty((count,) + tuple(self.cfg.xs), dtype=torch.uint8, device=torch.device("cuda", self.device))
         if not (out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and out.numel() >= count * int(np.prod(self.cfg.xs))):
             raise ValueError("decode(out=...): need a contiguous uint8 CUDA tensor with room for `count` images")
         self._same_device(streams, out)
         with on_device(self.device):
-            check(lib().bsw_codec_decode(self._h, streams.handle, first, count, out.data_ptr(), scheme, cuda_stream_ptr()))
+            if extent is None:
+                check(lib().bsw_codec_decode(self._h, streams.handle, first, count, out.data_ptr(), scheme, cuda_stream_ptr()))
+            else:
+                ext = self._extent(extent, count)
+                check(lib().bsw_codec_decode_ext(self._h, streams.handle, first, count, out.data_ptr(), ext.data_ptr(), scheme,
+                                                 cuda_stream_ptr()))
         return out
 
     @property
@@ -179,14 +200,16 @@ class PipelinedCodec:
         for st in self.streams:
             cur.wait_stream(st)
 
-    def encode(self, streams: StreamSet, x: torch.Tensor, first=0, scheme=BITSWAP):
+    def encode(self, streams: StreamSet, x: torch.Tensor, first=0, scheme=BITSWAP, extent=None):
         assert x.is_cuda and x.dtype == torch.uint8 and x.is_contiguous() and x.shape[0] <= self.max_batch
-        self._fan(x.shape[0], lambda c, b, n: c.encode(streams, x[b:b + n], first=first + b, scheme=scheme))
+        self._fan(x.shape[0], lambda c, b, n: c.encode(streams, x[b:b + n], first=first + b, scheme=scheme,
+                                                       extent=None if extent is None else extent[b:b + n]))
 
-    def decode(self, streams: StreamSet, count: int, first=0, scheme=BITSWAP, out=None):
+    def decode(self, streams: StreamSet, count: int, first=0, scheme=BITSWAP, out=None, extent=None):
         if out is None:
             out = torch.empty((count,) + tuple(self.cfg.xs), dtype=torch.uint8, device=torch.device("cuda", self.device))
-        self._fan(count, lambda c, b, n: c.decode(streams, n, first=first + b, scheme=scheme, out=out[b:b + n]))
+        self._fan(count, lambda c, b, n: c.decode(streams, n, first=first + b, scheme=scheme, out=out[b:b + n],
+                                                  extent=None if extent is None else extent[b:b + n]))
         return out
 
     def set_two_phase(self, on=True):

@@ -672,10 +672,13 @@ __device__ __forceinline__ void load_tile_row(double (&e)[NB], const double *til
     for (int j = 0; j < NB; ++j) e[j] = tile[lane * (NB + 1) + j];
 }
 
-template <int NB>
+// MASK (both kernels): pixel level with block extents, ext int16 [count][2]; rows outside the extent (bsw_x_live) are not
+// coded, and a pop leaves their symbols for the codec's pad kernel
+template <int NB, bool MASK>
 __global__ void __launch_bounds__(FW * 32) k_logistic_pop(bsw_streams sv, int first, int count,
         const float *__restrict__ mu, int64_t mss, const float *__restrict__ sc, int64_t sss,
-        const double *__restrict__ endp, int64_t ers, int16_t *__restrict__ sym, int64_t L, int bits, int q) {
+        const double *__restrict__ endp, int64_t ers, int16_t *__restrict__ sym, int64_t L, int bits, int q,
+        const int16_t *__restrict__ ext) {
     extern __shared__ double smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int si = blockIdx.x * FW + warp;
@@ -684,6 +687,8 @@ __global__ void __launch_bounds__(FW * 32) k_logistic_pop(bsw_streams sv, int fi
     WarpStream ws;
     ws.open(sv, b);
     if (ws.err) return;
+    int vh = 32, vw = 32;
+    if (MASK) { vh = ext[2 * si]; vw = ext[2 * si + 1]; }
     double *tile0 = smem + (size_t)warp * 2 * tile_doubles<NB>();
     double *tile1 = tile0 + tile_doubles<NB>();
     const float *mub = mu + (int64_t)si * mss, *scb = sc + (int64_t)si * sss;
@@ -716,23 +721,25 @@ __global__ void __launch_bounds__(FW * 32) k_logistic_pop(bsw_streams sv, int fi
                 cur ^= 1;
             }
         }
-        RowTable<NB> T;
-        build_row<NB>(e, __shfl_sync(FULL, mu_w, j32), __shfl_sync(FULL, sc_w, j32), mult, bits, lane, T);
-        // ---- search: s = max{k : C[k] <= m}  (cifar_compress.py:60-61) -----------------------------
-        uint32_t m = (uint32_t)ws.x & mask;
-        int owner = 31 - __clz(__ballot_sync(FULL, T.base <= m));
-        uint32_t acc = T.base, cs = T.base, ps = T.P[0];
-        int js = 0;
+        if (!MASK || bsw_x_live(i, vh, vw)) {
+            RowTable<NB> T;
+            build_row<NB>(e, __shfl_sync(FULL, mu_w, j32), __shfl_sync(FULL, sc_w, j32), mult, bits, lane, T);
+            // ---- search: s = max{k : C[k] <= m}  (cifar_compress.py:60-61) -------------------------
+            uint32_t m = (uint32_t)ws.x & mask;
+            int owner = 31 - __clz(__ballot_sync(FULL, T.base <= m));
+            uint32_t acc = T.base, cs = T.base, ps = T.P[0];
+            int js = 0;
 #pragma unroll
-        for (int j = 1; j < NB; ++j) {
-            acc += T.P[j - 1];
-            if (acc <= m) { cs = acc; ps = T.P[j]; js = j; }
+            for (int j = 1; j < NB; ++j) {
+                acc += T.P[j - 1];
+                if (acc <= m) { cs = acc; ps = T.P[j]; js = j; }
+            }
+            cs = __shfl_sync(FULL, cs, owner);
+            ps = __shfl_sync(FULL, ps, owner);
+            int s = owner * NB + __shfl_sync(FULL, js, owner);
+            if (lane == j32) my_sym = s;                                        // :62
+            ws.decode(ps, cs, m, bits, lane);                                   // :63-65
         }
-        cs = __shfl_sync(FULL, cs, owner);
-        ps = __shfl_sync(FULL, ps, owner);
-        int s = owner * NB + __shfl_sync(FULL, js, owner);
-        if (lane == j32) my_sym = s;                                            // :62
-        ws.decode(ps, cs, m, bits, lane);                                       // :63-65
         if (j32 == 0 || ws.err) {                      // block of rows done: coalesced symbol store
             int64_t r = (i & ~(int64_t)31) + lane;
             if (r < L && r >= i) sy[r] = (int16_t)my_sym;
@@ -743,10 +750,11 @@ __global__ void __launch_bounds__(FW * 32) k_logistic_pop(bsw_streams sv, int fi
     ws.close(sv, b, lane);
 }
 
-template <int NB>
+template <int NB, bool MASK>
 __global__ void __launch_bounds__(FW * 32) k_logistic_push(bsw_streams sv, int first, int count,
         const float *__restrict__ mu, int64_t mss, const float *__restrict__ sc, int64_t sss,
-        const double *__restrict__ endp, int64_t ers, const int16_t *__restrict__ sym, int64_t L, int bits, int q) {
+        const double *__restrict__ endp, int64_t ers, const int16_t *__restrict__ sym, int64_t L, int bits, int q,
+        const int16_t *__restrict__ ext) {
     extern __shared__ double smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int si = blockIdx.x * FW + warp;
@@ -755,6 +763,8 @@ __global__ void __launch_bounds__(FW * 32) k_logistic_push(bsw_streams sv, int f
     WarpStream ws;
     ws.open(sv, b);
     if (ws.err) return;
+    int vh = 32, vw = 32;
+    if (MASK) { vh = ext[2 * si]; vw = ext[2 * si + 1]; }
     ws.push_begin(lane);
     double *tile0 = smem + (size_t)warp * 2 * tile_doubles<NB>();
     double *tile1 = tile0 + tile_doubles<NB>();
@@ -788,6 +798,7 @@ __global__ void __launch_bounds__(FW * 32) k_logistic_push(bsw_streams sv, int f
                 cur ^= 1;
             }
         }
+        if (MASK && !bsw_x_live(i, vh, vw)) continue;
         RowTable<NB> T;
         build_row<NB>(e, __shfl_sync(FULL, mu_w, j32), __shfl_sync(FULL, sc_w, j32), mult, bits, lane, T);
         int s = __shfl_sync(FULL, sym_w, j32);
@@ -809,36 +820,43 @@ __global__ void __launch_bounds__(FW * 32) k_logistic_push(bsw_streams sv, int f
     ws.close(sv, b, lane);
 }
 
-template <int NB>
+template <int NB, bool MASK>
 static int launch_fused(bool push, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
                         int64_t sss, const double *endp, int64_t ers, int16_t *sym, int64_t L, int bits, int q,
-                        cudaStream_t st) {
+                        const int16_t *ext, cudaStream_t st) {
     size_t smem = (size_t)FW * 2 * tile_doubles<NB>() * sizeof(double);
     if (push) {
-        BSW_CUDA(cudaFuncSetAttribute(k_logistic_push<NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_logistic_push<NB><<<(count + FW - 1) / FW, FW * 32, smem, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q);
+        BSW_CUDA(cudaFuncSetAttribute(k_logistic_push<NB, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_logistic_push<NB, MASK><<<(count + FW - 1) / FW, FW * 32, smem, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext);
     } else {
-        BSW_CUDA(cudaFuncSetAttribute(k_logistic_pop<NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_logistic_pop<NB><<<(count + FW - 1) / FW, FW * 32, smem, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q);
+        BSW_CUDA(cudaFuncSetAttribute(k_logistic_pop<NB, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_logistic_pop<NB, MASK><<<(count + FW - 1) / FW, FW * 32, smem, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext);
     }
     BSW_LAUNCH_CHECK();
     return BSW_OK;
 }
+template <int NB>
+static int launch_fused(bool push, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
+                        int64_t sss, const double *endp, int64_t ers, int16_t *sym, int64_t L, int bits, int q,
+                        const int16_t *ext, cudaStream_t st) {
+    if (ext) return launch_fused<NB, true>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext, st);
+    return launch_fused<NB, false>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, nullptr, st);
+}
 static int dispatch_fused(bool push, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
                           int64_t sss, const double *endp, int64_t ers, int16_t *sym, int64_t L, int S, int bits, int q,
-                          void *stream) {
+                          const int16_t *ext, void *stream) {
     if (int rc = check_range(s, first, count)) return rc;
     BSW_REQUIRE(mu && sc && endp && sym && L > 0, "fused coder: null argument");
     BSW_REQUIRE(bits > 0 && bits <= 31 && q >= 0 && q < bits, "fused coder: bits/quantbits out of range");
     BSW_REQUIRE((ers == 0 || ers >= S) && (((uintptr_t)endp) & 7) == 0, "fused coder: endpoint rows must hold S doubles (+inf padded)");
     cudaStream_t st = (cudaStream_t)stream;
     switch (S) {
-        case 32:   return launch_fused<1>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, st);
-        case 64:   return launch_fused<2>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, st);
-        case 128:  return launch_fused<4>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, st);
-        case 256:  return launch_fused<8>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, st);
-        case 512:  return launch_fused<16>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, st);
-        case 1024: return launch_fused<32>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, st);
+        case 32:   return launch_fused<1>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext, st);
+        case 64:   return launch_fused<2>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext, st);
+        case 128:  return launch_fused<4>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext, st);
+        case 256:  return launch_fused<8>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext, st);
+        case 512:  return launch_fused<16>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext, st);
+        case 1024: return launch_fused<32>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext, st);
     }
     bsw_set_error("fused coder: support must be one of 32,64,...,1024 (got %d)", S);
     return BSW_E_INVALID;
@@ -846,12 +864,18 @@ static int dispatch_fused(bool push, bsw_streams *s, int first, int count, const
 extern "C" int bsw_logistic_push(bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
                                  int64_t sss, const double *endp, int64_t ers, const int16_t *sym, int64_t L, int S,
                                  int bits, int q, void *stream) {
-    return dispatch_fused(true, s, first, count, mu, mss, sc, sss, endp, ers, (int16_t *)sym, L, S, bits, q, stream);
+    return dispatch_fused(true, s, first, count, mu, mss, sc, sss, endp, ers, (int16_t *)sym, L, S, bits, q, nullptr, stream);
 }
 extern "C" int bsw_logistic_pop(bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
                                 int64_t sss, const double *endp, int64_t ers, int16_t *sym, int64_t L, int S, int bits,
                                 int q, void *stream) {
-    return dispatch_fused(false, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, S, bits, q, stream);
+    return dispatch_fused(false, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, S, bits, q, nullptr, stream);
+}
+// the codec's pixel level with block extents (ext int16 [count][2], see bsw_x_live)
+int bsw_logistic_fused_ext(bool push, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
+                           int64_t sss, const double *endp, int64_t ers, int16_t *sym, int64_t L, int S, int bits, int q,
+                           const int16_t *ext, cudaStream_t st) {
+    return dispatch_fused(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, S, bits, q, ext, st);
 }
 
 // ================================================================================================

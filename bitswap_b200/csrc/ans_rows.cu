@@ -269,8 +269,10 @@ __global__ void __launch_bounds__(RW * 32, 2) k_rows(int count, int64_t L, const
 
 // ---- phase B: push -------------------------------------------------------------------------------------------------
 constexpr int BW = 4;
+// MASK: pixel level with block extents (bsw_x_live); the 32 rows of a block are one image row, so the coded ones are a prefix
+template <bool MASK>
 __global__ void __launch_bounds__(BW * 32) k_push_pairs(bsw_streams sv, int first, int count, const uint4 *__restrict__ pairs,
-                                                        int64_t L, int bits) {
+                                                        int64_t L, int bits, const int16_t *__restrict__ ext) {
     const int lane = threadIdx.x & 31;
     const int si = blockIdx.x * BW + (threadIdx.x >> 5);
     if (si >= count) return;
@@ -278,6 +280,8 @@ __global__ void __launch_bounds__(BW * 32) k_push_pairs(bsw_streams sv, int firs
     WarpStream2 ws;
     ws.open(sv, b);
     if (ws.err) return;
+    int vh = 32, vw = 32;
+    if (MASK) { vh = ext[2 * si]; vw = ext[2 * si + 1]; }
     ws.push_begin(lane);
     const uint4 *pp = pairs + (int64_t)si * L;
     uint4 nxt = (lane < L) ? __ldg(pp + lane) : make_uint4(1, 0, 0xffffffffu, 0xffffffffu);
@@ -286,6 +290,7 @@ __global__ void __launch_bounds__(BW * 32) k_push_pairs(bsw_streams sv, int firs
         int64_t r = i0 + 32 + lane;
         if (r < L) nxt = __ldg(pp + r);                   // prefetch the next 32 rows
         int n = (int)min((int64_t)32, L - i0);
+        if (MASK) n = (int)((i0 >> 5) & 31) < vh ? min(n, vw) : 0;
         for (int j = 0; j < n && !ws.err; ++j) {
             uint64_t M = ((uint64_t)__shfl_sync(FULL, cur.w, j) << 32) | __shfl_sync(FULL, cur.z, j);
             const uint32_t pj = __shfl_sync(FULL, cur.x, j);
@@ -298,11 +303,11 @@ __global__ void __launch_bounds__(BW * 32) k_push_pairs(bsw_streams sv, int firs
 }
 
 // ---- phase B: pop ----------------------------------------------------------------------------------------------------
-template <int NB>
+template <int NB, bool MASK>
 __global__ void __launch_bounds__(BW * 32) k_pop_coarse(bsw_streams sv, int first, int count, const float *__restrict__ mu,
         int64_t mss, const float *__restrict__ sc, int64_t sss, const double *__restrict__ endp, int64_t ers,
         const uint32_t *__restrict__ coarse, const uint2 *__restrict__ fix, int16_t *__restrict__ sym, int64_t L,
-        int bits, int q) {
+        int bits, int q, const int16_t *__restrict__ ext) {
     const int lane = threadIdx.x & 31;
     const int si = blockIdx.x * BW + (threadIdx.x >> 5);
     if (si >= count) return;
@@ -310,6 +315,8 @@ __global__ void __launch_bounds__(BW * 32) k_pop_coarse(bsw_streams sv, int firs
     WarpStream2 ws;
     ws.open(sv, b);
     if (ws.err) return;
+    int vh = 32, vw = 32;
+    if (MASK) { vh = ext[2 * si]; vw = ext[2 * si + 1]; }
     constexpr int S = 32 * NB;
     const float *mub = mu + (int64_t)si * mss, *scb = sc + (int64_t)si * sss;
     const uint32_t *cb = coarse + (int64_t)si * L * NB;
@@ -351,25 +358,27 @@ __global__ void __launch_bounds__(BW * 32) k_pop_coarse(bsw_streams sv, int firs
         const uint32_t base = base_n1;
         base_n1 = base_n2;
         if (i > 1) base_n2 = (lane < NB) ? __ldg(cb + (i - 2) * NB + lane) : 0xffffffffu;
-        const double rs = __ddiv_rn(1.0, s_);
-        const uint32_t mm = (uint32_t)ws.x & mask;                                       // cifar_compress.py:60
-        const int chunk = 31 - __clz(__ballot_sync(FULL, base <= mm));                   // base of lanes >= NB is UINT_MAX
-        const int k = chunk * 32 + lane;
-        const double *e = endp + i * ers;
-        // two independent cdf evaluations per lane (upper and lower endpoint of my bin)
-        double c_hi = (k == S - 1) ? 1.0 : bsw_cdf_fast(__ldg(e + k), m_, s_, rs);
-        double c_lo = (k == 0) ? 0.0 : bsw_cdf_fast(__ldg(e + k - 1), m_, s_, rs);
-        uint32_t v = __double2uint_rz(__dmul_rn(__dsub_rn(c_hi, c_lo), mult)) + 1u + (k == bi ? rem : 0u);
-        uint32_t incl = v;
-        for (int o = 1; o < 32; o <<= 1) {
-            uint32_t t = __shfl_up_sync(FULL, incl, o);
-            if (lane >= o) incl += t;
+        if (!MASK || bsw_x_live(i, vh, vw)) {             // a masked dim leaves the head alone; its symbol is padded later
+            const double rs = __ddiv_rn(1.0, s_);
+            const uint32_t mm = (uint32_t)ws.x & mask;                                   // cifar_compress.py:60
+            const int chunk = 31 - __clz(__ballot_sync(FULL, base <= mm));               // base of lanes >= NB is UINT_MAX
+            const int k = chunk * 32 + lane;
+            const double *e = endp + i * ers;
+            // two independent cdf evaluations per lane (upper and lower endpoint of my bin)
+            double c_hi = (k == S - 1) ? 1.0 : bsw_cdf_fast(__ldg(e + k), m_, s_, rs);
+            double c_lo = (k == 0) ? 0.0 : bsw_cdf_fast(__ldg(e + k - 1), m_, s_, rs);
+            uint32_t v = __double2uint_rz(__dmul_rn(__dsub_rn(c_hi, c_lo), mult)) + 1u + (k == bi ? rem : 0u);
+            uint32_t incl = v;
+            for (int o = 1; o < 32; o <<= 1) {
+                uint32_t t = __shfl_up_sync(FULL, incl, o);
+                if (lane >= o) incl += t;
+            }
+            const uint32_t cex = __shfl_sync(FULL, base, chunk) + incl - v;              // integer cdf at my bin
+            const int js = 31 - __clz(__ballot_sync(FULL, cex <= mm));                   // :61 searchsorted 'right' - 1
+            const uint32_t ps = __shfl_sync(FULL, v, js), cs = __shfl_sync(FULL, cex, js);
+            if (lane == j32) my_sym = chunk * 32 + js;                                   // :62
+            ws.decode(ps, cs, mm, bits, lane);                                           // :63-65
         }
-        const uint32_t cex = __shfl_sync(FULL, base, chunk) + incl - v;                  // integer cdf at my bin
-        const int js = 31 - __clz(__ballot_sync(FULL, cex <= mm));                       // :61 searchsorted 'right' - 1
-        const uint32_t ps = __shfl_sync(FULL, v, js), cs = __shfl_sync(FULL, cex, js);
-        if (lane == j32) my_sym = chunk * 32 + js;                                       // :62
-        ws.decode(ps, cs, mm, bits, lane);                                               // :63-65
         if (j32 == 0 || ws.err) {
             int64_t r = (i & ~(int64_t)31) + lane;
             if (r < L && r >= i) sy[r] = (int16_t)my_sym;
@@ -453,10 +462,19 @@ int launch_pop_full(bsw_streams *s, int first, int count, const uint32_t *pfull,
     return BSW_OK;
 }
 
+int launch_push_pairs(bsw_streams *s, int first, int count, const void *scratch, int64_t L, int bits, const int16_t *ext,
+                      cudaStream_t st) {
+    BSW_MAX_SHARED_ONCE(k_push_pairs<false>); BSW_MAX_SHARED_ONCE(k_push_pairs<true>);
+    if (ext) k_push_pairs<true><<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, (const uint4 *)scratch, L, bits, ext);
+    else k_push_pairs<false><<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, (const uint4 *)scratch, L, bits, nullptr);
+    BSW_LAUNCH_CHECK();
+    return BSW_OK;
+}
+
 template <int NB>
 int launch_rows(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
                 int64_t sss, const double *endp, int64_t ers, int16_t *sym, int64_t L, int bits, int q, void *scratch,
-                cudaStream_t st) {
+                const int16_t *ext, cudaStream_t st) {
     dim3 grid((unsigned)L, (count + RW - 1) / RW);
     // pop scratch layout: [coarse: count*L*NB u32, rounded up to 8 bytes] [fix: count*L uint2]
     uint4 *pairs = (uint4 *)scratch;
@@ -468,7 +486,7 @@ int launch_rows(int phase, bool pop, bsw_streams *s, int first, int count, const
     const bool exact = bits > 31 || env_exact;
     BSW_MAX_SHARED_ONCE((k_rows<NB, true, false>)); BSW_MAX_SHARED_ONCE((k_rows<NB, true, true>));
     BSW_MAX_SHARED_ONCE((k_rows<NB, false, false>)); BSW_MAX_SHARED_ONCE((k_rows<NB, false, true>));
-    BSW_MAX_SHARED_ONCE(k_pop_coarse<NB>); BSW_MAX_SHARED_ONCE(k_push_pairs);
+    BSW_MAX_SHARED_ONCE((k_pop_coarse<NB, false>)); BSW_MAX_SHARED_ONCE((k_pop_coarse<NB, true>));
     if (phase == 0) {
         if (pop) {
             if (exact) k_rows<NB, true, false><<<grid, RW * 32, 0, st>>>(count, L, mu, mss, sc, sss, endp, ers, nullptr, bits, q, nullptr, coarse, fix, kp);
@@ -478,16 +496,10 @@ int launch_rows(int phase, bool pop, bsw_streams *s, int first, int count, const
             else k_rows<NB, false, true><<<grid, RW * 32, 0, st>>>(count, L, mu, mss, sc, sss, endp, ers, sym, bits, q, pairs, nullptr, nullptr, kp);
         }
     } else {
-        if (pop) k_pop_coarse<NB><<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, coarse, fix, sym, L, bits, q);
-        else k_push_pairs<<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, pairs, L, bits);
+        if (!pop) return launch_push_pairs(s, first, count, pairs, L, bits, ext, st);
+        if (ext) k_pop_coarse<NB, true><<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, coarse, fix, sym, L, bits, q, ext);
+        else k_pop_coarse<NB, false><<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, coarse, fix, sym, L, bits, q, nullptr);
     }
-    BSW_LAUNCH_CHECK();
-    return BSW_OK;
-}
-
-int launch_push_pairs(bsw_streams *s, int first, int count, const void *scratch, int64_t L, int bits, cudaStream_t st) {
-    BSW_MAX_SHARED_ONCE(k_push_pairs);
-    k_push_pairs<<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, (const uint4 *)scratch, L, bits);
     BSW_LAUNCH_CHECK();
     return BSW_OK;
 }
@@ -527,7 +539,7 @@ int bsw_pop_shared_table(bsw_streams *s, int first, int count, const uint32_t *P
 int bsw_rows6_build_meta(const double *endp, int64_t ers, int64_t L, int S, void *meta_dev, int *n_affine_host, cudaStream_t st);
 int bsw_rows6_launch(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
                      int64_t sss, const double *endp, int64_t ers, const void *meta, int16_t *sym, int64_t L, int S, int bits,
-                     int q, void *scratch, size_t scratch_bytes, cudaStream_t st);
+                     int q, void *scratch, size_t scratch_bytes, const int16_t *ext, cudaStream_t st);
 
 // Scratch bytes of the two-phase coder for `count` streams of L rows: per row 16 B (push: P, C, reciprocal) or
 // 136 B (pop: 32 chunk bases + argmax/remnant), whichever kernel family runs.
@@ -536,26 +548,27 @@ size_t bsw_rows_scratch_bytes(int count, int64_t L) { return (size_t)count * L *
 // Two-phase variants of bsw_logistic_push / bsw_logistic_pop (same arguments + caller-provided scratch).
 // phase 0 = the parallel row-table kernel, phase 1 = the serial coder; call both, in order, on one stream, with the
 // same scratch.  meta != NULL selects the affine-row kernels of ans_rows6.cu (meta = bsw_rows6_build_meta of these
-// endpoint rows); meta == NULL the generic ones above.
+// endpoint rows); meta == NULL the generic ones above.  ext != NULL (pixel level only): phase 1 codes just the dims inside
+// each stream's block extent (bsw_x_live); phase 0 computes every row either way.
 int bsw_logistic_2p(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
                     int64_t sss, const double *endp, int64_t ers, const void *meta, int16_t *sym, int64_t L, int S, int bits,
-                    int q, void *scratch, size_t scratch_bytes, cudaStream_t st) {
+                    int q, void *scratch, size_t scratch_bytes, const int16_t *ext, cudaStream_t st) {
     BSW_REQUIRE(s && first >= 0 && count > 0 && first + count <= s->B, "stream range out of bounds");
     BSW_REQUIRE(mu && sc && endp && sym && scratch && L > 0 && L < 65536 * 32, "two-phase coder: bad arguments");
     BSW_REQUIRE(ers == 0 || ers >= S, "two-phase coder: endpoint rows must hold S doubles (+1e300 padded)");
     BSW_REQUIRE(scratch_bytes >= (pop ? bsw_rows_scratch_bytes(count, L) : (size_t)count * L * 16), "two-phase coder: scratch too small");
     BSW_REQUIRE((((uintptr_t)scratch) & 15) == 0, "two-phase coder: scratch must be 16-byte aligned");
     if (meta) {
-        if (phase == 1 && !pop) return launch_push_pairs(s, first, count, scratch, L, bits, st);
-        return bsw_rows6_launch(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, meta, sym, L, S, bits, q, scratch, scratch_bytes, st);
+        if (phase == 1 && !pop) return launch_push_pairs(s, first, count, scratch, L, bits, ext, st);
+        return bsw_rows6_launch(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, meta, sym, L, S, bits, q, scratch, scratch_bytes, ext, st);
     }
     switch (S) {
-        case 32:   return launch_rows<1>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, st);
-        case 64:   return launch_rows<2>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, st);
-        case 128:  return launch_rows<4>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, st);
-        case 256:  return launch_rows<8>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, st);
-        case 512:  return launch_rows<16>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, st);
-        case 1024: return launch_rows<32>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, st);
+        case 32:   return launch_rows<1>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
+        case 64:   return launch_rows<2>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
+        case 128:  return launch_rows<4>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
+        case 256:  return launch_rows<8>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
+        case 512:  return launch_rows<16>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
+        case 1024: return launch_rows<32>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
     }
     bsw_set_error("two-phase coder: support must be one of 32,64,...,1024 (got %d)", S);
     return BSW_E_INVALID;
@@ -703,8 +716,8 @@ static int abi_2p(bool pop, bsw_streams *s, int first, int count, const float *m
         if (mode == 1 || n_aff == (ers == 0 ? 1 : (int)L)) meta = m;
     }
     const size_t sb = bsw_rows_scratch_bytes(count, L);
-    if (int rc = bsw_logistic_2p(0, pop, s, first, count, mu, mss, sc, sss, endp, ers, meta, sym, L, S, bits, q, scratch, sb, st)) return rc;
-    return bsw_logistic_2p(1, pop, s, first, count, mu, mss, sc, sss, endp, ers, meta, sym, L, S, bits, q, scratch, sb, st);
+    if (int rc = bsw_logistic_2p(0, pop, s, first, count, mu, mss, sc, sss, endp, ers, meta, sym, L, S, bits, q, scratch, sb, nullptr, st)) return rc;
+    return bsw_logistic_2p(1, pop, s, first, count, mu, mss, sc, sss, endp, ers, meta, sym, L, S, bits, q, scratch, sb, nullptr, st);
 }
 extern "C" int bsw_logistic_push_2p(bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc, int64_t sss,
                                     const double *endp, int64_t ers, const int16_t *sym, int64_t L, int S, int bits, int q,

@@ -324,10 +324,13 @@ __device__ __forceinline__ double shfl_d(double v, int src) {
     return __hiloint2double(__shfl_sync(FULL, __double2hiint(v), src), __shfl_sync(FULL, __double2loint(v), src));
 }
 
+// MASK: pixel level with block extents -- rows outside the extent keep the block loads and the prefetch going but skip the
+// search and the decode (bsw_x_live, warp-uniform); their symbols are written later by the codec's pad kernel
+template <bool MASK>
 __global__ void __launch_bounds__(PW6 * 32) k_pop6(bsw_streams sv, int first, int count, const float *__restrict__ mu, int64_t mss,
         const float *__restrict__ sc, int64_t sss, const double *__restrict__ endp, int64_t ers,
         const R6RowMeta *__restrict__ meta, int64_t mrs, const uint32_t *__restrict__ bases, const uint2 *__restrict__ fix,
-        int16_t *__restrict__ sym, int64_t L, int S, int bits, int q) {
+        int16_t *__restrict__ sym, int64_t L, int S, int bits, int q, const int16_t *__restrict__ ext) {
     const int lane = threadIdx.x & 31;
     const int si = blockIdx.x * PW6 + (threadIdx.x >> 5);
     if (si >= count) return;
@@ -335,6 +338,8 @@ __global__ void __launch_bounds__(PW6 * 32) k_pop6(bsw_streams sv, int first, in
     WarpStream6 ws;
     ws.open(sv, b);
     if (ws.err) return;
+    int vh = 32, vw = 32;
+    if (MASK) { vh = ext[2 * si]; vw = ext[2 * si + 1]; }
     const float *mub = mu + (int64_t)si * mss, *scb = sc + (int64_t)si * sss;
     const uint32_t *bb = bases + (int64_t)si * L * 32;
     const uint2 *fb = fix + (int64_t)si * L;
@@ -383,40 +388,42 @@ __global__ void __launch_bounds__(PW6 * 32) k_pop6(bsw_streams sv, int first, in
         const uint32_t base = base_n1;
         base_n1 = base_n2;
         if (i > 1) base_n2 = __ldg(bb + (i - 2) * 32 + lane);
-        const uint32_t mm = (uint32_t)ws.x & mask;                                       // cifar_compress.py:60
-        const uint32_t Ckh = (1u << bits) - (uint32_t)(S - kh);                          // integer cdf at bin kh (dead bins: P = 1)
-        uint32_t ps, cs;
-        int s;
-        if (mm < (uint32_t)kl) { s = (int)mm; ps = 1u; cs = mm; }                        // dead bins on the left: C[k] = k
-        else if (mm >= Ckh) { s = kh + (int)(mm - Ckh); ps = 1u; cs = mm; }              // dead bins on the right
-        else {
-            const int chunk = 31 - __clz(__ballot_sync(FULL, base <= mm));              // empty chunks hold Ckh > mm
-            const int k = kl + chunk * m + lane;
-            const bool active = lane < m && k < kh;
-            const double th = __fma_rn((double)k, dt, t0);                               // t at my bin's upper endpoint
-            const double c_hi = (k >= S - 1) ? 1.0 : r6_rcp3(__dadd_rn(1.0, r6_exp_neg(th)));
-            const double c_lo = (k <= 0) ? 0.0 : r6_rcp3(__dadd_rn(1.0, r6_exp_neg(__dsub_rn(th, dt))));
-            const double z = __fma_rn(__dsub_rn(c_hi, c_lo), mult2, magic);
-            uint32_t raw = r6_raw(z);
-            const bool doubt = active && (r6_doubt(z, dmask) || raw < 0x80000000u);
-            if (__any_sync(FULL, doubt)) {                                               // rare: the exact function on the real endpoints
-                const double m_ = (double)__shfl_sync(FULL, mu_w, j32), s_ = (double)__shfl_sync(FULL, sc_w, j32);
-                const double rs = shfl_d(rs_w, j32);
-                if (doubt) raw = r6_exact_pm(endp + i * ers, k, S, m_, s_, rs, mult) + 0x80000000u;
+        if (!MASK || bsw_x_live(i, vh, vw)) {
+            const uint32_t mm = (uint32_t)ws.x & mask;                                   // cifar_compress.py:60
+            const uint32_t Ckh = (1u << bits) - (uint32_t)(S - kh);                      // integer cdf at bin kh (dead bins: P = 1)
+            uint32_t ps, cs;
+            int s;
+            if (mm < (uint32_t)kl) { s = (int)mm; ps = 1u; cs = mm; }                    // dead bins on the left: C[k] = k
+            else if (mm >= Ckh) { s = kh + (int)(mm - Ckh); ps = 1u; cs = mm; }          // dead bins on the right
+            else {
+                const int chunk = 31 - __clz(__ballot_sync(FULL, base <= mm));          // empty chunks hold Ckh > mm
+                const int k = kl + chunk * m + lane;
+                const bool active = lane < m && k < kh;
+                const double th = __fma_rn((double)k, dt, t0);                           // t at my bin's upper endpoint
+                const double c_hi = (k >= S - 1) ? 1.0 : r6_rcp3(__dadd_rn(1.0, r6_exp_neg(th)));
+                const double c_lo = (k <= 0) ? 0.0 : r6_rcp3(__dadd_rn(1.0, r6_exp_neg(__dsub_rn(th, dt))));
+                const double z = __fma_rn(__dsub_rn(c_hi, c_lo), mult2, magic);
+                uint32_t raw = r6_raw(z);
+                const bool doubt = active && (r6_doubt(z, dmask) || raw < 0x80000000u);
+                if (__any_sync(FULL, doubt)) {                                           // rare: the exact function on the real endpoints
+                    const double m_ = (double)__shfl_sync(FULL, mu_w, j32), s_ = (double)__shfl_sync(FULL, sc_w, j32);
+                    const double rs = shfl_d(rs_w, j32);
+                    if (doubt) raw = r6_exact_pm(endp + i * ers, k, S, m_, s_, rs, mult) + 0x80000000u;
+                }
+                const uint32_t v = active ? (raw + 0x80000001u) + (k == bi ? rem : 0u) : 0u;   // :29 trunc, :32 +1, :35 remnant
+                uint32_t incl = v;
+                for (int o = 1; o < 32; o <<= 1) {
+                    const uint32_t t = __shfl_up_sync(FULL, incl, o);
+                    if (lane >= o) incl += t;
+                }
+                const uint32_t cex = __shfl_sync(FULL, base, chunk) + incl - v;          // integer cdf at my bin
+                const int js = 31 - __clz(__ballot_sync(FULL, active && cex <= mm));     // :61 searchsorted 'right' - 1
+                ps = __shfl_sync(FULL, v, js); cs = __shfl_sync(FULL, cex, js);
+                s = kl + chunk * m + js;
             }
-            const uint32_t v = active ? (raw + 0x80000001u) + (k == bi ? rem : 0u) : 0u;  // :29 trunc, :32 +1, :35 remnant
-            uint32_t incl = v;
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t t = __shfl_up_sync(FULL, incl, o);
-                if (lane >= o) incl += t;
-            }
-            const uint32_t cex = __shfl_sync(FULL, base, chunk) + incl - v;              // integer cdf at my bin
-            const int js = 31 - __clz(__ballot_sync(FULL, active && cex <= mm));         // :61 searchsorted 'right' - 1
-            ps = __shfl_sync(FULL, v, js); cs = __shfl_sync(FULL, cex, js);
-            s = kl + chunk * m + js;
+            if (lane == j32) my_sym = s;                                                 // :62
+            ws.decode(ps, cs, mm, bits, lane);                                           // :63-65
         }
-        if (lane == j32) my_sym = s;                                                     // :62
-        ws.decode(ps, cs, mm, bits, lane);                                               // :63-65
         if (j32 == 0 || ws.err) {
             const int64_t r = (i & ~(int64_t)31) + lane;
             if (r < L && r >= i) sy[r] = (int16_t)my_sym;
@@ -458,7 +465,7 @@ size_t bsw_rows6_scratch_bytes(int count, int64_t L) {
 
 int bsw_rows6_launch(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
                      int64_t sss, const double *endp, int64_t ers, const void *meta, int16_t *sym, int64_t L, int S, int bits,
-                     int q, void *scratch, size_t scratch_bytes, cudaStream_t st) {
+                     int q, void *scratch, size_t scratch_bytes, const int16_t *ext, cudaStream_t st) {
     BSW_REQUIRE(S >= 8 && S <= 1024 && (S & 3) == 0, "affine coder: support must be a multiple of 4 in [8, 1024]");
     BSW_REQUIRE(bits >= 8 && bits <= 31 && q >= 0 && q < bits, "affine coder: bits/quantbits out of range");
     BSW_REQUIRE(scratch_bytes >= (pop ? bsw_rows6_scratch_bytes(count, L) : (size_t)count * L * 16), "affine coder: scratch too small");
@@ -490,8 +497,9 @@ int bsw_rows6_launch(int phase, bool pop, bsw_streams *s, int first, int count, 
 #undef R6_LAUNCH
     } else {
         BSW_REQUIRE(pop, "affine coder: phase B of a push is k_push_pairs");
-        BSW_MAX_SHARED_ONCE(k_pop6);
-        k_pop6<<<(count + PW6 - 1) / PW6, PW6 * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, mt, mrs, bases, fix, sym, L, S, bits, q);
+        BSW_MAX_SHARED_ONCE(k_pop6<false>); BSW_MAX_SHARED_ONCE(k_pop6<true>);
+        if (ext) k_pop6<true><<<(count + PW6 - 1) / PW6, PW6 * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, mt, mrs, bases, fix, sym, L, S, bits, q, ext);
+        else k_pop6<false><<<(count + PW6 - 1) / PW6, PW6 * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, mt, mrs, bases, fix, sym, L, S, bits, q, nullptr);
     }
     BSW_LAUNCH_CHECK();
     return BSW_OK;

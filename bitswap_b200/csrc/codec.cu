@@ -53,7 +53,10 @@ int bsw_pop_shared_table(bsw_streams *s, int first, int count, const uint32_t *P
                          int16_t *sym, int64_t L, int S, int bits, cudaStream_t st);
 int bsw_logistic_2p(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
                     int64_t sss, const double *endp, int64_t ers, const void *meta, int16_t *sym, int64_t L, int S, int bits, int q,
-                    void *scratch, size_t scratch_bytes, cudaStream_t st);
+                    void *scratch, size_t scratch_bytes, const int16_t *ext, cudaStream_t st);
+int bsw_logistic_fused_ext(bool push, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
+                           int64_t sss, const double *endp, int64_t ers, int16_t *sym, int64_t L, int S, int bits, int q,
+                           const int16_t *ext, cudaStream_t st);
 
 __global__ void k_u8_to_i16(const uint8_t *__restrict__ in, int16_t *__restrict__ out, int64_t n) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -62,6 +65,29 @@ __global__ void k_u8_to_i16(const uint8_t *__restrict__ in, int16_t *__restrict_
 __global__ void k_i16_to_u8(const int16_t *__restrict__ in, uint8_t *__restrict__ out, int64_t n) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = (uint8_t)in[i];
+}
+
+// ---- partial edge blocks (bsw_codec_encode_ext / bsw_codec_decode_ext) ------------------------------------------------
+__device__ __forceinline__ bool extent_ok(int vh, int vw) { return vh >= 1 && vh <= 32 && vw >= 1 && vw <= 32; }
+// A stream whose extent lies outside [1, 32]^2 is flagged BSW_E_INVALID before any coder kernel of the call runs, so every
+// coder kernel skips it (WarpStream::open reads the flag); the first failure of a stream is kept.
+__global__ void k_check_extent(bsw_streams sv, int first, int count, const int16_t *__restrict__ ext) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < count && !extent_ok(ext[2 * i], ext[2 * i + 1]) && sv.flags[first + i] == 0) sv.flags[first + i] = BSW_E_INVALID;
+}
+// The fixed padding rule: pixel (c, r, col) outside the extent (vh, vw) takes the value of (c, min(r, vh-1), min(col, vw-1)),
+// i.e. np.pad(mode="edge") of the valid region.  Threads read only inside the extent and write only outside it.  Both
+// sides run it before infer(0) -- the encoder on the caller's pixels, the decoder on the popped ones -- so the nets see the
+// same block and the bitstream does not depend on what the caller left in the pad area.
+__global__ void k_pad_x(int16_t *__restrict__ x, const int16_t *__restrict__ ext, int64_t n, int xdim) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int64_t si = i / xdim;
+    const int d = (int)(i - si * xdim);
+    const int vh = ext[2 * si], vw = ext[2 * si + 1];
+    if (!extent_ok(vh, vw) || bsw_x_live(d, vh, vw)) return;
+    const int r = min((d >> 5) & 31, vh - 1), col = min(d & 31, vw - 1);
+    x[i] = x[i - d + (d & ~1023) + r * 32 + col];
 }
 
 extern "C" int bsw_codec_create(bsw_codec **out, bsw_model *m, bsw_bins *b, int max_batch) {
@@ -170,6 +196,7 @@ struct Ctx {
     bsw_codec *c; bsw_streams *s; int first, count;
     cudaStream_t conv, rows, ser;
     cudaStream_t caller = nullptr;
+    const int16_t *ext = nullptr;      // block extents of the pixel level, NULL = full 32x32 blocks
     int nl = 0;
     void begin(cudaStream_t user) {
         caller = user;
@@ -236,11 +263,13 @@ struct Ctx {
         const int64_t sss = x ? (c->m->d.cond_xscale ? c->xdim : 0) : c->zdim;
         const int cat_rows = x ? CAT_ROWS_X : CAT_ROWS_Z;
         const int cat_ser = x ? (pop ? CAT_POP_X : CAT_PUSH_X) : (pop ? CAT_POP_Z : CAT_PUSH_Z);
+        const int16_t *lext = x ? ext : nullptr;
         if (!c->two_phase) {
             hop(rows, ser);
             ++nl;
             c->prof.begin(cat_ser, ser);
-            int rc = pop ? bsw_logistic_pop(s, first, count, mu, L, sc, sss, endp, ers, sym, L, S, 31, q, ser)
+            int rc = lext ? bsw_logistic_fused_ext(!pop, s, first, count, mu, L, sc, sss, endp, ers, sym, L, S, 31, q, lext, ser)
+                   : pop ? bsw_logistic_pop(s, first, count, mu, L, sc, sss, endp, ers, sym, L, S, 31, q, ser)
                          : bsw_logistic_push(s, first, count, mu, L, sc, sss, endp, ers, sym, L, S, 31, q, ser);
             c->prof.end(ser);
             return rc;
@@ -251,14 +280,28 @@ struct Ctx {
         const size_t scr_bytes = (!pop && c->dual_stream) ? c->scratch_push_bytes : c->scratch_bytes;
         nl += 2;
         c->prof.begin(cat_rows, rows);
-        int rc = bsw_logistic_2p(0, pop, s, first, count, mu, L, sc, sss, endp, ers, meta, sym, L, S, 31, q, scr, scr_bytes, rows);
+        int rc = bsw_logistic_2p(0, pop, s, first, count, mu, L, sc, sss, endp, ers, meta, sym, L, S, 31, q, scr, scr_bytes, nullptr, rows);
         c->prof.end(rows);
         if (rc) return rc;
         hop(rows, ser);
         c->prof.begin(cat_ser, ser);
-        rc = bsw_logistic_2p(1, pop, s, first, count, mu, L, sc, sss, endp, ers, meta, sym, L, S, 31, q, scr, scr_bytes, ser);
+        rc = bsw_logistic_2p(1, pop, s, first, count, mu, L, sc, sss, endp, ers, meta, sym, L, S, 31, q, scr, scr_bytes, lext, ser);
         c->prof.end(ser);
         return rc;
+    }
+    // extents: flag bad ones on the serial stream before its first coder kernel; pad xsym where xsym is produced (conv)
+    int check_ext() {
+        ++nl;
+        k_check_extent<<<(count + 255) / 256, 256, 0, ser>>>(*s, first, count, ext);
+        BSW_LAUNCH_CHECK();
+        return BSW_OK;
+    }
+    int pad_x() {
+        ++nl;
+        const int64_t n = (int64_t)count * c->xdim;
+        k_pad_x<<<(unsigned)((n + 255) / 256), 256, 0, conv>>>(c->xsym, ext, n, c->xdim);
+        BSW_LAUNCH_CHECK();
+        return BSW_OK;
     }
     int push_prior(const int16_t *sym) {
         ++nl;
@@ -310,20 +353,37 @@ static int ensure_zs(bsw_codec *c) {
 // back to back while the float64 table kernels of the push run beside infer(zi+1) on the rows stream: tensor-pipe work
 // and FP64-pipe work of ONE chain share the SMs (the persistent conv kernel leaves room for a table CTA on every SM).
 // Buffers that make this legal: separate (mu, sigma) for the two nets, separate scratch for the push rows.
-extern "C" int bsw_codec_encode(bsw_codec *c, bsw_streams *s, int first, int count, const uint8_t *x, int scheme, void *stream) {
+// ext (the _ext entry points): int16 [count][2] block extents (vh, vw) of the pixel level on the device, NULL = full blocks.
+static int codec_ext_ok(bsw_codec *c, const int16_t *ext) {
+    BSW_REQUIRE(!ext || c->xdim % 1024 == 0, "bsw_codec: block extents need 32x32 image blocks");
+    return BSW_OK;
+}
+
+extern "C" int bsw_codec_encode_ext(bsw_codec *c, bsw_streams *s, int first, int count, const uint8_t *x, const int16_t *ext,
+                                    int scheme, void *stream) {
     RC(codec_args_ok(c, s, first, count, x));
+    RC(codec_ext_ok(c, ext));
     Ctx k{c, s, first, count};
+    k.ext = ext;
     k.begin((cudaStream_t)stream);
     const int nz = c->nz;
     int64_t nx = (int64_t)count * c->xdim;
-    k_u8_to_i16<<<(unsigned)((nx + 255) / 256), 256, 0, k.rows>>>(x, c->xsym, nx);       // (read by the push_x table kernel)
-    BSW_LAUNCH_CHECK();
+    if (ext) {
+        // the nets read the padded pixels, so they are gathered from xsym on the conv stream instead of from x
+        RC(k.check_ext());
+        k_u8_to_i16<<<(unsigned)((nx + 255) / 256), 256, 0, k.conv>>>(x, c->xsym, nx);
+        BSW_LAUNCH_CHECK();
+        RC(k.pad_x());
+    } else {
+        k_u8_to_i16<<<(unsigned)((nx + 255) / 256), 256, 0, k.rows>>>(x, c->xsym, nx);   // (read by the push_x table kernel)
+        BSW_LAUNCH_CHECK();
+    }
     ++k.nl;
     int16_t *zsym = c->sym[0], *ztop = c->sym[1];
     if (scheme == 0) {
         // Bit-Swap sender (cifar_compress.py:178-204)
         for (int zi = 0; zi < nz; ++zi) {
-            if (zi == 0) RC(k.gather_x(x)); else RC(k.gather_z(zi - 1, zsym));           // :180
+            if (zi == 0) RC(ext ? k.gather_x16(c->xsym) : k.gather_x(x)); else RC(k.gather_z(zi - 1, zsym));   // :180
             RC(k.net(true, zi));                                                            // :181
             k.hop(k.conv, k.rows);
             RC(k.level(true, zi, true, ztop));                                              // :182-187
@@ -339,7 +399,7 @@ extern "C" int bsw_codec_encode(bsw_codec *c, bsw_streams *s, int first, int cou
         // BB-ANS sender (cifar_compress.py:208-242): all pops first, then all pushes
         RC(ensure_zs(c));
         for (int zi = 0; zi < nz; ++zi) {
-            if (zi == 0) RC(k.gather_x(x)); else RC(k.gather_z(zi - 1, c->zs[zi - 1]));
+            if (zi == 0) RC(ext ? k.gather_x16(c->xsym) : k.gather_x(x)); else RC(k.gather_z(zi - 1, c->zs[zi - 1]));
             RC(k.net(true, zi));
             k.hop(k.conv, k.rows);
             RC(k.level(true, zi, true, c->zs[zi]));
@@ -360,13 +420,20 @@ extern "C" int bsw_codec_encode(bsw_codec *c, bsw_streams *s, int first, int cou
     c->launches = k.nl;
     return BSW_OK;
 }
+extern "C" int bsw_codec_encode(bsw_codec *c, bsw_streams *s, int first, int count, const uint8_t *x, int scheme, void *stream) {
+    return bsw_codec_encode_ext(c, s, first, count, x, nullptr, scheme, stream);
+}
 
-extern "C" int bsw_codec_decode(bsw_codec *c, bsw_streams *s, int first, int count, uint8_t *x, int scheme, void *stream) {
+extern "C" int bsw_codec_decode_ext(bsw_codec *c, bsw_streams *s, int first, int count, uint8_t *x, const int16_t *ext,
+                                    int scheme, void *stream) {
     RC(codec_args_ok(c, s, first, count, x));
+    RC(codec_ext_ok(c, ext));
     Ctx k{c, s, first, count};
+    k.ext = ext;
     k.begin((cudaStream_t)stream);
     const int nz = c->nz;
     int16_t *ztop = c->sym[0], *sym = c->sym[1];
+    if (ext) RC(k.check_ext());
     if (scheme == 0) {
         // Bit-Swap receiver (cifar_compress.py:283-317)
         RC(k.pop_prior(ztop));                                                              // :284-289
@@ -377,6 +444,7 @@ extern "C" int bsw_codec_decode(bsw_codec *c, bsw_streams *s, int first, int cou
             k.hop(k.conv, k.rows);
             RC(k.level(true, zi == 0 ? -1 : zi - 1, false, zi == 0 ? c->xsym : sym));       // :298-303
             k.hop(k.ser, k.conv);
+            if (zi == 0 && ext) RC(k.pad_x());                                              // popped pixels -> padded block
             if (zi == 0) RC(k.gather_x16(c->xsym)); else RC(k.gather_z(zi - 1, sym));       // :306
             RC(k.net(true, zi));                                                            // :307
             k.hop(k.conv, k.rows);
@@ -395,6 +463,7 @@ extern "C" int bsw_codec_decode(bsw_codec *c, bsw_streams *s, int first, int cou
             RC(k.level(true, zi == 0 ? -1 : zi - 1, false, zi == 0 ? c->xsym : c->zs[zi - 1]));
             k.hop(k.ser, k.conv);
         }
+        if (ext) RC(k.pad_x());                                                             // popped pixels -> padded block
         for (int zi = nz - 1; zi >= 0; --zi) {
             if (zi == 0) RC(k.gather_x16(c->xsym)); else RC(k.gather_z(zi - 1, c->zs[zi - 1]));
             RC(k.net(true, zi));
@@ -409,4 +478,7 @@ extern "C" int bsw_codec_decode(bsw_codec *c, bsw_streams *s, int first, int cou
     k.end();
     c->launches = k.nl + 1;
     return BSW_OK;
+}
+extern "C" int bsw_codec_decode(bsw_codec *c, bsw_streams *s, int first, int count, uint8_t *x, int scheme, void *stream) {
+    return bsw_codec_decode_ext(c, s, first, count, x, nullptr, scheme, stream);
 }

@@ -219,7 +219,8 @@ class StreamSet:
         if (f == 1).any():
             raise IndexError(f"pop from empty ANS stack (streams {np.nonzero(f == 1)[0][:8].tolist()})")   # cifar_compress.py:65
         if (f == 4).any():
-            raise IndexError(f"symbol outside the table's support (streams {np.nonzero(f == 4)[0][:8].tolist()})")   # P[i, s] in the reference
+            raise IndexError(f"symbol outside the table's support or block extent outside [1, 32] x [1, 32] "     # P[i, s] in the reference
+                             f"(streams {np.nonzero(f == 4)[0][:8].tolist()})")
         if (f == 2).any():
             raise OverflowError(f"ANS word-stack capacity exhausted (streams {np.nonzero(f == 2)[0][:8].tolist()})")
         if (f != 0).any():

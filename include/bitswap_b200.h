@@ -312,6 +312,17 @@ int bsw_codec_encode(bsw_codec *c, bsw_streams *s, int first, int count, const u
                      void *stream);
 int bsw_codec_decode(bsw_codec *c, bsw_streams *s, int first, int count, uint8_t *x_dev, int scheme,
                      void *stream);
+/* The same calls for partial edge blocks of a larger image.  extent_dev int16 [count][2] on the device, indexed like x_dev:
+ * the block's valid extent (vh, vw) in [1, 32]^2; NULL = full blocks (then identical to bsw_codec_encode/decode).
+ * Only the pixel level changes: dims (c, r, col) with r >= vh or col >= vw are neither pushed nor popped (the order and
+ * the tables of the coded dims are those of a full call), and before infer(0) both sides fill them by edge replication,
+ * (c, min(r, vh-1), min(col, vw-1)) -- np.pad(mode="edge") of the valid region -- so the bitstream does not depend on
+ * what the caller left there.  The decoder writes the padded blocks to x_dev.  A stream with an extent outside
+ * [1, 32]^2 is flagged BSW_E_INVALID and left uncoded; the other streams are unaffected.  Needs xs = (C, 32, 32). */
+int bsw_codec_encode_ext(bsw_codec *c, bsw_streams *s, int first, int count, const uint8_t *x_dev,
+                         const int16_t *extent_dev, int scheme, void *stream);
+int bsw_codec_decode_ext(bsw_codec *c, bsw_streams *s, int first, int count, uint8_t *x_dev,
+                         const int16_t *extent_dev, int scheme, void *stream);
 /* Number of kernel launches the last encode/decode call enqueued (bench.py's gpu_launches). */
 int64_t bsw_codec_last_launches(const bsw_codec *c);
 /* Stream placement inside one encode/decode call: 0 (default) = every kernel on the caller's stream; 1 = conv kernels
