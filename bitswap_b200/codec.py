@@ -16,13 +16,23 @@ from .model import Model
 from .streams import StreamSet
 
 BITSWAP, BBANS = 0, 1
+MAX_QUANTBITS = 12          # widest latent support of the device codec: 4096 bins
+FUSED_MAX_SUPPORT = 1024    # the fused coder keeps a row table in one warp's registers
+
+
+def check_quantbits(q):
+    """ValueError unless 1 <= q <= MAX_QUANTBITS (raised before any device work)."""
+    if not (isinstance(q, (int, np.integer)) and 1 <= int(q) <= MAX_QUANTBITS):
+        raise ValueError(f"quantbits must be an integer in [1, {MAX_QUANTBITS}], got {q!r}")
 
 
 class Bins:
     """Device copy of the discretisation tables (zendpoints [nz,zdim,2^q-1], zcentres [nz,zdim,2^q],
-    the layout discretize() returns, discretization.py:99)."""
+    the layout discretize() returns, discretization.py:99).  quantbits 1 to 12: up to 4096 bins per latent dimension
+    (at 12, cifar8's bins take 1.07 GB of device memory)."""
 
     def __init__(self, cfg: CodecConfig, zendpoints, zcentres, device=None):
+        check_quantbits(cfg.quantbits)
         self.device = device_index(device)
         ze = np.ascontiguousarray(zendpoints.detach().cpu().numpy() if torch.is_tensor(zendpoints) else zendpoints, dtype=np.float64)
         zc = np.ascontiguousarray(zcentres.detach().cpu().numpy() if torch.is_tensor(zcentres) else zcentres, dtype=np.float64)
@@ -127,7 +137,11 @@ class BitSwapCodec:
         check(lib().bsw_codec_set_dual_stream(self._h, int(on)))
 
     def set_two_phase(self, on=True):
-        """True (default): parallel row-table kernel + serial coder; False: fused one-warp-per-stream kernels."""
+        """True (default): parallel row-table kernel + serial coder; False: fused one-warp-per-stream kernels, which hold a
+        row's table in registers and so take at most 1024 bins (quantbits <= 10): ValueError above that."""
+        if not on and self.cfg.zsupport > FUSED_MAX_SUPPORT:
+            raise ValueError(f"set_two_phase(False): the fused coder takes at most {FUSED_MAX_SUPPORT} bins per row, these bins "
+                             f"have {self.cfg.zsupport} (quantbits {self.cfg.quantbits}); keep the two-phase coder")
         check(lib().bsw_codec_set_two_phase(self._h, int(on)))
 
     def profile(self, enable=-1):
@@ -213,6 +227,9 @@ class PipelinedCodec:
         return out
 
     def set_two_phase(self, on=True):
+        if not on and self.cfg.zsupport > FUSED_MAX_SUPPORT:
+            raise ValueError(f"set_two_phase(False): the fused coder takes at most {FUSED_MAX_SUPPORT} bins per row, these bins "
+                             f"have {self.cfg.zsupport} (quantbits {self.cfg.quantbits}); keep the two-phase coder")
         for c in self.codecs:
             c.set_two_phase(on)
 

@@ -858,7 +858,7 @@ static int dispatch_fused(bool push, bsw_streams *s, int first, int count, const
         case 512:  return launch_fused<16>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext, st);
         case 1024: return launch_fused<32>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext, st);
     }
-    bsw_set_error("fused coder: support must be one of 32,64,...,1024 (got %d)", S);
+    bsw_set_error("fused coder: support must be one of 32,64,...,1024 (got %d; wider supports need the two-phase coder)", S);
     return BSW_E_INVALID;
 }
 extern "C" int bsw_logistic_push(bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
@@ -884,7 +884,9 @@ int bsw_logistic_fused_ext(bool push, bsw_streams *s, int first, int count, cons
 int bsw_rows6_build_meta(const double *endp, int64_t ers, int64_t L, int S, void *meta_dev, int *n_affine_host, cudaStream_t st);   // ans_rows6.cu
 extern "C" int bsw_bins_create(bsw_bins **out, int nz, int zdim, int q, int xdim, const double *zend_host,
                                const double *zcen_host) {
-    BSW_REQUIRE(out && nz > 0 && zdim > 0 && q > 0 && q <= 10 && zend_host && zcen_host, "bsw_bins_create: bad arguments");
+    // q <= 12: supports up to 4096 bins, coded by the two-phase kernels (the fused ones stop at 1024, see
+    // bsw_codec_set_two_phase).  At q = 12 the eight 2048-dim levels of cifar8 hold 2 x 8 x 2048 x 4096 doubles: 1.07 GB.
+    BSW_REQUIRE(out && nz > 0 && zdim > 0 && q > 0 && q <= 12 && zend_host && zcen_host, "bsw_bins_create: bad arguments");
     bsw_bins *b = new bsw_bins();
     b->nz = nz; b->zdim = zdim; b->q = q; b->S = 1 << q; b->xdim = xdim;
     const int S = b->S;

@@ -388,6 +388,254 @@ __global__ void __launch_bounds__(BW * 32) k_pop_coarse(bsw_streams sv, int firs
     ws.close(sv, b, lane);
 }
 
+// ---- wide supports (S = 32 * 32 * NP = 2048 or 4096: quantbits 11 and 12) ----------------------------------------------
+// A lane cannot keep NB = S/32 = 64 or 128 float64 endpoints in registers, and 128 chunk bases per row would make the pop
+// scratch four times larger.  So lane l owns the pop chunk l -- the CH = S/32 consecutive bins [l*CH, l*CH + CH) -- and walks
+// it in NP passes of 32 bins.  Pass p stages the 32 x 32 endpoints {l*CH + p*32 + j} into the same padded tile as k_rows<32>,
+// runs the same 4-bin groups on them and carries the lane's running sum, its first maximum and (push) its prefix below the
+// symbol into the next pass.  The screening test and the exact fallback are those of k_rows; the chunk bases are the
+// lane-exclusive prefix sums, 32 per row as for S <= 1024.
+__device__ __noinline__ uint32_t rows_exact_pm_g(const double *__restrict__ e, int k, int S, double m, double s, double rs, double mult) {
+    const double c = (k == S - 1) ? 1.0 : bsw_cdf_fast(__ldg(e + k), m, s, rs);    // (the row's last bin: cdf = 1, :184)
+    const double p = (k == 0) ? 0.0 : bsw_cdf_fast(__ldg(e + k - 1), m, s, rs);
+    return __double2uint_rz(__dmul_rn(__dsub_rn(c, p), mult));
+}
+
+template <int NP, bool POP, bool APX>
+__global__ void __launch_bounds__(RW * 32, 2) k_rows_wide(int count, int64_t L, const float *__restrict__ mu, int64_t mss,
+        const float *__restrict__ sc, int64_t sss, const double *__restrict__ endp, int64_t ers,
+        const int16_t *__restrict__ sym, int bits, int q, uint4 *__restrict__ pairs, uint32_t *__restrict__ coarse,
+        uint2 *__restrict__ fix, const BswApxRegs KA) {
+    constexpr int NB = 32;                               // bins per lane and pass
+    constexpr int CH = NB * NP;                          // bins per lane = one pop chunk
+    constexpr int S = 32 * CH;
+    constexpr int G = 4;
+    using RT = RowTile<NB>;
+    __shared__ __align__(16) double tile[RT::DOUBLES];
+    __shared__ __align__(16) double t32[APX ? BSW_APX_TABLE_DOUBLES : 2];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t row = blockIdx.x;
+    const int si = blockIdx.y * RW + warp;
+    const bool live = si < count;                        // every warp stages every pass: no warp leaves before the last barrier
+    const double *e = endp + row * ers;
+    if (APX) bsw_apx_table_fill(t32, threadIdx.x, RW * 32);
+    const double m = live ? (double)mu[(int64_t)si * mss + row] : 0.0, s = live ? (double)sc[(int64_t)si * sss + row] : 1.0;
+    const double rs = __ddiv_rn(1.0, s);
+    const double mult = (double)(((int64_t)1 << bits) - ((int64_t)1 << q));
+    const double mult2 = mult * 1048576.0;
+    const double magic2 = 6755399441055744.0 + (double)BSW_APX_WINDOW;
+    int sy = 0;
+    if (!POP && live) sy = (int)sym[(int64_t)si * L + row];
+    const int owner = sy / CH, js = sy - owner * CH;     // push: lane and in-chunk position of the coded symbol
+
+    BswExpRegs K;
+    if (!APX) K.load();
+    const double *my = tile + lane * RT::STRIDE;
+    const uint32_t tl = smem_u32r(t32) + 8u * lane;
+    bool wide = true;                                    // (|t| > 690 somewhere in the row: the clamped loop, as in k_rows)
+    if (APX) {
+        const double t_lo = __dmul_rn(__dsub_rn(__ldg(e), m), rs);
+        const double t_hi = __dmul_rn(__dsub_rn(__ldg(e + S - 2), m), rs);
+        wide = !(fabs(t_lo) <= 690.0 && fabs(t_hi) <= 690.0);
+    }
+    auto cdf_at = [&](int j, auto clampc) -> double {
+        if (APX) return bsw_cdf_apx<decltype(clampc)::value>(my[j], m, rs, tl, KA);
+        return bsw_cdf_fast_regs(my[j], m, s, rs, K);
+    };
+    // lower edge of my first bin: the upper endpoint of the previous lane's chunk, evaluated from global memory
+    double prev = 0.0;
+    if (lane > 0) prev = APX ? bsw_cdf_apx<true>(__ldg(e + lane * CH - 1), m, rs, tl, KA) : bsw_cdf_fast_regs(__ldg(e + lane * CH - 1), m, s, rs, K);
+    uint32_t lsum = 0, lbest = 0, pre = 0, pv = 0;
+    uint32_t bestv[G];
+    int bestj0 = 0;
+#pragma unroll
+    for (int t = 0; t < G; ++t) bestv[t] = 0;
+    for (int p = 0; p < NP; ++p) {
+        if (p) __syncthreads();                          // every warp is done with the previous pass's tile
+        for (int kk = threadIdx.x; kk < 32 * NB; kk += RW * 32)
+            tile[(kk / NB) * RT::STRIDE + (kk % NB)] = __ldg(e + (kk / NB) * CH + p * NB + (kk % NB));
+        __syncthreads();
+        if (!live) continue;
+        const bool row_end = lane == 31 && p == NP - 1;  // the row's last bin: upper cdf = 1 exactly (:184)
+        const int kbase = lane * CH + p * NB;            // global index of this pass's first bin of mine
+        const int jsp = js - p * NB;                     // the symbol's position relative to this pass (may lie outside it)
+        auto group = [&](int j0, auto clampc) {
+            uint32_t vv[G];
+            bool doubt[G];
+            bool any = false;
+            uint32_t all_hi = 0x80000000u;
+#pragma unroll
+            for (int t = 0; t < G; ++t) {
+                double c = cdf_at(j0 + t, clampc);
+                if (t == G - 1 && row_end && j0 + t == NB - 1) c = 1.0;
+                if (APX) {
+                    const double z = __fma_rn(__dsub_rn(c, prev), mult2, magic2);
+                    const uint32_t raw = __funnelshift_r((uint32_t)__double2loint(z), (uint32_t)__double2hiint(z), 20);
+                    doubt[t] = ((uint32_t)__double2loint(z) & (0xfffffu & ~(2u * BSW_APX_WINDOW - 1u))) == 0u && raw != 0x80000000u;
+                    any |= doubt[t];
+                    all_hi &= raw;
+                    vv[t] = raw + 0x80000001u;                                             // :29 trunc, :32 +1
+                } else {
+                    vv[t] = __double2uint_rz(__dmul_rn(__dsub_rn(c, prev), mult)) + 1u;
+                }
+                prev = c;
+            }
+            if (APX && (any || !(all_hi & 0x80000000u))) {
+                const bool all = !(all_hi & 0x80000000u);
+#pragma unroll
+                for (int t = 0; t < G; ++t)
+                    if (doubt[t] || all) vv[t] = rows_exact_pm_g(e, kbase + j0 + t, S, m, s, rs, mult) + 1u;
+            }
+            uint32_t gsum = 0, gmax = 0;
+#pragma unroll
+            for (int t = 0; t < G; ++t) { gsum += vv[t]; gmax = max(gmax, vv[t]); }
+            lsum += gsum;
+            if (gmax > lbest) {                           // strict: the earlier group keeps a tie (:35 first maximum)
+                lbest = gmax; bestj0 = p * NB + j0;
+#pragma unroll
+                for (int t = 0; t < G; ++t) bestv[t] = vv[t];
+            }
+            if (!POP) {
+                if (j0 + G <= jsp) pre += gsum;
+                else if (j0 <= jsp) {
+#pragma unroll
+                    for (int t = 0; t < G; ++t) {
+                        pre += (j0 + t < jsp) ? vv[t] : 0u;
+                        if (j0 + t == jsp) pv = vv[t];
+                    }
+                }
+            }
+        };
+        if (wide) {
+#pragma unroll 1
+            for (int j0 = 0; j0 < NB; j0 += G) group(j0, std::true_type{});
+        } else {
+#pragma unroll 1
+            for (int j0 = 0; j0 < NB; j0 += G) group(j0, std::false_type{});
+        }
+    }
+    if (!live) return;
+    int lbi = bestj0;
+#pragma unroll
+    for (int t = G - 1; t >= 0; --t) if (bestv[t] == lbest) lbi = bestj0 + t;
+    uint32_t incl = lsum;
+    for (int o = 1; o < 32; o <<= 1) {
+        uint32_t t = __shfl_up_sync(FULL, incl, o);
+        if (lane >= o) incl += t;
+    }
+    const uint32_t total = __shfl_sync(FULL, incl, 31);
+    const uint32_t rowmax = __reduce_max_sync(FULL, lbest);
+    const int wl = __ffs(__ballot_sync(FULL, lbest == rowmax)) - 1;
+    const int bi = __shfl_sync(FULL, lane * CH + lbi, wl);
+    const uint32_t rem = (1u << bits) - total;
+    const int64_t out = (int64_t)si * L + row;
+    if (POP) {
+        coarse[out * 32 + lane] = incl - lsum + ((lane * CH > bi) ? rem : 0u);
+        if (lane == 0) fix[out] = make_uint2((uint32_t)bi, rem);
+    } else {
+        const uint32_t cb = __shfl_sync(FULL, incl - lsum + pre, owner & 31);
+        const uint32_t pb = __shfl_sync(FULL, pv, owner & 31);
+        if (lane == 0) {
+            const uint32_t pf = pb + (bi == sy ? rem : 0u);
+            const uint64_t M = pf == 1u ? ~0ull : ~0ull / (uint64_t)pf;
+            if ((unsigned)sy >= (unsigned)S) pairs[out] = make_uint4(0u, 0u, 0u, 0u);   // out-of-range symbol: flagged by the serial phase
+            else pairs[out] = make_uint4(pf, cb + (bi < sy ? rem : 0u), (uint32_t)M, (uint32_t)(M >> 32));
+        }
+    }
+}
+
+// Pop of the wide generic rows: the ballot over the 32 chunk bases picks the chunk, which is then walked in sub-chunks of
+// 32 bins with the cdf carried between them (same per-bin arithmetic as k_pop_coarse).
+template <int NP, bool MASK>
+__global__ void __launch_bounds__(BW * 32) k_pop_coarse_wide(bsw_streams sv, int first, int count, const float *__restrict__ mu,
+        int64_t mss, const float *__restrict__ sc, int64_t sss, const double *__restrict__ endp, int64_t ers,
+        const uint32_t *__restrict__ coarse, const uint2 *__restrict__ fix, int16_t *__restrict__ sym, int64_t L,
+        int bits, int q, const int16_t *__restrict__ ext) {
+    constexpr int CH = 32 * NP, S = 32 * CH;
+    const int lane = threadIdx.x & 31;
+    const int si = blockIdx.x * BW + (threadIdx.x >> 5);
+    if (si >= count) return;
+    const int b = first + si;
+    WarpStream2 ws;
+    ws.open(sv, b);
+    if (ws.err) return;
+    int vh = 32, vw = 32;
+    if (MASK) { vh = ext[2 * si]; vw = ext[2 * si + 1]; }
+    const float *mub = mu + (int64_t)si * mss, *scb = sc + (int64_t)si * sss;
+    const uint32_t *cb = coarse + (int64_t)si * L * 32;
+    const uint2 *fb = fix + (int64_t)si * L;
+    int16_t *sy = sym + (int64_t)si * L;
+    const double mult = (double)(((int64_t)1 << bits) - ((int64_t)1 << q));
+    const uint32_t mask = (uint32_t)(((uint64_t)1 << bits) - 1);
+    float mu_w = 0.f, sc_w = 1.f;
+    uint2 fx_w = make_uint2(0, 0);
+    int my_sym = 0;
+    float mu_nx, sc_nx;
+    uint2 fx_nx;
+    {
+        int64_t r = ((L - 1) & ~(int64_t)31) + lane;
+        mu_nx = r < L ? mub[r] : 0.f;
+        sc_nx = r < L ? scb[r] : 1.f;
+        fx_nx = r < L ? __ldg(fb + r) : make_uint2(0, 0);
+    }
+    uint32_t base_n1 = __ldg(cb + (L - 1) * 32 + lane);
+    uint32_t base_n2 = L > 1 ? __ldg(cb + (L - 2) * 32 + lane) : 0xffffffffu;
+    for (int64_t i = L - 1; i >= 0; --i) {
+        const int j32 = (int)(i & 31);
+        const bool new_block = (j32 == 31 || i == L - 1);
+        if (new_block) { mu_w = mu_nx; sc_w = sc_nx; fx_w = fx_nx; }
+        const double m_ = (double)__shfl_sync(FULL, mu_w, j32), s_ = (double)__shfl_sync(FULL, sc_w, j32);
+        const int bi = (int)__shfl_sync(FULL, fx_w.x, j32);
+        const uint32_t rem = __shfl_sync(FULL, fx_w.y, j32);
+        if (new_block) {
+            int64_t r = (i & ~(int64_t)31) - 32 + lane;
+            mu_nx = r >= 0 ? mub[r] : 0.f;
+            sc_nx = r >= 0 ? scb[r] : 1.f;
+            fx_nx = r >= 0 ? __ldg(fb + r) : make_uint2(0, 0);
+        }
+        const uint32_t base = base_n1;
+        base_n1 = base_n2;
+        if (i > 1) base_n2 = __ldg(cb + (i - 2) * 32 + lane);
+        if (!MASK || bsw_x_live(i, vh, vw)) {
+            const double rs = __ddiv_rn(1.0, s_);
+            const uint32_t mm = (uint32_t)ws.x & mask;                                   // cifar_compress.py:60
+            const int chunk = 31 - __clz(__ballot_sync(FULL, base <= mm));
+            const double *e = endp + i * ers;
+            uint32_t carry = __shfl_sync(FULL, base, chunk), ps = 1u, cs = 0u;
+            int s = 0;
+#pragma unroll 1
+            for (int sub = 0; sub < NP; ++sub) {
+                const int k = chunk * CH + sub * 32 + lane;
+                const double c_hi = (k == S - 1) ? 1.0 : bsw_cdf_fast(__ldg(e + k), m_, s_, rs);
+                const double c_lo = (k == 0) ? 0.0 : bsw_cdf_fast(__ldg(e + k - 1), m_, s_, rs);
+                const uint32_t v = __double2uint_rz(__dmul_rn(__dsub_rn(c_hi, c_lo), mult)) + 1u + (k == bi ? rem : 0u);
+                uint32_t incl = v;
+                for (int o = 1; o < 32; o <<= 1) {
+                    uint32_t t = __shfl_up_sync(FULL, incl, o);
+                    if (lane >= o) incl += t;
+                }
+                const uint32_t cex = carry + incl - v;
+                const uint32_t next = carry + __shfl_sync(FULL, incl, 31);
+                if (sub == NP - 1 || next > mm) {                                        // the symbol is in this sub-chunk
+                    const int js = 31 - __clz(__ballot_sync(FULL, cex <= mm));           // :61 searchsorted 'right' - 1
+                    ps = __shfl_sync(FULL, v, js); cs = __shfl_sync(FULL, cex, js);
+                    s = chunk * CH + sub * 32 + js;
+                    break;
+                }
+                carry = next;
+            }
+            if (lane == j32) my_sym = s;                                                 // :62
+            ws.decode(ps, cs, mm, bits, lane);                                           // :63-65
+        }
+        if (j32 == 0 || ws.err) {
+            int64_t r = (i & ~(int64_t)31) + lane;
+            if (r < L && r >= i) sy[r] = (int16_t)my_sym;
+            if (ws.err) break;
+        }
+    }
+    ws.close(sv, b, lane);
+}
+
 // ---- phase B: pop from the full integer table (small batches) --------------------------------------------------------
 // Same search as k_pop_coarse, but the 32 integer pmfs of the chosen chunk are read back from phase A's table instead of
 // being recomputed: no float64 on the serial path (per row: coarse cdf [prefetched] -> ballot -> one 128-byte load ->
@@ -504,6 +752,38 @@ int launch_rows(int phase, bool pop, bsw_streams *s, int first, int count, const
     return BSW_OK;
 }
 
+// S = 2048 (NP = 2) or 4096 (NP = 4); same scratch layout as launch_rows<32>: 32 chunk bases per row, then the fix words
+template <int NP>
+int launch_rows_wide(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
+                     int64_t sss, const double *endp, int64_t ers, int16_t *sym, int64_t L, int bits, int q, void *scratch,
+                     const int16_t *ext, cudaStream_t st) {
+    dim3 grid((unsigned)L, (count + RW - 1) / RW);
+    uint4 *pairs = (uint4 *)scratch;
+    uint32_t *coarse = (uint32_t *)scratch;
+    uint2 *fix = (uint2 *)((uint8_t *)scratch + (size_t)count * L * 32 * 4);
+    const BswApxRegs kp = bsw_apx_params();
+    static const bool env_exact = getenv("BSW_ROWS_EXACT") && getenv("BSW_ROWS_EXACT")[0] == '1';
+    const bool exact = bits > 31 || env_exact;
+    BSW_MAX_SHARED_ONCE((k_rows_wide<NP, true, false>)); BSW_MAX_SHARED_ONCE((k_rows_wide<NP, true, true>));
+    BSW_MAX_SHARED_ONCE((k_rows_wide<NP, false, false>)); BSW_MAX_SHARED_ONCE((k_rows_wide<NP, false, true>));
+    BSW_MAX_SHARED_ONCE((k_pop_coarse_wide<NP, false>)); BSW_MAX_SHARED_ONCE((k_pop_coarse_wide<NP, true>));
+    if (phase == 0) {
+        if (pop) {
+            if (exact) k_rows_wide<NP, true, false><<<grid, RW * 32, 0, st>>>(count, L, mu, mss, sc, sss, endp, ers, nullptr, bits, q, nullptr, coarse, fix, kp);
+            else k_rows_wide<NP, true, true><<<grid, RW * 32, 0, st>>>(count, L, mu, mss, sc, sss, endp, ers, nullptr, bits, q, nullptr, coarse, fix, kp);
+        } else {
+            if (exact) k_rows_wide<NP, false, false><<<grid, RW * 32, 0, st>>>(count, L, mu, mss, sc, sss, endp, ers, sym, bits, q, pairs, nullptr, nullptr, kp);
+            else k_rows_wide<NP, false, true><<<grid, RW * 32, 0, st>>>(count, L, mu, mss, sc, sss, endp, ers, sym, bits, q, pairs, nullptr, nullptr, kp);
+        }
+    } else {
+        if (!pop) return launch_push_pairs(s, first, count, pairs, L, bits, ext, st);
+        if (ext) k_pop_coarse_wide<NP, true><<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, coarse, fix, sym, L, bits, q, ext);
+        else k_pop_coarse_wide<NP, false><<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, coarse, fix, sym, L, bits, q, nullptr);
+    }
+    BSW_LAUNCH_CHECK();
+    return BSW_OK;
+}
+
 }  // namespace
 
 // Pop from ONE materialised table shared by every stream (the Logistic(0,1) prior): P [L][S] with the remnant already
@@ -542,7 +822,7 @@ int bsw_rows6_launch(int phase, bool pop, bsw_streams *s, int first, int count, 
                      int q, void *scratch, size_t scratch_bytes, const int16_t *ext, cudaStream_t st);
 
 // Scratch bytes of the two-phase coder for `count` streams of L rows: per row 16 B (push: P, C, reciprocal) or
-// 136 B (pop: 32 chunk bases + argmax/remnant), whichever kernel family runs.
+// 136 B (pop: 32 chunk bases + argmax/remnant), whichever kernel family runs and for every support up to 4096.
 size_t bsw_rows_scratch_bytes(int count, int64_t L) { return (size_t)count * L * 136; }
 
 // Two-phase variants of bsw_logistic_push / bsw_logistic_pop (same arguments + caller-provided scratch).
@@ -569,8 +849,10 @@ int bsw_logistic_2p(int phase, bool pop, bsw_streams *s, int first, int count, c
         case 256:  return launch_rows<8>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
         case 512:  return launch_rows<16>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
         case 1024: return launch_rows<32>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
+        case 2048: return launch_rows_wide<2>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
+        case 4096: return launch_rows_wide<4>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
     }
-    bsw_set_error("two-phase coder: support must be one of 32,64,...,1024 (got %d)", S);
+    bsw_set_error("two-phase coder: support must be one of 32,64,...,4096 (got %d)", S);
     return BSW_E_INVALID;
 }
 

@@ -45,6 +45,16 @@ __device__ __noinline__ double r6_slow_pmf(const float *__restrict__ mu, int64_t
     const double m = (double)mu[(int64_t)si * mss + row], s = (double)sc[(int64_t)si * sss + row];
     return r6_exact_pmf(endp + row * ers, k, S, m, s, __ddiv_rn(1.0, s));
 }
+// Re-anchor of a wide walk's chain: exp(-t) at endpoint k - 1, with t0 and dt derived exactly as r6_plan derives them.  Same
+// by-value style as r6_slow_pmf, so that the hot loop does not keep t0 and dt alive.
+__device__ __noinline__ double r6_anchor(const float *__restrict__ mu, int64_t mss, const float *__restrict__ sc, int64_t sss,
+                                         const R6RowMeta *__restrict__ meta, int64_t mrs, int64_t row, int si, int k) {
+    const R6RowMeta M = meta[row * mrs];
+    const double m = (double)mu[(int64_t)si * mss + row], s = (double)sc[(int64_t)si * sss + row];
+    const double rs = __ddiv_rn(1.0, s);
+    const double t0 = r6_mul(r6_add(M.a, -m), rs), dt = r6_mul(M.d, rs);
+    return r6_exp_neg(__fma_rn((double)(k - 1), dt, t0));
+}
 
 // ---- per-row metadata: least-effort affine fit through the first and last endpoint + its worst deviation ------------------
 __global__ void k_row_meta(const double *__restrict__ endp, int64_t ers, int64_t L, int S, R6RowMeta *__restrict__ meta,
@@ -84,7 +94,9 @@ __global__ void k_row_meta(const double *__restrict__ endp, int64_t ers, int64_t
 // vstat (VERIFY builds only): [0] bins whose emitted integer differs from the exact function's, [1] worst
 // |screened - exact| scaled pmf of a bin that was trusted, in thousandths of that row's window (1000 = the error that
 // could flip a truncation), [2] bins checked, [3] bins that took the exact path.
-template <bool POP, bool VERIFY, int LPR>
+// WIDE: S = 2048 or 4096 (chunks of up to 128 bins): the chain is re-anchored every R6_ANCHOR_BINS bins and the fix word
+// takes the wide layout (r6_fix_wide).  WIDE = false is the S <= 1024 kernel, unchanged.
+template <bool POP, bool VERIFY, int LPR, bool WIDE>
 __global__ void __launch_bounds__(512, 2) k_rows6(int count, int64_t L, int S, const float *__restrict__ mu, int64_t mss,
         const float *__restrict__ sc, int64_t sss, const double *__restrict__ endp, int64_t ers,
         const R6RowMeta *__restrict__ meta, int64_t mrs, const int16_t *__restrict__ sym, int bits, int q,
@@ -141,6 +153,7 @@ __global__ void __launch_bounds__(512, 2) k_rows6(int count, int64_t L, int S, c
         // one 4-bin group; `last`: the group that ends the row, whose upper edge is cdf = 1 exactly (:184) -- peeled out of the
         // loop below so that the loop does not carry the test and the two selects
         auto group = [&](const int k0, const bool last) __attribute__((always_inline)) {
+            if (WIDE && k0 != ks0 && ((k0 - ks0) & (R6_ANCHOR_BINS - 1)) == 0) ub = r6_anchor(mu, mss, sc, sss, meta, mrs, row, si, k0);
             if (POP && k0 == next_chunk) {                // chunk boundary: remember the P-sum so far
                 const uint32_t sofar = rsum + (uint32_t)(k0 - ks0);
 #pragma unroll
@@ -266,8 +279,10 @@ __global__ void __launch_bounds__(512, 2) k_rows6(int count, int64_t L, int S, c
 #pragma unroll
                 for (int t = 0; t < CPL; ++t) bo[t] = bs[t];
             }
-            if (j == 0)
-                fix[out] = make_uint2((uint32_t)bi | ((uint32_t)(pl.kl >> 2) << 10) | ((uint32_t)(pl.kh >> 2) << 18) | ((uint32_t)(pl.m >> 2) << 27), rem);
+            if (j == 0) {
+                if (WIDE) fix[out] = make_uint2(r6_fix_wide(bi, pl.kl, pl.kh), rem);
+                else fix[out] = make_uint2((uint32_t)bi | ((uint32_t)(pl.kl >> 2) << 10) | ((uint32_t)(pl.kh >> 2) << 18) | ((uint32_t)(pl.m >> 2) << 27), rem);
+            }
         }
     } else {
         // the row's C_s and P_s: sums over the row's lanes (one lane holds pv; every lane holds its share of the prefix)
@@ -325,8 +340,9 @@ __device__ __forceinline__ double shfl_d(double v, int src) {
 }
 
 // MASK: pixel level with block extents -- rows outside the extent keep the block loads and the prefetch going but skip the
-// search and the decode (bsw_x_live, warp-uniform); their symbols are written later by the codec's pad kernel
-template <bool MASK>
+// search and the decode (bsw_x_live, warp-uniform); their symbols are written later by the codec's pad kernel.
+// WIDE: S = 2048 or 4096 -- the wide fix layout and chunks of up to 128 bins (see the branch below).
+template <bool MASK, bool WIDE>
 __global__ void __launch_bounds__(PW6 * 32) k_pop6(bsw_streams sv, int first, int count, const float *__restrict__ mu, int64_t mss,
         const float *__restrict__ sc, int64_t sss, const double *__restrict__ endp, int64_t ers,
         const R6RowMeta *__restrict__ meta, int64_t mrs, const uint32_t *__restrict__ bases, const uint2 *__restrict__ fix,
@@ -384,7 +400,9 @@ __global__ void __launch_bounds__(PW6 * 32) k_pop6(bsw_streams sv, int first, in
         const double t0 = shfl_d(t0_w, j32), dt = shfl_d(dt_w, j32), magic = shfl_d(magic_w, j32);
         const uint32_t dmask = __shfl_sync(FULL, dmask_w, j32);
         const uint32_t fx = __shfl_sync(FULL, fx_w.x, j32), rem = __shfl_sync(FULL, fx_w.y, j32);
-        const int bi = (int)(fx & 1023u), kl = (int)((fx >> 10) & 255u) << 2, kh = (int)((fx >> 18) & 511u) << 2, m = (int)((fx >> 27) & 15u) << 2;
+        int bi, kl, kh, m;
+        if (WIDE) r6_unfix_wide(fx, bi, kl, kh, m);
+        else { bi = (int)(fx & 1023u); kl = (int)((fx >> 10) & 255u) << 2; kh = (int)((fx >> 18) & 511u) << 2; m = (int)((fx >> 27) & 15u) << 2; }
         const uint32_t base = base_n1;
         base_n1 = base_n2;
         if (i > 1) base_n2 = __ldg(bb + (i - 2) * 32 + lane);
@@ -395,7 +413,43 @@ __global__ void __launch_bounds__(PW6 * 32) k_pop6(bsw_streams sv, int first, in
             int s;
             if (mm < (uint32_t)kl) { s = (int)mm; ps = 1u; cs = mm; }                    // dead bins on the left: C[k] = k
             else if (mm >= Ckh) { s = kh + (int)(mm - Ckh); ps = 1u; cs = mm; }          // dead bins on the right
-            else {
+            else if (WIDE) {
+                // a chunk of up to 128 bins, walked in sub-chunks of 32 with the cdf carried between them: the symbol lies in
+                // the first sub-chunk whose successor starts above mm (or in the chunk's last one)
+                const int chunk = 31 - __clz(__ballot_sync(FULL, base <= mm));
+                const int kc = kl + chunk * m, kce = min(kc + m, kh);
+                uint32_t carry = __shfl_sync(FULL, base, chunk);
+                for (int k32 = kc;; k32 += 32) {
+                    const int k = k32 + lane;
+                    const bool active = k < kce;
+                    const double th = __fma_rn((double)k, dt, t0);
+                    const double c_hi = (k >= S - 1) ? 1.0 : r6_rcp3(__dadd_rn(1.0, r6_exp_neg(th)));
+                    const double c_lo = (k <= 0) ? 0.0 : r6_rcp3(__dadd_rn(1.0, r6_exp_neg(__dsub_rn(th, dt))));
+                    const double z = __fma_rn(__dsub_rn(c_hi, c_lo), mult2, magic);
+                    uint32_t raw = r6_raw(z);
+                    const bool doubt = active && (r6_doubt(z, dmask) || raw < 0x80000000u);
+                    if (__any_sync(FULL, doubt)) {
+                        const double m_ = (double)__shfl_sync(FULL, mu_w, j32), s_ = (double)__shfl_sync(FULL, sc_w, j32);
+                        const double rs = shfl_d(rs_w, j32);
+                        if (doubt) raw = r6_exact_pm(endp + i * ers, k, S, m_, s_, rs, mult) + 0x80000000u;
+                    }
+                    const uint32_t v = active ? (raw + 0x80000001u) + (k == bi ? rem : 0u) : 0u;
+                    uint32_t incl = v;
+                    for (int o = 1; o < 32; o <<= 1) {
+                        const uint32_t t = __shfl_up_sync(FULL, incl, o);
+                        if (lane >= o) incl += t;
+                    }
+                    const uint32_t cex = carry + incl - v;
+                    const uint32_t next = carry + __shfl_sync(FULL, incl, 31);
+                    if (k32 + 32 >= kce || next > mm) {
+                        const int js = 31 - __clz(__ballot_sync(FULL, active && cex <= mm));
+                        ps = __shfl_sync(FULL, v, js); cs = __shfl_sync(FULL, cex, js);
+                        s = k32 + js;
+                        break;
+                    }
+                    carry = next;
+                }
+            } else {
                 const int chunk = 31 - __clz(__ballot_sync(FULL, base <= mm));          // empty chunks hold Ckh > mm
                 const int k = kl + chunk * m + lane;
                 const bool active = lane < m && k < kh;
@@ -463,10 +517,11 @@ size_t bsw_rows6_scratch_bytes(int count, int64_t L) {
     return (size_t)count * L * (32 * 4 + 8);              // pop: 32 chunk bases + fix; push needs 16 B per row
 }
 
-int bsw_rows6_launch(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
-                     int64_t sss, const double *endp, int64_t ers, const void *meta, int16_t *sym, int64_t L, int S, int bits,
-                     int q, void *scratch, size_t scratch_bytes, const int16_t *ext, cudaStream_t st) {
-    BSW_REQUIRE(S >= 8 && S <= 1024 && (S & 3) == 0, "affine coder: support must be a multiple of 4 in [8, 1024]");
+namespace {
+template <bool WIDE>
+int rows6_launch(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
+                 int64_t sss, const double *endp, int64_t ers, const void *meta, int16_t *sym, int64_t L, int S, int bits,
+                 int q, void *scratch, size_t scratch_bytes, const int16_t *ext, cudaStream_t st) {
     BSW_REQUIRE(bits >= 8 && bits <= 31 && q >= 0 && q < bits, "affine coder: bits/quantbits out of range");
     BSW_REQUIRE(scratch_bytes >= (pop ? bsw_rows6_scratch_bytes(count, L) : (size_t)count * L * 16), "affine coder: scratch too small");
     const R6RowMeta *mt = (const R6RowMeta *)meta;
@@ -480,8 +535,8 @@ int bsw_rows6_launch(int phase, bool pop, bsw_streams *s, int first, int count, 
         const int env_lpr = g_lpr > 0 ? g_lpr : env_lpr0;
         if (g_verify && !g_vstat) { BSW_CUDA(cudaMalloc(&g_vstat, 32)); BSW_CUDA(cudaMemset(g_vstat, 0, 32)); }
 #define R6_LAUNCH(POP_, VER_, LPR_)                                                                                             \
-    BSW_MAX_SHARED_ONCE((k_rows6<POP_, VER_, LPR_>));                                                                             \
-    k_rows6<POP_, VER_, LPR_><<<dim3((unsigned)((L + 32 / LPR_ - 1) / (32 / LPR_)), (count + 15) / 16), 512, 0, st>>>(            \
+    BSW_MAX_SHARED_ONCE((k_rows6<POP_, VER_, LPR_, WIDE>));                                                                       \
+    k_rows6<POP_, VER_, LPR_, WIDE><<<dim3((unsigned)((L + 32 / LPR_ - 1) / (32 / LPR_)), (count + 15) / 16), 512, 0, st>>>(            \
         count, L, S, mu, mss, sc, sss, endp, ers, mt, mrs, POP_ ? nullptr : sym, bits, q, POP_ ? nullptr : pairs,                 \
         POP_ ? bases : nullptr, POP_ ? fix : nullptr, VER_ ? g_vstat : nullptr, 0,                                                \
         (double)(((int64_t)1 << bits) - ((int64_t)1 << q)) * 1048576.0,                                                           \
@@ -497,12 +552,23 @@ int bsw_rows6_launch(int phase, bool pop, bsw_streams *s, int first, int count, 
 #undef R6_LAUNCH
     } else {
         BSW_REQUIRE(pop, "affine coder: phase B of a push is k_push_pairs");
-        BSW_MAX_SHARED_ONCE(k_pop6<false>); BSW_MAX_SHARED_ONCE(k_pop6<true>);
-        if (ext) k_pop6<true><<<(count + PW6 - 1) / PW6, PW6 * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, mt, mrs, bases, fix, sym, L, S, bits, q, ext);
-        else k_pop6<false><<<(count + PW6 - 1) / PW6, PW6 * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, mt, mrs, bases, fix, sym, L, S, bits, q, nullptr);
+        BSW_MAX_SHARED_ONCE((k_pop6<false, WIDE>)); BSW_MAX_SHARED_ONCE((k_pop6<true, WIDE>));
+        if (ext) k_pop6<true, WIDE><<<(count + PW6 - 1) / PW6, PW6 * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, mt, mrs, bases, fix, sym, L, S, bits, q, ext);
+        else k_pop6<false, WIDE><<<(count + PW6 - 1) / PW6, PW6 * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, mt, mrs, bases, fix, sym, L, S, bits, q, nullptr);
     }
     BSW_LAUNCH_CHECK();
     return BSW_OK;
+}
+}  // namespace
+
+int bsw_rows6_launch(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
+                     int64_t sss, const double *endp, int64_t ers, const void *meta, int16_t *sym, int64_t L, int S, int bits,
+                     int q, void *scratch, size_t scratch_bytes, const int16_t *ext, cudaStream_t st) {
+    BSW_REQUIRE(S >= 8 && (S <= 1024 || S == 2048 || S == 4096) && (S & 3) == 0,
+                "affine coder: support must be a multiple of 4 in [8, 1024], 2048 or 4096");
+    if (S > 1024)
+        return rows6_launch<true>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, meta, sym, L, S, bits, q, scratch, scratch_bytes, ext, st);
+    return rows6_launch<false>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, meta, sym, L, S, bits, q, scratch, scratch_bytes, ext, st);
 }
 
 // Debug switch: 1 = every k_rows6 launch also evaluates the exact function for every bin and counts disagreements

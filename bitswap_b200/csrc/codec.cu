@@ -125,7 +125,8 @@ extern "C" int bsw_codec_create(bsw_codec **out, bsw_model *m, bsw_bins *b, int 
     BSW_CUDA(cudaMemcpy(dms, ms, sizeof(ms), cudaMemcpyHostToDevice));
     const double *zend = b->zend + (size_t)(c->nz - 1) * c->zdim * c->S;
     int rc = bsw_logistic_tables(zend, c->S, dms, dms + 1, 0, c->zdim, c->S, 31, c->q, c->priorP, c->priorC, nullptr);
-    if (!rc && c->S >= 128) {
+    // S > 1024: the prior pop searches priorC directly (bsw_ans_pop_i16, any support) instead of k_pop_full
+    if (!rc && c->S >= 128 && c->S <= 1024) {
         BSW_CUDA(cudaMalloc(&c->priorCoarse, sizeof(uint32_t) * (size_t)c->zdim * (c->S / 32)));
         BSW_CUDA(cudaMalloc(&c->priorFix, sizeof(uint2) * (size_t)c->zdim));
         rc = bsw_prior_coarse(c->priorC, c->zdim, c->S, c->priorCoarse, c->priorFix, nullptr);
@@ -171,6 +172,12 @@ extern "C" int bsw_codec_set_dual_stream(bsw_codec *c, int on) {
 
 extern "C" int bsw_codec_set_two_phase(bsw_codec *c, int on) {
     BSW_REQUIRE(c, "null codec");
+    // the fused kernels keep a whole row table in one warp's registers (S/32 bins per lane): 1024 bins at most
+    if (!on && c->S > 1024) {
+        bsw_set_error("bsw_codec_set_two_phase: the fused coder holds at most 1024 bins per row in registers; these bins "
+                      "have %d (quantbits %d), so only the two-phase coder can code them", c->S, c->q);
+        return BSW_E_INVALID;
+    }
     c->two_phase = on ? 1 : 0;
     return BSW_OK;
 }

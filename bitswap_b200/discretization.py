@@ -53,6 +53,8 @@ def discretize(nz, quantbits, type, device, model, dataset, images=None, ppb=30,
     them into per-dimension running extrema; the equal-width fit (bsw_discretize_edges) then needs no pass over the
     2 * ppb * 2^q * zdim samples of a level."""
     from ._lib import lib, check, cuda_stream_ptr
+    from .codec import check_quantbits
+    check_quantbits(quantbits)                          # 1..12, before any device work
     assert images is not None, "offline: pass the training images explicitly (the reference downloads them)"
     cfg = model.cfg
     assert cfg.nz == nz

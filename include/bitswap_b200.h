@@ -170,7 +170,8 @@ int bsw_logistic_tables(const double *endpoints_dev, int64_t endp_row_stride, co
  *     model/cifar_train.py:375-376 does); element [b*mu_stream_stride + r].  A stream stride of 0
  *     shares the vector between streams (the unconditional x-scale, cifar_train.py:411).
  *     endpoints as above but each row holds S doubles, the last one +inf (library layout, see
- *     bsw_bins_*).  S must be a multiple of 32 and <= 1024.
+ *     bsw_bins_*).  S must be a multiple of 32 and <= 1024: the fused kernels keep a row's table in one warp's
+ *     registers.  Wider supports (S = 2048, 4096: quantbits 11, 12) go through the two-phase entry points below.
  *     sym: int16 [count, L].
  * ---------------------------------------------------------------------------------------------- */
 int bsw_logistic_push(bsw_streams *s, int first, int count, const float *mu_dev, int64_t mu_stream_stride,
@@ -188,7 +189,9 @@ int bsw_logistic_pop(bsw_streams *s, int first, int count, const float *mu_dev, 
  * Two kernel families: the generic one (any sorted endpoint rows) and the affine-row one for rows that are uniform
  * grids -- which is every row discretize_kbins() builds (discretization.py:105-118) and the ImageBins pixel row
  * (utils/torch/rand.py:146-147).  These two entry points probe the rows on every call (one small kernel + a stream
- * synchronise); the codec uses the classification bsw_bins_create made. */
+ * synchronise); the codec uses the classification bsw_bins_create made.
+ * S: a power of two from 32 to 4096 (quantbits up to 12) for the generic family; a multiple of 4 in [8, 1024], 2048 or
+ * 4096 for the affine one.  The scratch size does not depend on S (136 bytes per row and stream for a pop). */
 int64_t bsw_logistic_scratch_bytes(int count, int64_t L, int S, int full_tables);
 /* Kernel family for bsw_logistic_*_2p and the codec: -1 = by row classification (default; BSW_ROWS_MODE overrides),
  * 0 = generic kernels only, 1 = affine-row kernels for every row (non-uniform rows take the exact path per bin). */
@@ -224,7 +227,8 @@ int bsw_logistic_pop_2p(bsw_streams *s, int first, int count, const float *mu_de
  * (utils/torch/rand.py:134-153); the library keeps its own padded copy (each endpoint row padded
  * with +1e300 to S entries so that cdf_{S-1} == 1 falls out of the same formula).
  * ---------------------------------------------------------------------------------------------- */
-/* zendpoints_host [nz, zdim, S-1], zcentres_host [nz, zdim, S] float64 (reference layout). */
+/* zendpoints_host [nz, zdim, S-1], zcentres_host [nz, zdim, S] float64 (reference layout); quantbits in [1, 12]
+ * (S = 2^quantbits).  Device memory: 16 * nz * zdim * S bytes (padded endpoints + centres), 1.07 GB for cifar8 at 12. */
 int bsw_bins_create(bsw_bins **out, int nz, int zdim, int quantbits, int xdim,
                     const double *zendpoints_host, const double *zcentres_host);
 int bsw_bins_destroy(bsw_bins *b);
@@ -330,7 +334,9 @@ int64_t bsw_codec_last_launches(const bsw_codec *c);
  * `stream` at the end (an experiment in co-scheduling tensor-bound and FP64-bound CTAs). */
 int bsw_codec_set_dual_stream(bsw_codec *c, int on);
 /* Coder variant: 1 (default) = two-phase (ans_rows.cu: fully parallel float64 row tables, then the serial integer
- * coder), 0 = fused one-warp-per-stream kernels (bsw_logistic_push/pop).  Bit-identical results. */
+ * coder), 0 = fused one-warp-per-stream kernels (bsw_logistic_push/pop).  Bit-identical results.  0 is refused
+ * (BSW_E_INVALID) when the codec's bins have more than 1024 bins per row (quantbits 11 and 12): the fused kernels
+ * cannot hold such a table in registers. */
 int bsw_codec_set_two_phase(bsw_codec *c, int on);
 /* Per-kernel-category device time (CUDA events on the launching stream) accumulated since profiling was
  * enabled.  ms_out/n_out: 12 entries {misc, conv_in, conv_dense3x3, conv_dense5x5, conv_head, pop_z, push_z,
