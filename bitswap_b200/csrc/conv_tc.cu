@@ -6,7 +6,8 @@
 //
 // GEMM view (per image):  D[p, o] = sum_{tap, c} A_tap[p, c] * W[tap][o, c]
 //     one tile = 128 pixels (8 image rows of a 16x16 image) x N output channels (N = 128 for the W->W convs and the
-//     in-convs, 32 for the heads), K = taps x input channels, walked as (tap, 32-channel chunk) k-blocks.
+//     in-convs, 64 for those of a model of padded width 64, 32 for the heads), K = taps x input channels, walked as
+//     (tap, 32-channel chunk) k-blocks.
 //   * A_tap is never materialised (no im2col): the activation tensor is NHWC bf16 and one 4-D TMA box
 //     {32 ch, 16 w, 8 h, 1 img} at coordinates (c0, dx-r, dy-r+8*half, img) IS the shifted tile; TMA's
 //     out-of-bounds zero fill supplies the "same" padding.
@@ -29,6 +30,8 @@
 //     to itself and the peer that shares them, so every CTA pulls 16 of its 32 KB per k-block from L2 (the launches are
 //     bound by L2 -> SM bytes, not by their MMAs).  A stage is refilled only after all three CTAs writing into it
 //     released it.
+//     A model of padded width 64 (reswidth 1..64, the MNIST models) has one 64-channel block per pixel half: its dense
+//     convs and in-convs run the narrow tile (NarrowArgs) as single CTAs, one per tile.
 //   * fixed k order, no split-K, no atomics: results are bit-identical for any batch size, position in the batch
 //     or grid (the decoder must regenerate the encoder's tables exactly, SURVEY.md H3).
 #include <cuda.h>
@@ -45,6 +48,7 @@ namespace {
 constexpr int BK = 32;                      // channels per k-block (64-byte rows, SWIZZLE_64B)
 constexpr int MT = 128;                     // pixels per tile: two warpgroups x 64
 constexpr int BN = 128;                     // output channels per tile of the W->W convs and in-convs
+constexpr int NW = 64;                      // output channels per tile of a padded-width-64 model's W->W convs and in-convs
 constexpr int HD_N = 32;                    // output channels of the heads (n_mu + n_sc <= 32, zero padded)
 constexpr int A_BYTES = MT * BK * 2;        // one 128-row x 32-col bf16 activation tile = 8 KB
 constexpr int WG_THREADS = 384;             // two consumer warpgroups + the producer / epilogue warpgroup
@@ -59,12 +63,16 @@ constexpr int HD_LD = MT + 4;               // heads' hand-off row stride (float
 template <int N> struct TileCfg {
     static constexpr int W_BYTES = N * BK * 2;                       // one N-row weight tile
     static constexpr int STAGE = 2 * A_BYTES + 2 * W_BYTES;          // A_hi, A_lo, B_hi, B_lo
-    static constexpr int NSTAGE = N == BN ? 4 : 5;                   // 128 KB (N = 128) / 100 KB (N = 32) of stages
-    // fp32 hand-off tile (main + cross) from the consumers to the epilogue warps: 64 KB (N = 128) / 16.5 KB (N = 32)
-    static constexpr int HAND = N == BN ? MT * N * 4 : N * HD_LD * 4;
+    // 128 KB (N = 128) / 144 KB (N = 64: six 24 KB stages, 2.7 of a dense 3x3's 18 k-blocks in flight) / 100 KB
+    // (N = 32) of stages
+    static constexpr int NSTAGE = N == BN ? 4 : N == NW ? 6 : 5;
+    // fp32 hand-off tile (main + cross) from the consumers to the epilogue warps: 64 KB (N = 128) / 32 KB (N = 64) /
+    // 16.5 KB (N = 32)
+    static constexpr int HAND = N == HD_N ? N * HD_LD * 4 : MT * N * 4;
     static constexpr int SMEM = NSTAGE * STAGE + HAND + 1024 /*align*/ + 256 /*barriers*/;
 };
 static_assert(TileCfg<BN>::SMEM <= 227 * 1024, "stages and hand-off must fit one H100 SM's shared memory");
+static_assert(TileCfg<NW>::SMEM <= TileCfg<BN>::SMEM, "the narrow tile takes no more shared memory than the wide one");
 
 struct TcState {
     // bf16 hi/lo activation planes, ping-pong: [max_batch, 256 px, 256 ch]
@@ -187,6 +195,20 @@ template <> struct Wgmma<128> {
             : "l"(da), "l"(db), "r"(1));
     }
 };
+template <> struct Wgmma<64> {
+    static __device__ __forceinline__ void mma(float (&d)[32], uint64_t da, uint64_t db) {
+        asm volatile(
+            "{\n"
+            ".reg .pred p;\n"
+            "setp.ne.b32 p, %34, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+            "%32, %33, p, 1, 1, 0, 0;\n"
+            "}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "l"(da), "l"(db), "r"(1));
+    }
+};
 template <> struct Wgmma<32> {
     static __device__ __forceinline__ void mma(float (&d)[16], uint64_t da, uint64_t db) {
         asm volatile(
@@ -232,35 +254,63 @@ struct TcArgs {
     int A_elu;
 };
 
-// Hand-off tile of the dense convs and in-convs: s = main + cross as fp32 [128 px][128 ch], the 32-byte column chunks
-// of row r XOR-swizzled by r & 3.  The consumers' float2 writes (a half warp covers 4 rows x 4 pairs of one chunk) and
-// the epilogue's float4 row reads (8 lanes read 4 whole chunks of one row) then both hit 32 distinct banks.
-__device__ __forceinline__ int hand_idx(int r, int c) { return r * BN + (((c >> 3) ^ (r & 3)) << 3) + (c & 7); }
+// Dense W->W convs and in-convs of a model of padded width 64: one 64-channel block per pixel half (kCoBlocks = 1, so
+// single CTAs; tile t -> image t / 2, pixel half t & 1).  Trunk, residual, planes and bias are 64 channels wide.
+struct NarrowArgs {
+    static constexpr int kN = NW, kCoBlocks = 1;
+    int taps, ks;
+    int cchunks;             // 32-channel chunks per tap: 2 for the dense W->W convs, 1 for the in-convs
+    const float *bias;       // [64]
+    const float *resid;      // [n,256,64] fp32 or null
+    float *T;                // trunk out or null
+    int T_elu;
+    __nv_bfloat16 *A_hi, *A_lo;   // next conv's input planes [n,256,64] or null
+    int A_elu;
+};
 
-__device__ __forceinline__ void hand_store(const TcArgs &, float *hand, const float (&dm)[64], const float (&dc)[64], int row,
-                                           int lane) {
+// Hand-off tile of the dense convs and in-convs: s = main + cross as fp32 [128 px][N ch] (N = 128, or 64 for NarrowArgs),
+// the 32-byte column chunks of row r XOR-swizzled by r & 3.  A row is a whole number of 128-byte bank lines, so without
+// the swizzle chunk j of rows r..r+3 would sit on the same 8 banks.  The consumers' float2 writes (a half warp covers
+// chunk j of 4 consecutive rows) go to chunks j ^ 0..3, and the epilogue's float4 reads (a quarter warp covers 4
+// consecutive chunks of one row) to 4 chunks; either way the low two chunk bits differ -> 32 distinct banks.
+template <int N> __device__ __forceinline__ int hand_idx(int r, int c) { return r * N + (((c >> 3) ^ (r & 3)) << 3) + (c & 7); }
+
+template <int N>
+__device__ __forceinline__ void dense_hand_store(float *hand, const float (&dm)[N / 2], const float (&dc)[N / 2], int row, int lane) {
 #pragma unroll
-    for (int j = 0; j < 16; ++j)
+    for (int j = 0; j < N / 8; ++j)
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int i = 4 * j + 2 * h;
-            *reinterpret_cast<float2 *>(hand + hand_idx(row + 8 * h, 8 * j + 2 * (lane & 3))) =
+            *reinterpret_cast<float2 *>(hand + hand_idx<N>(row + 8 * h, 8 * j + 2 * (lane & 3))) =
                 make_float2(dm[i] + dc[i], dm[i + 1] + dc[i + 1]);
         }
 }
+__device__ __forceinline__ void hand_store(const TcArgs &, float *hand, const float (&dm)[64], const float (&dc)[64], int row,
+                                           int lane) {
+    dense_hand_store<BN>(hand, dm, dc, row, lane);
+}
+__device__ __forceinline__ void hand_store(const NarrowArgs &, float *hand, const float (&dm)[32], const float (&dc)[32], int row,
+                                           int lane) {
+    dense_hand_store<NW>(hand, dm, dc, row, lane);
+}
 
 // Dense / in-conv epilogue, run by the epilogue warps from the hand-off tile: s + bias (+ residual) (-> ELU) -> trunk;
-// (-> ELU) -> bf16 hi/lo planes of the next conv.  Warp ew takes tile rows ew, ew + 3, ...; lane l channels co0 + 4l..+3,
-// so a warp stores 512 contiguous bytes of the trunk and 256 of each plane per row.  The residual is the trunk itself
+// (-> ELU) -> bf16 hi/lo planes of the next conv.  Tensors are NHWC with LD channels per pixel and the hand-off tile has
+// N channels per row; ROWS tile rows are stored per warp step, 32 / ROWS lanes per row, 4 channels per lane (TcArgs:
+// one 128-channel half row per step; NarrowArgs: two 64-channel rows).  Warp ew takes row steps ew, ew + 3, ..., so a
+// warp stores 512 contiguous bytes of the trunk and 256 of each plane per step.  The residual is the trunk itself
 // (updated in place: resid == T): each element is read and then written by the same thread, and the loads of the next
-// RD rows are issued before the current row's stores.
-__device__ __forceinline__ void epilogue(const TcArgs &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
-    constexpr int RD = 3;
-    const float4 bq = __ldg(reinterpret_cast<const float4 *>(a.bias + co0) + lane);
-    const int64_t base = ((int64_t)img * 256 + mh * 128) * 256 + co0 + 4 * lane;     // + r * 256
-    const int nr = (MT - ew + EPI_WARPS - 1) / EPI_WARPS;
+// RD steps are issued before the current step's stores.
+template <int LD, int N, int ROWS, class Args>
+__device__ __forceinline__ void dense_epilogue(const Args &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
+    constexpr int RD = 3, LPR = 32 / ROWS;
+    const int hl = lane % LPR, sub = lane / LPR;
+    const float4 bq = __ldg(reinterpret_cast<const float4 *>(a.bias + co0) + hl);
+    const int64_t base = ((int64_t)img * 256 + mh * 128 + sub) * LD + co0 + 4 * hl;     // + ROWS * step * LD
+    const int nr = (MT / ROWS - ew + EPI_WARPS - 1) / EPI_WARPS;
     auto resid = [&](int k) {
-        return (a.resid && k < nr) ? *reinterpret_cast<const float4 *>(a.resid + base + (ew + EPI_WARPS * k) * 256)
+        return (a.resid && k < nr) ? *reinterpret_cast<const float4 *>(a.resid + base + ROWS * (ew + EPI_WARPS * k) * LD)
                                    : make_float4(0.f, 0.f, 0.f, 0.f);
     };
     float4 q[RD];
@@ -269,17 +319,17 @@ __device__ __forceinline__ void epilogue(const TcArgs &a, const float *hand, int
     for (int k0 = 0; k0 < nr; k0 += RD) {
 #pragma unroll
         for (int d = 0; d < RD; ++d) {
-            const int k = k0 + d, r = ew + EPI_WARPS * k;
+            const int k = k0 + d, rs = ew + EPI_WARPS * k, r = ROWS * rs + sub;
             if (k >= nr) break;
             const float4 rq = q[d];
             q[d] = resid(k + RD);
-            const float4 s = *reinterpret_cast<const float4 *>(hand + hand_idx(r, 4 * lane));
+            const float4 s = *reinterpret_cast<const float4 *>(hand + hand_idx<N>(r, 4 * hl));
             float x[4] = {s.x + bq.x, s.y + bq.y, s.z + bq.z, s.w + bq.w};
             if (a.resid) { x[0] += rq.x; x[1] += rq.y; x[2] += rq.z; x[3] += rq.w; }
             if (a.T_elu)
 #pragma unroll
                 for (int e = 0; e < 4; ++e) x[e] = elu1(x[e]);
-            const int64_t off = base + r * 256;
+            const int64_t off = base + ROWS * rs * LD;
             if (a.T) *reinterpret_cast<float4 *>(a.T + off) = make_float4(x[0], x[1], x[2], x[3]);
             if (a.A_hi) {
                 __nv_bfloat16 hi[4], lo[4];
@@ -294,6 +344,13 @@ __device__ __forceinline__ void epilogue(const TcArgs &a, const float *hand, int
             }
         }
     }
+}
+__device__ __forceinline__ void epilogue(const TcArgs &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
+    dense_epilogue<256, BN, 1>(a, hand, img, mh, co0, ew, lane);
+}
+
+__device__ __forceinline__ void epilogue(const NarrowArgs &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
+    dense_epilogue<NW, NW, 2>(a, hand, img, mh, co0, ew, lane);
 }
 
 // mu/sigma heads: the 3x3 W -> (n_mu + n_sc <= 32) convolution that ends every net (cifar_train.py:349,368,411,426),
@@ -551,16 +608,18 @@ int encode_map(CUtensorMap *m, void *base, int rank, const cuuint64_t *dims, con
 struct TcSlot { CUtensorMap map_hi, map_lo; };
 
 int bsw_model_tc_prepare(bsw_model *m) {
-    BSW_REQUIRE(m->Wp == 256, "tensor-core conv path needs a padded width of 256 (reswidth 193..256)");
+    BSW_REQUIRE(m->Wp == 256 || m->Wp == NW,
+                "tensor-core conv path needs a padded width of 64 or 256 (reswidth 1..64 or 193..256)");
+    const int Wp = m->Wp;
     TcState *ts = new TcState();
     m->tc_state = ts;
-    const size_t act_elems = (size_t)m->d.max_batch * 256 * 256;
+    const size_t act_elems = (size_t)m->d.max_batch * 256 * Wp;
     for (int b = 0; b < 2; ++b)
         for (int pl = 0; pl < 2; ++pl) {
             BSW_CUDA(cudaMalloc(&ts->act[b][pl], act_elems * sizeof(__nv_bfloat16)));
             BSW_CUDA(cudaMemset(ts->act[b][pl], 0, act_elems * sizeof(__nv_bfloat16)));
-            cuuint64_t dims[4] = {256, 16, 16, (cuuint64_t)m->d.max_batch};
-            cuuint64_t str[3] = {256 * 2, 16 * 256 * 2, 256 * 256 * 2};
+            cuuint64_t dims[4] = {(cuuint64_t)Wp, 16, 16, (cuuint64_t)m->d.max_batch};
+            cuuint64_t str[3] = {(cuuint64_t)Wp * 2, (cuuint64_t)16 * Wp * 2, (cuuint64_t)256 * Wp * 2};
             cuuint32_t box[4] = {BK, 16, 8, 1};
             if (int rc = encode_map(&ts->act_map[b][pl], ts->act[b][pl], 4, dims, str, box)) return rc;
         }
@@ -572,21 +631,24 @@ int bsw_model_tc_prepare(bsw_model *m) {
         cuuint32_t box[4] = {BK, 16, 8, 1};
         if (int rc = encode_map(&ts->inp_map[pl], ts->inp[pl], 4, dims, str, box)) return rc;
     }
-    // weights: [tap][o=256][c=Kc] bf16 hi/lo planes, K (=c) innermost; Kc = 256 for the dense convs, 32 for the in-convs
+    // weights: [tap][o=rows][c=Kc] bf16 hi/lo planes, K (=c) innermost; Kc = Wp for the dense convs and heads, 32 for the
+    // in-convs; rows = Wp for the dense convs and in-convs, 32 for the heads
     std::vector<TcSlot> *slots = new std::vector<TcSlot>();
     std::vector<char> is_in(m->convs.size(), 0), is_head(m->convs.size(), 0);
     for (auto &np : m->infer) { is_in[np.in_conv] = 1; is_head[np.head] = 1; }
     for (auto &np : m->gen) { is_in[np.in_conv] = 1; is_head[np.head] = 1; }
     for (size_t ci_ = 0; ci_ < m->convs.size(); ++ci_) {
         ConvSlot &c = m->convs[ci_];
-        bool dense = (c.Cin == m->d.reswidth && c.Cout == m->d.reswidth);
+        // by role, not by shape alone: on a narrow model an in-conv (zchannels = reswidth) or a head (2 zchannels =
+        // reswidth) can have the dense convs' W -> W shape
+        bool dense = !is_in[ci_] && !is_head[ci_] && c.Cin == m->d.reswidth && c.Cout == m->d.reswidth;
         bool inconv = is_in[ci_] && c.Cin <= 32 && c.Cout == m->d.reswidth;
         bool head = is_head[ci_] && !dense && c.Cin == m->d.reswidth && c.Cout <= HD_N;
         if (!dense && !inconv && !head) continue;
         BSW_REQUIRE(!c.host_w.empty(), "tc_prepare: host weights already released");
         const int taps = c.ks * c.ks;
-        const int Kc = inconv ? 32 : 256;
-        const int rows = head ? HD_N : 256;              // output-channel rows per tap (heads: zero padded to 32)
+        const int Kc = inconv ? 32 : Wp;
+        const int rows = head ? HD_N : Wp;               // output-channel rows per tap (heads: zero padded to 32)
         std::vector<__nv_bfloat16> hi((size_t)taps * rows * Kc), lo(hi.size());
         for (int tp = 0; tp < taps; ++tp)
             for (int ci = 0; ci < Kc; ++ci)
@@ -606,7 +668,7 @@ int bsw_model_tc_prepare(bsw_model *m) {
         TcSlot s;
         cuuint64_t dims[3] = {(cuuint64_t)Kc, (cuuint64_t)rows, (cuuint64_t)taps};
         cuuint64_t str[2] = {(cuuint64_t)Kc * 2, (cuuint64_t)rows * Kc * 2};
-        cuuint32_t box[3] = {BK, (cuuint32_t)(head ? HD_N : BN), 1};
+        cuuint32_t box[3] = {BK, (cuuint32_t)(head ? HD_N : Wp == NW ? NW : BN), 1};
         if (int rc = encode_map(&s.map_hi, c.w_hi, 3, dims, str, box)) return rc;
         if (int rc = encode_map(&s.map_lo, c.w_lo, 3, dims, str, box)) return rc;
         c.tc_index = (int)slots->size();
@@ -615,8 +677,10 @@ int bsw_model_tc_prepare(bsw_model *m) {
     m->tc_slots = slots;
     BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<TcArgs>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<BN>::SMEM));
     BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<HeadArgs>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<HD_N>::SMEM));
+    BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<NarrowArgs>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<NW>::SMEM));
     // one SM-wide L1/shared split for every kernel of the path (see bsw_prefer_max_shared)
     bsw_prefer_max_shared(k_conv_wg<TcArgs>); bsw_prefer_max_shared(k_conv_wg<HeadArgs>);
+    bsw_prefer_max_shared(k_conv_wg<NarrowArgs>);
     bsw_prefer_max_shared(k_given_to_planes);
     m->tc_ready = true;
     return BSW_OK;
@@ -644,7 +708,7 @@ void bsw_tc_planes(bsw_model *m, int which, void **hi, void **lo) {
 
 int bsw_tc_split(bsw_model *m, const float *in, int which, int64_t n, cudaStream_t st) {
     TcState *ts = (TcState *)m->tc_state;
-    int64_t cnt = n * 256 * 256;
+    int64_t cnt = n * 256 * m->Wp;
     k_split_planes<<<(unsigned)((cnt + 255) / 256), 256, 0, st>>>(in, ts->act[which][0], ts->act[which][1], cnt);
     BSW_LAUNCH_CHECK();
     return BSW_OK;
@@ -653,7 +717,8 @@ int bsw_tc_split(bsw_model *m, const float *in, int which, int64_t n, cudaStream
 // Launch shape of the convolutions, a bit mask -- 1 / 2 = dense 3x3 / 5x5, 4 = in-convs and heads on a persistent grid
 // (one CTA or cluster per SM / cluster slot walking the tiles, the TMA ring prefetching across tile boundaries); a clear
 // bit means one CTA per tile.  8 = the dense convs and in-convs without TMA multicast: single CTAs, each loading its whole
-// stage.  Default 7 (BSW_TC_PERSIST overrides).  Same tiles, same k order per tile: results are bit-identical in every mode.
+// stage; it has no effect on a model of padded width 64, whose narrow tiles always run as single CTAs.  Default 7
+// (BSW_TC_PERSIST overrides).  Same tiles, same k order per tile: results are bit-identical in every mode.
 static int g_tc_mode = -1;
 static int tc_mode() {
     static const int env = getenv("BSW_TC_PERSIST") ? atoi(getenv("BSW_TC_PERSIST")) : 7;
@@ -716,19 +781,41 @@ static int launch_tc(const CUtensorMap &amap_hi, const CUtensorMap &amap_lo, con
     return BSW_OK;
 }
 
+// Dense convs and in-convs of a model of padded width 64: single CTAs, one per tile or a persistent grid of one per SM.
+static int launch_tc_narrow(const CUtensorMap &amap_hi, const CUtensorMap &amap_lo, const TcSlot &s, const NarrowArgs &t,
+                            int64_t n, bool persistent, cudaStream_t st) {
+    const int ntiles = (int)n * 2;
+    k_conv_wg<NarrowArgs><<<tc_grid(ntiles, persistent), WG_THREADS, TileCfg<NW>::SMEM, st>>>(amap_hi, amap_lo, s.map_hi,
+                                                                                             s.map_lo, t, ntiles);
+    BSW_LAUNCH_CHECK();
+    return BSW_OK;
+}
+
+// Fills the fields TcArgs and NarrowArgs share (everything but cchunks).
+template <class Args> static Args tc_args(TcState *ts, const ConvSlot &c, const ConvArgs &a, const float *resid) {
+    Args t;
+    t.taps = c.ks * c.ks; t.ks = c.ks;
+    t.bias = c.bias; t.resid = resid; t.T = a.T; t.T_elu = a.T_elu;
+    t.A_hi = a.A_planes >= 0 ? ts->act[a.A_planes][0] : nullptr;
+    t.A_lo = a.A_planes >= 0 ? ts->act[a.A_planes][1] : nullptr;
+    t.A_elu = a.A_elu;
+    return t;
+}
+
 // a.in must be one of the plane buffers: a.in_planes = 0/1 selects it; outputs a.A_planes = 0/1/-1.
 int bsw_conv_tc(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t n, cudaStream_t st) {
     TcState *ts = (TcState *)m->tc_state;
     BSW_REQUIRE(ts && c.tc_index >= 0, "bsw_conv_tc: conv has no tensor-core weights");
     const TcSlot &s = (*(std::vector<TcSlot> *)m->tc_slots)[c.tc_index];
-    TcArgs t;
-    t.taps = c.ks * c.ks; t.ks = c.ks;
+    const bool persistent = tc_persistent(c.ks <= 3 ? 1 : 2);
+    if (m->Wp == NW) {
+        NarrowArgs t = tc_args<NarrowArgs>(ts, c, a, a.resid);
+        t.cchunks = NW / BK;
+        return launch_tc_narrow(ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1], s, t, n, persistent, st);
+    }
+    TcArgs t = tc_args<TcArgs>(ts, c, a, a.resid);
     t.cchunks = 8;
-    t.bias = c.bias; t.resid = a.resid; t.T = a.T; t.T_elu = a.T_elu;
-    t.A_hi = a.A_planes >= 0 ? ts->act[a.A_planes][0] : nullptr;
-    t.A_lo = a.A_planes >= 0 ? ts->act[a.A_planes][1] : nullptr;
-    t.A_elu = a.A_elu;
-    return launch_tc(ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1], s, t, n, tc_persistent(c.ks <= 3 ? 1 : 2), st);
+    return launch_tc(ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1], s, t, n, persistent, st);
 }
 
 // Heads: reads the planes the last ResNet conv wrote (in_planes), writes mu / sigma.  BSW_TC_HEADS=0 keeps the float32 SIMT
@@ -742,7 +829,7 @@ int bsw_conv_tc_head(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t
     BSW_REQUIRE(ts && c.tc_index >= 0 && a.n_mu + a.n_sc <= HD_N, "bsw_conv_tc_head: conv has no tensor-core head weights");
     const TcSlot &s = (*(std::vector<TcSlot> *)m->tc_slots)[c.tc_index];
     HeadArgs h;
-    h.taps = c.ks * c.ks; h.ks = c.ks; h.cchunks = 8; h.bias = c.bias; h.mu = a.mu; h.scale = a.scale; h.n_mu = a.n_mu; h.n_sc = a.n_sc;
+    h.taps = c.ks * c.ks; h.ks = c.ks; h.cchunks = m->Wp / BK; h.bias = c.bias; h.mu = a.mu; h.scale = a.scale; h.n_mu = a.n_mu; h.n_sc = a.n_sc;
     h.scale_kind = a.scale_kind; h.out_mode = a.out_mode; h.out_dim = a.out_dim;
     const int ntiles = (int)n * 2;
     k_conv_wg<HeadArgs><<<tc_grid(ntiles, tc_persistent(4)), WG_THREADS, TileCfg<HD_N>::SMEM, st>>>(
@@ -760,14 +847,17 @@ int bsw_conv_tc_in(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t n
     int64_t cnt = n * 256 * 32;
     k_given_to_planes<<<(unsigned)((cnt + 255) / 256), 256, 0, st>>>(a.in, a.in_dim, c.Cin, a.in_mode, ts->inp[0], ts->inp[1], n);
     BSW_LAUNCH_CHECK();
-    TcArgs t;
-    t.taps = c.ks * c.ks; t.ks = c.ks;
-    t.cchunks = 1;
-    t.bias = c.bias; t.resid = nullptr; t.T = a.T; t.T_elu = a.T_elu;
-    t.A_hi = a.A_planes >= 0 ? ts->act[a.A_planes][0] : nullptr;
-    t.A_lo = a.A_planes >= 0 ? ts->act[a.A_planes][1] : nullptr;
-    t.A_elu = a.A_elu;
-    if (int rc = launch_tc(ts->inp_map[0], ts->inp_map[1], s, t, n, tc_persistent(4), st)) return rc;
+    int rc;
+    if (m->Wp == NW) {
+        NarrowArgs t = tc_args<NarrowArgs>(ts, c, a, nullptr);
+        t.cchunks = 1;
+        rc = launch_tc_narrow(ts->inp_map[0], ts->inp_map[1], s, t, n, tc_persistent(4), st);
+    } else {
+        TcArgs t = tc_args<TcArgs>(ts, c, a, nullptr);
+        t.cchunks = 1;
+        rc = launch_tc(ts->inp_map[0], ts->inp_map[1], s, t, n, tc_persistent(4), st);
+    }
+    if (rc) return rc;
     *launches += 2;
     return BSW_OK;
 }

@@ -532,8 +532,8 @@ static int run_net(bsw_model *m, const NetPlan &np, const float *given, int64_t 
 // Test hook: one conv of a loaded model through dispatch_conv, with the epilogue selected by `flags`.  The conv's role
 // and net come from the model's plans; a head is named by its mu prefix.  Tensor-core dense convs and heads read plane
 // buffer 0, split from in_dev here by the same RNE split the epilogues use; dense convs write plane buffer 1, in-convs
-// plane buffer 0.  The written buffer is filled with 0xffff first and copied whole ([2][max_batch,256,256]) to
-// planes_dev, so rows the conv must not touch can be checked.
+// plane buffer 0.  The written buffer is filled with 0xffff first and copied whole ([2][max_batch,256,Wp], Wp = 64 or
+// 256) to planes_dev, so rows the conv must not touch can be checked.
 extern "C" int bsw_selftest_conv(bsw_model *m, const char *prefix, const float *in_dev, int64_t n, int flags, float *T_dev,
                                  float *A_dev, uint16_t *planes_dev, float *mu_dev, float *scale_dev, void *stream) {
     BSW_REQUIRE(m && prefix && in_dev, "bsw_selftest_conv: null argument");
@@ -560,7 +560,7 @@ extern "C" int bsw_selftest_conv(bsw_model *m, const char *prefix, const float *
     BSW_REQUIRE(np, "bsw_selftest_conv: the conv is in no net");
     const ConvSlot &c = m->convs[slot];
     cudaStream_t st = (cudaStream_t)stream;
-    const size_t plane_bytes = (size_t)m->d.max_batch * 256 * 256 * sizeof(uint16_t);
+    const size_t plane_bytes = (size_t)m->d.max_batch * 256 * m->Wp * sizeof(uint16_t);
     ConvArgs a = {};
     a.Cin = c.Cin; a.CinP = c.CinP; a.w = c.w; a.bias = c.bias; a.CoutP = c.CoutP;
     a.in = in_dev; a.in_planes = 0; a.A_planes = -1;

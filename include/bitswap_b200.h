@@ -55,7 +55,7 @@ int         bsw_selftest_cdf_apx(int64_t n, uint64_t seed, double *worst_units_h
  *   flags:   epilogue of in-convs and dense convs, r = conv + bias: BSW_CONV_RESID r += T_dev (the residual, updated in
  *            place), BSW_CONV_T writes T_dev = (T_ELU ? ELU(r) : r), BSW_CONV_A writes the next conv's input
  *            (A_ELU ? ELU(T) : T) to A_dev (SIMT; NULL = an internal buffer) or to bf16 hi/lo planes (tensor cores).
- *   T_dev, A_dev: float32 [n,256,Wp].  planes_dev: uint16 [2][max_batch,256,256] (hi, lo) receives the whole plane
+ *   T_dev, A_dev: float32 [n,256,Wp].  planes_dev: uint16 [2][max_batch,256,Wp] (hi, lo) receives the whole plane
  *            buffer the conv wrote, pre-filled with 0xffff; tensor-core path with BSW_CONV_A only.
  *   mu_dev, scale_dev: head outputs [n, dim_out] flat CHW, as bsw_vae_* returns them (scale only with a scale head). */
 #define BSW_CONV_RESID 1
@@ -208,8 +208,8 @@ int bsw_rows6_set_lanes_per_row(int lpr);
 /* Launch shape of the tensor-core convolutions, a bit mask: 1 / 2 / 4 = dense 3x3 / dense 5x5 / in-convs and heads on a
  * persistent grid (one CTA per SM, or one four-CTA cluster per four SMs, walking half-image tiles); a clear bit = one
  * CTA per tile.  8 = dense convs and in-convs as single CTAs without TMA multicast (by default each image's four tiles
- * run as one cluster sharing their operand loads).  -1 = default (BSW_TC_PERSIST if set, else 7).  Bit-identical
- * results. */
+ * run as one cluster sharing their operand loads); no effect on a model of padded width 64, whose narrow tiles always
+ * run as single CTAs.  -1 = default (BSW_TC_PERSIST if set, else 7).  Bit-identical results. */
 int bsw_set_conv_mode(int mode);
 int bsw_rows6_verify_read(uint64_t *out4_host);
 int bsw_logistic_push_2p(bsw_streams *s, int first, int count, const float *mu_dev, int64_t mu_stream_stride,
@@ -277,7 +277,8 @@ typedef struct {
     int32_t reswidth;
     int32_t cond_xscale;   /* imagenetcrop: x-scale from a conv head */
     int32_t max_batch;     /* activations are preallocated for this many images */
-    int32_t use_tensor_cores; /* 1: wgmma tensor-core path for the W->W convs (needs padded width 256); 0: fp32 SIMT */
+    int32_t use_tensor_cores; /* 1: wgmma tensor-core path for the W->W convs (needs padded width 64 or 256, i.e.
+                                 reswidth 1..64 or 193..256); 0: fp32 SIMT */
 } bsw_model_desc;
 
 int bsw_model_create(bsw_model **out, const bsw_model_desc *desc);
