@@ -22,6 +22,12 @@ class CodecConfig:
     ansbits: int = 31                        # rANS probability precision (cifar_compress.py:75)
     cond_xscale: bool = False                # imagenetcrop: x-scale is a conv head, not a parameter
 
+    def __post_init__(self):
+        # the reference's --kernel: ResNet blocks, z in-convs and heads; "same" padding needs it odd, and the device
+        # convs are built for 1, 3, 5 and 7
+        if self.kernel_size not in (1, 3, 5, 7):
+            raise ValueError(f"kernel_size must be 1, 3, 5 or 7 (odd, at most 7), got {self.kernel_size!r}")
+
     @property
     def zdim(self) -> int:
         return self.zchannels * 16 * 16

@@ -6,7 +6,7 @@
 //
 // GEMM view (per image):  D[p, o] = sum_{tap, c} A_tap[p, c] * W[tap][o, c]
 //     one tile = 128 pixels (8 image rows of a 16x16 image) x N output channels (N = 128 for the W->W convs and the
-//     in-convs, 64 for those of a model of padded width 64, 32 for the heads), K = taps x input channels, walked as
+//     in-convs, 64 for those of a model of padded width 64 or 192, 32 for the heads), K = taps x input channels, walked as
 //     (tap, 32-channel chunk) k-blocks.
 //   * A_tap is never materialised (no im2col): the activation tensor is NHWC bf16 and one 4-D TMA box
 //     {32 ch, 16 w, 8 h, 1 img} at coordinates (c0, dx-r, dy-r+8*half, img) IS the shifted tile; TMA's
@@ -31,7 +31,11 @@
 //     bound by L2 -> SM bytes, not by their MMAs).  A stage is refilled only after all three CTAs writing into it
 //     released it.
 //     A model of padded width 64 (reswidth 1..64, the MNIST models) has one 64-channel block per pixel half: its dense
-//     convs and in-convs run the narrow tile (NarrowArgs) as single CTAs, one per tile.
+//     convs and in-convs run the narrow tile (NarrowArgs) as single CTAs, one per tile.  Padded width 128 runs the
+//     N = 128 tile with one channel block (Tc128Args), padded width 192 the N = 64 tile with three (Tc192Args), both
+//     as single CTAs.
+//   * the kernel size (1, 3, 5 or 7) is a run-time argument: taps = ks^2 k-blocks per input chunk, TMA's zero fill pads
+//     every shift; a 1x1 in-conv tile is a single k-block.
 //   * fixed k order, no split-K, no atomics: results are bit-identical for any batch size, position in the batch
 //     or grid (the decoder must regenerate the encoder's tables exactly, SURVEY.md H3).
 #include <cuda.h>
@@ -268,6 +272,36 @@ struct NarrowArgs {
     int A_elu;
 };
 
+// Dense W->W convs and in-convs of a model of padded width 128 (reswidth 65..128): the N = 128 tile with one channel
+// block per pixel half, single CTAs (tile t -> image t / 2, pixel half t & 1).  Trunk, residual, planes and bias are 128
+// channels wide.
+struct Tc128Args {
+    static constexpr int kN = BN, kCoBlocks = 1;
+    int taps, ks;
+    int cchunks;             // 32-channel chunks per tap: 4 for the dense W->W convs, 1 for the in-convs
+    const float *bias;       // [128]
+    const float *resid;      // [n,256,128] fp32 or null
+    float *T;                // trunk out or null
+    int T_elu;
+    __nv_bfloat16 *A_hi, *A_lo;   // next conv's input planes [n,256,128] or null
+    int A_elu;
+};
+
+// Dense W->W convs and in-convs of a model of padded width 192 (reswidth 129..192): the N = 64 tile with three channel
+// blocks per pixel half, single CTAs (tile t -> image t / 6, channel block (t >> 1) % 3, pixel half t & 1).  Trunk,
+// residual, planes and bias are 192 channels wide.
+struct Tc192Args {
+    static constexpr int kN = NW, kCoBlocks = 3;
+    int taps, ks;
+    int cchunks;             // 32-channel chunks per tap: 6 for the dense W->W convs, 1 for the in-convs
+    const float *bias;       // [192]
+    const float *resid;      // [n,256,192] fp32 or null
+    float *T;                // trunk out or null
+    int T_elu;
+    __nv_bfloat16 *A_hi, *A_lo;   // next conv's input planes [n,256,192] or null
+    int A_elu;
+};
+
 // Hand-off tile of the dense convs and in-convs: s = main + cross as fp32 [128 px][N ch] (N = 128, or 64 for NarrowArgs),
 // the 32-byte column chunks of row r XOR-swizzled by r & 3.  A row is a whole number of 128-byte bank lines, so without
 // the swizzle chunk j of rows r..r+3 would sit on the same 8 banks.  The consumers' float2 writes (a half warp covers
@@ -291,6 +325,14 @@ __device__ __forceinline__ void hand_store(const TcArgs &, float *hand, const fl
     dense_hand_store<BN>(hand, dm, dc, row, lane);
 }
 __device__ __forceinline__ void hand_store(const NarrowArgs &, float *hand, const float (&dm)[32], const float (&dc)[32], int row,
+                                           int lane) {
+    dense_hand_store<NW>(hand, dm, dc, row, lane);
+}
+__device__ __forceinline__ void hand_store(const Tc128Args &, float *hand, const float (&dm)[64], const float (&dc)[64], int row,
+                                           int lane) {
+    dense_hand_store<BN>(hand, dm, dc, row, lane);
+}
+__device__ __forceinline__ void hand_store(const Tc192Args &, float *hand, const float (&dm)[32], const float (&dc)[32], int row,
                                            int lane) {
     dense_hand_store<NW>(hand, dm, dc, row, lane);
 }
@@ -351,6 +393,15 @@ __device__ __forceinline__ void epilogue(const TcArgs &a, const float *hand, int
 
 __device__ __forceinline__ void epilogue(const NarrowArgs &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
     dense_epilogue<NW, NW, 2>(a, hand, img, mh, co0, ew, lane);
+}
+
+// Padded widths 128 and 192: the trunk and planes are the model's Wp channels wide; each row step of the N = 64 tile
+// stores 64 of a pixel's 192 channels, at channel block co0.
+__device__ __forceinline__ void epilogue(const Tc128Args &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
+    dense_epilogue<128, BN, 1>(a, hand, img, mh, co0, ew, lane);
+}
+__device__ __forceinline__ void epilogue(const Tc192Args &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
+    dense_epilogue<192, NW, 2>(a, hand, img, mh, co0, ew, lane);
 }
 
 // mu/sigma heads: the 3x3 W -> (n_mu + n_sc <= 32) convolution that ends every net (cifar_train.py:349,368,411,426),
@@ -608,9 +659,12 @@ int encode_map(CUtensorMap *m, void *base, int rank, const cuuint64_t *dims, con
 struct TcSlot { CUtensorMap map_hi, map_lo; };
 
 int bsw_model_tc_prepare(bsw_model *m) {
-    BSW_REQUIRE(m->Wp == 256 || m->Wp == NW,
-                "tensor-core conv path needs a padded width of 64 or 256 (reswidth 1..64 or 193..256)");
+    BSW_REQUIRE(m->Wp == 256 || m->Wp == 192 || m->Wp == 128 || m->Wp == NW,
+                "tensor-core conv path needs a padded width of 64, 128, 192 or 256 (reswidth 1..256)");
     const int Wp = m->Wp;
+    // output channels per tile of the dense convs and in-convs: the N = 64 tile for padded widths 64 and 192 (one and
+    // three channel blocks), the N = 128 tile for 128 and 256 (one and two)
+    const int dense_n = (Wp == NW || Wp == 192) ? NW : BN;
     TcState *ts = new TcState();
     m->tc_state = ts;
     const size_t act_elems = (size_t)m->d.max_batch * 256 * Wp;
@@ -668,7 +722,7 @@ int bsw_model_tc_prepare(bsw_model *m) {
         TcSlot s;
         cuuint64_t dims[3] = {(cuuint64_t)Kc, (cuuint64_t)rows, (cuuint64_t)taps};
         cuuint64_t str[2] = {(cuuint64_t)Kc * 2, (cuuint64_t)rows * Kc * 2};
-        cuuint32_t box[3] = {BK, (cuuint32_t)(head ? HD_N : Wp == NW ? NW : BN), 1};
+        cuuint32_t box[3] = {BK, (cuuint32_t)(head ? HD_N : dense_n), 1};
         if (int rc = encode_map(&s.map_hi, c.w_hi, 3, dims, str, box)) return rc;
         if (int rc = encode_map(&s.map_lo, c.w_lo, 3, dims, str, box)) return rc;
         c.tc_index = (int)slots->size();
@@ -678,9 +732,12 @@ int bsw_model_tc_prepare(bsw_model *m) {
     BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<TcArgs>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<BN>::SMEM));
     BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<HeadArgs>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<HD_N>::SMEM));
     BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<NarrowArgs>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<NW>::SMEM));
+    BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<Tc128Args>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<BN>::SMEM));
+    BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<Tc192Args>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<NW>::SMEM));
     // one SM-wide L1/shared split for every kernel of the path (see bsw_prefer_max_shared)
     bsw_prefer_max_shared(k_conv_wg<TcArgs>); bsw_prefer_max_shared(k_conv_wg<HeadArgs>);
     bsw_prefer_max_shared(k_conv_wg<NarrowArgs>);
+    bsw_prefer_max_shared(k_conv_wg<Tc128Args>); bsw_prefer_max_shared(k_conv_wg<Tc192Args>);
     bsw_prefer_max_shared(k_given_to_planes);
     m->tc_ready = true;
     return BSW_OK;
@@ -714,10 +771,11 @@ int bsw_tc_split(bsw_model *m, const float *in, int which, int64_t n, cudaStream
     return BSW_OK;
 }
 
-// Launch shape of the convolutions, a bit mask -- 1 / 2 = dense 3x3 / 5x5, 4 = in-convs and heads on a persistent grid
-// (one CTA or cluster per SM / cluster slot walking the tiles, the TMA ring prefetching across tile boundaries); a clear
-// bit means one CTA per tile.  8 = the dense convs and in-convs without TMA multicast: single CTAs, each loading its whole
-// stage; it has no effect on a model of padded width 64, whose narrow tiles always run as single CTAs.  Default 7
+// Launch shape of the convolutions, a bit mask -- 1 / 2 = dense convs of kernel size <= 3 / >= 5 (1x1 and 3x3 go with
+// 3x3, 7x7 with 5x5), 4 = in-convs and heads on a persistent grid (one CTA or cluster per SM / cluster slot walking the
+// tiles, the TMA ring prefetching across tile boundaries); a clear bit means one CTA per tile.  8 = the dense convs and
+// in-convs without TMA multicast: single CTAs, each loading its whole stage; it has no effect on a model of padded width
+// 64, 128 or 192, whose tiles always run as single CTAs.  Default 7
 // (BSW_TC_PERSIST overrides).  Same tiles, same k order per tile: results are bit-identical in every mode.
 static int g_tc_mode = -1;
 static int tc_mode() {
@@ -781,20 +839,23 @@ static int launch_tc(const CUtensorMap &amap_hi, const CUtensorMap &amap_lo, con
     return BSW_OK;
 }
 
-// Dense convs and in-convs of a model of padded width 64: single CTAs, one per tile or a persistent grid of one per SM.
-static int launch_tc_narrow(const CUtensorMap &amap_hi, const CUtensorMap &amap_lo, const TcSlot &s, const NarrowArgs &t,
-                            int64_t n, bool persistent, cudaStream_t st) {
-    const int ntiles = (int)n * 2;
-    k_conv_wg<NarrowArgs><<<tc_grid(ntiles, persistent), WG_THREADS, TileCfg<NW>::SMEM, st>>>(amap_hi, amap_lo, s.map_hi,
-                                                                                             s.map_lo, t, ntiles);
+// Dense convs and in-convs of a model of padded width 64, 128 or 192: single CTAs, one per tile or a persistent grid of
+// one per SM.
+template <class Args>
+static int launch_tc_single(const CUtensorMap &amap_hi, const CUtensorMap &amap_lo, const TcSlot &s, const Args &t, int64_t n,
+                            bool persistent, cudaStream_t st) {
+    const int ntiles = (int)n * 2 * Args::kCoBlocks;
+    k_conv_wg<Args><<<tc_grid(ntiles, persistent), WG_THREADS, TileCfg<Args::kN>::SMEM, st>>>(amap_hi, amap_lo, s.map_hi,
+                                                                                              s.map_lo, t, ntiles);
     BSW_LAUNCH_CHECK();
     return BSW_OK;
 }
 
-// Fills the fields TcArgs and NarrowArgs share (everything but cchunks).
-template <class Args> static Args tc_args(TcState *ts, const ConvSlot &c, const ConvArgs &a, const float *resid) {
+// Fills the fields the dense Args types share; cchunks = 32-channel chunks per tap of the input planes.
+template <class Args>
+static Args tc_args(TcState *ts, const ConvSlot &c, const ConvArgs &a, const float *resid, int cchunks) {
     Args t;
-    t.taps = c.ks * c.ks; t.ks = c.ks;
+    t.taps = c.ks * c.ks; t.ks = c.ks; t.cchunks = cchunks;
     t.bias = c.bias; t.resid = resid; t.T = a.T; t.T_elu = a.T_elu;
     t.A_hi = a.A_planes >= 0 ? ts->act[a.A_planes][0] : nullptr;
     t.A_lo = a.A_planes >= 0 ? ts->act[a.A_planes][1] : nullptr;
@@ -802,20 +863,26 @@ template <class Args> static Args tc_args(TcState *ts, const ConvSlot &c, const 
     return t;
 }
 
+// One dense conv or in-conv on the tile of the model's padded width, reading the planes behind amap_hi / amap_lo.
+static int launch_dense(bsw_model *m, const CUtensorMap &amap_hi, const CUtensorMap &amap_lo, const TcSlot &s,
+                        const ConvSlot &c, const ConvArgs &a, const float *resid, int cchunks, int64_t n, bool persistent,
+                        cudaStream_t st) {
+    TcState *ts = (TcState *)m->tc_state;
+    switch (m->Wp) {
+        case NW:  return launch_tc_single(amap_hi, amap_lo, s, tc_args<NarrowArgs>(ts, c, a, resid, cchunks), n, persistent, st);
+        case 128: return launch_tc_single(amap_hi, amap_lo, s, tc_args<Tc128Args>(ts, c, a, resid, cchunks), n, persistent, st);
+        case 192: return launch_tc_single(amap_hi, amap_lo, s, tc_args<Tc192Args>(ts, c, a, resid, cchunks), n, persistent, st);
+        default:  return launch_tc(amap_hi, amap_lo, s, tc_args<TcArgs>(ts, c, a, resid, cchunks), n, persistent, st);
+    }
+}
+
 // a.in must be one of the plane buffers: a.in_planes = 0/1 selects it; outputs a.A_planes = 0/1/-1.
 int bsw_conv_tc(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t n, cudaStream_t st) {
     TcState *ts = (TcState *)m->tc_state;
     BSW_REQUIRE(ts && c.tc_index >= 0, "bsw_conv_tc: conv has no tensor-core weights");
     const TcSlot &s = (*(std::vector<TcSlot> *)m->tc_slots)[c.tc_index];
-    const bool persistent = tc_persistent(c.ks <= 3 ? 1 : 2);
-    if (m->Wp == NW) {
-        NarrowArgs t = tc_args<NarrowArgs>(ts, c, a, a.resid);
-        t.cchunks = NW / BK;
-        return launch_tc_narrow(ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1], s, t, n, persistent, st);
-    }
-    TcArgs t = tc_args<TcArgs>(ts, c, a, a.resid);
-    t.cchunks = 8;
-    return launch_tc(ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1], s, t, n, persistent, st);
+    return launch_dense(m, ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1], s, c, a, a.resid, m->Wp / BK, n,
+                        tc_persistent(c.ks <= 3 ? 1 : 2), st);
 }
 
 // Heads: reads the planes the last ResNet conv wrote (in_planes), writes mu / sigma.  BSW_TC_HEADS=0 keeps the float32 SIMT
@@ -847,17 +914,7 @@ int bsw_conv_tc_in(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t n
     int64_t cnt = n * 256 * 32;
     k_given_to_planes<<<(unsigned)((cnt + 255) / 256), 256, 0, st>>>(a.in, a.in_dim, c.Cin, a.in_mode, ts->inp[0], ts->inp[1], n);
     BSW_LAUNCH_CHECK();
-    int rc;
-    if (m->Wp == NW) {
-        NarrowArgs t = tc_args<NarrowArgs>(ts, c, a, nullptr);
-        t.cchunks = 1;
-        rc = launch_tc_narrow(ts->inp_map[0], ts->inp_map[1], s, t, n, tc_persistent(4), st);
-    } else {
-        TcArgs t = tc_args<TcArgs>(ts, c, a, nullptr);
-        t.cchunks = 1;
-        rc = launch_tc(ts->inp_map[0], ts->inp_map[1], s, t, n, tc_persistent(4), st);
-    }
-    if (rc) return rc;
+    if (int rc = launch_dense(m, ts->inp_map[0], ts->inp_map[1], s, c, a, nullptr, 1, n, tc_persistent(4), st)) return rc;
     *launches += 2;
     return BSW_OK;
 }

@@ -46,11 +46,14 @@ __device__ __forceinline__ float scale_transform(float r, int kind) {
 // 8-pixel row segment x TCO output channels.
 // ------------------------------------------------------------------------------------------------
 constexpr int CC = 8;          // input channels per shared-memory chunk
-constexpr int IWS = 20;        // padded row stride of the input patch (floats)
+// padded row stride of the input patch (floats): at least its 16 + KS - 1 columns, a multiple of 4 for the float4 row loads
+template <int KS> constexpr int IWS_OF = KS <= 5 ? 20 : 24;
 
+// Shared memory: [CC][IH][IWS] input patch + [KS^2][CC][COT] weights.  KS = 7, TCO = 8: 16.5 KB + 98 KB = 114.5 KB, so
+// one CTA per SM (the KS <= 5 instantiations keep two); KS = 7, TCO = 2: 41 KB.
 template <int KS, int TCO>
 __global__ void __launch_bounds__(256, 2) k_conv_simt(ConvArgs a) {
-    constexpr int R = KS / 2, IH = 16 + KS - 1, COT = 8 * TCO, TAPS = KS * KS;
+    constexpr int R = KS / 2, IH = 16 + KS - 1, COT = 8 * TCO, TAPS = KS * KS, IWS = IWS_OF<KS>;
     extern __shared__ float sm[];
     float *in_s = sm;                               // [CC][IH][IWS]
     float *w_s = sm + CC * IH * IWS;                // [TAPS][CC][COT]
@@ -111,15 +114,17 @@ __global__ void __launch_bounds__(256, 2) k_conv_simt(ConvArgs a) {
 #pragma unroll
             for (int dy = 0; dy < KS; ++dy) {
                 const float *rp = in_s + (ci * IH + prow + dy) * IWS + pcol0;
-                float iv[8 + KS - 1];
+                // the 8 + KS - 1 patch values this row of taps reads: float4 loads, then a float2 tail (KS = 3, 7)
+                constexpr int NV = 8 + KS - 1, NV4 = NV / 4 * 4;
+                float iv[NV];
 #pragma unroll
-                for (int v4 = 0; v4 < (8 + KS - 1) / 4; ++v4) {
+                for (int v4 = 0; v4 < NV / 4; ++v4) {
                     float4 q4 = *reinterpret_cast<const float4 *>(rp + 4 * v4);
                     iv[4 * v4] = q4.x; iv[4 * v4 + 1] = q4.y; iv[4 * v4 + 2] = q4.z; iv[4 * v4 + 3] = q4.w;
                 }
-                if constexpr ((8 + KS - 1) % 4 == 2) {
-                    float2 q2 = *reinterpret_cast<const float2 *>(rp + 8);
-                    iv[8] = q2.x; iv[9] = q2.y;
+                if constexpr (NV % 4 == 2) {
+                    float2 q2 = *reinterpret_cast<const float2 *>(rp + NV4);
+                    iv[NV4] = q2.x; iv[NV4 + 1] = q2.y;
                 }
 #pragma unroll
                 for (int dx = 0; dx < KS; ++dx) {
@@ -197,7 +202,7 @@ __global__ void __launch_bounds__(256, 2) k_conv_simt(ConvArgs a) {
 template <int KS, int TCO>
 static int launch_conv_simt(const ConvArgs &a, int64_t n, cudaStream_t st) {
     constexpr int IH = 16 + KS - 1, COT = 8 * TCO;
-    size_t smem = sizeof(float) * (CC * IH * IWS + KS * KS * CC * COT);
+    size_t smem = sizeof(float) * (CC * IH * IWS_OF<KS> + KS * KS * CC * COT);
     static bool attr_done = false;
     if (!attr_done) {
         BSW_CUDA(cudaFuncSetAttribute(k_conv_simt<KS, TCO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -214,7 +219,9 @@ int bsw_conv_simt(const ConvArgs &a, int ks, int64_t n, cudaStream_t st) {
     bool wide = (a.CoutP % 64) == 0;
     if (ks == 5) return wide ? launch_conv_simt<5, 8>(a, n, st) : launch_conv_simt<5, 2>(a, n, st);
     if (ks == 3) return wide ? launch_conv_simt<3, 8>(a, n, st) : launch_conv_simt<3, 2>(a, n, st);
-    bsw_set_error("conv kernel size %d not supported (3 or 5)", ks);
+    if (ks == 1) return wide ? launch_conv_simt<1, 8>(a, n, st) : launch_conv_simt<1, 2>(a, n, st);
+    if (ks == 7) return wide ? launch_conv_simt<7, 8>(a, n, st) : launch_conv_simt<7, 2>(a, n, st);
+    bsw_set_error("conv kernel size %d not supported (1, 3, 5 or 7)", ks);
     return BSW_E_INVALID;
 }
 
@@ -252,14 +259,18 @@ static void add_block(bsw_model *m, NetPlan &np, const std::string &prefix, int 
 
 extern "C" int bsw_model_create(bsw_model **out, const bsw_model_desc *d) {
     BSW_REQUIRE(out && d, "bsw_model_create: null argument");
-    BSW_REQUIRE(d->nz >= 1 && d->xc >= 1 && d->zchannels >= 1 && d->reswidth >= 1 && d->kernel_size == 3 &&
-                d->nprocessing >= 0 && d->resdepth >= 0 && d->max_batch >= 1, "bsw_model_create: bad descriptor");
+    BSW_REQUIRE(d->nz >= 1 && d->xc >= 1 && d->zchannels >= 1 && d->reswidth >= 1 && d->nprocessing >= 0 &&
+                d->resdepth >= 0 && d->max_batch >= 1, "bsw_model_create: bad descriptor");
+    BSW_REQUIRE(d->kernel_size == 1 || d->kernel_size == 3 || d->kernel_size == 5 || d->kernel_size == 7,
+                "bsw_model_create: kernel_size must be 1, 3, 5 or 7");
     bsw_model *m = new bsw_model();
     m->d = *d;
     m->Wp = round_up(d->reswidth, 64);
     m->zdim = d->zchannels * 256;
     m->xdim = d->xc * 1024;
-    const int W = d->reswidth, zc = d->zchannels, C = d->xc, nz = d->nz;
+    // ks: the reference's self.kernel_size (ResNet blocks res1 / deep*_res, z in-convs, heads); infer_in and the
+    // nprocessing blocks are 5x5 whatever it is (padding_proc, cifar_train.py:45-47)
+    const int W = d->reswidth, zc = d->zchannels, C = d->xc, nz = d->nz, ks = d->kernel_size;
     std::vector<int> rd(nz, 0);                        // model/cifar_train.py:66-72
     for (int r = 0, i = 0; r < d->resdepth; ++r) { if (i == nz) i = 0; rd[i++]++; }
 
@@ -272,8 +283,8 @@ extern "C" int bsw_model_create(bsw_model **out, const bsw_model_desc *d) {
         m->names["infer_in.1"] = {np.in_conv, 0};
         np.in_mode = IN_CHW_X; np.in_dim = m->xdim;
         add_block(m, np, "infer_res0.0", 5, d->nprocessing);
-        add_block(m, np, "infer_res1.0", 3, rd[0]);
-        np.head = add_conv(m, "infer_mu|infer_std", W, 2 * zc, 3, 16);
+        add_block(m, np, "infer_res1.0", ks, rd[0]);
+        np.head = add_conv(m, "infer_mu|infer_std", W, 2 * zc, ks, 16);
         m->convs[np.head].CinP = m->Wp; m->convs[np.head].parts = 2;
         m->names["infer_mu"] = {np.head, 0};
         m->names["infer_std"] = {np.head, zc};
@@ -285,11 +296,11 @@ extern "C" int bsw_model_create(bsw_model **out, const bsw_model_desc *d) {
         for (int j = 0; j + 1 < nz; ++j) {
             NetPlan &np = kind == 0 ? m->infer[j + 1] : m->gen[j + 1];
             std::string js = std::to_string(j);
-            np.in_conv = add_conv(m, nm + "_in." + js + ".0", zc, W, 3, 64);
+            np.in_conv = add_conv(m, nm + "_in." + js + ".0", zc, W, ks, 64);
             m->names[nm + "_in." + js + ".0"] = {np.in_conv, 0};
             np.in_mode = IN_CHW_Z; np.in_dim = m->zdim;
-            add_block(m, np, nm + "_res." + js + ".0", 3, rd[j + 1]);
-            np.head = add_conv(m, nm + "_mu|std." + js, W, 2 * zc, 3, 16);
+            add_block(m, np, nm + "_res." + js + ".0", ks, rd[j + 1]);
+            np.head = add_conv(m, nm + "_mu|std." + js, W, 2 * zc, ks, 16);
             m->convs[np.head].CinP = m->Wp; m->convs[np.head].parts = 2;
             m->names[nm + "_mu." + js + ".0"] = {np.head, 0};
             m->names[nm + "_std." + js + ".0"] = {np.head, zc};
@@ -300,13 +311,13 @@ extern "C" int bsw_model_create(bsw_model **out, const bsw_model_desc *d) {
     // ---- generate(0): cifar_train.py:247-308, 396-411
     {
         NetPlan &np = m->gen[0];
-        np.in_conv = add_conv(m, "gen_in.0", zc, W, 3, 64);
+        np.in_conv = add_conv(m, "gen_in.0", zc, W, ks, 64);
         m->names["gen_in.0"] = {np.in_conv, 0};
         np.in_mode = IN_CHW_Z; np.in_dim = m->zdim;
-        add_block(m, np, "gen_res1.0", 3, rd[0]);
+        add_block(m, np, "gen_res1.0", ks, rd[0]);
         add_block(m, np, "gen_res0.0", 5, d->nprocessing);
         int nh = d->cond_xscale ? 8 * C : 4 * C;
-        np.head = add_conv(m, "gen_mu.0|gen_std.0", W, nh, 3, 16);
+        np.head = add_conv(m, "gen_mu.0|gen_std.0", W, nh, ks, 16);
         m->convs[np.head].CinP = m->Wp; m->convs[np.head].parts = d->cond_xscale ? 2 : 1;
         m->names["gen_mu.0"] = {np.head, 0};
         if (d->cond_xscale) m->names["gen_std.0"] = {np.head, 4 * C};
@@ -508,7 +519,7 @@ static int run_net(bsw_model *m, const NetPlan &np, const float *given, int64_t 
                     a.in_planes = 1; a.A_planes = (last_layer && last_block) ? -1 : 0;
                     if (last_layer && last_block && tc_head) { a.A_planes = 0; a.A_elu = 0; }     // planes = the trunk itself (already ELU'd)
                 }
-                prof->begin(c.ks == 5 ? CAT_CONV_DENSE5 : CAT_CONV_DENSE3, st);
+                prof->begin(c.ks <= 3 ? CAT_CONV_DENSE3 : CAT_CONV_DENSE5, st);     // as conv mode bits 1 / 2
                 if (int rc = dispatch_conv(m, np, ROLE_DENSE, c, a, n, st, launches)) return rc;
                 prof->end(st);
             }
@@ -532,8 +543,8 @@ static int run_net(bsw_model *m, const NetPlan &np, const float *given, int64_t 
 // Test hook: one conv of a loaded model through dispatch_conv, with the epilogue selected by `flags`.  The conv's role
 // and net come from the model's plans; a head is named by its mu prefix.  Tensor-core dense convs and heads read plane
 // buffer 0, split from in_dev here by the same RNE split the epilogues use; dense convs write plane buffer 1, in-convs
-// plane buffer 0.  The written buffer is filled with 0xffff first and copied whole ([2][max_batch,256,Wp], Wp = 64 or
-// 256) to planes_dev, so rows the conv must not touch can be checked.
+// plane buffer 0.  The written buffer is filled with 0xffff first and copied whole ([2][max_batch,256,Wp], Wp = 64, 128,
+// 192 or 256) to planes_dev, so rows the conv must not touch can be checked.
 extern "C" int bsw_selftest_conv(bsw_model *m, const char *prefix, const float *in_dev, int64_t n, int flags, float *T_dev,
                                  float *A_dev, uint16_t *planes_dev, float *mu_dev, float *scale_dev, void *stream) {
     BSW_REQUIRE(m && prefix && in_dev, "bsw_selftest_conv: null argument");

@@ -27,11 +27,12 @@ class _Desc(ctypes.Structure):
 class Model:
     def __init__(self, xs=(3, 32, 32), nz=1, zchannels=16, nprocessing=1, kernel_size=3, resdepth=2, reswidth=256,
                  dropout_p=0., tag='', root_process=True, cond_xscale=False, max_batch=1, use_tensor_cores=False, device=None):
+        # the config validates the architecture (kernel_size: ValueError) before any device work
+        self.cfg = CodecConfig(xs=tuple(xs), nz=nz, zchannels=zchannels, nprocessing=nprocessing, kernel_size=kernel_size,
+                               resdepth=resdepth, reswidth=reswidth, cond_xscale=cond_xscale)
         if not torch.cuda.is_available():
             raise RuntimeError("bitswap_b200.Model needs a CUDA device (no CPU fallback)")
         assert tuple(xs[1:]) == (32, 32), "blocks are always 32x32 (latents 16x16)"
-        self.cfg = CodecConfig(xs=tuple(xs), nz=nz, zchannels=zchannels, nprocessing=nprocessing, kernel_size=kernel_size,
-                               resdepth=resdepth, reswidth=reswidth, cond_xscale=cond_xscale)
         self.xs, self.nz, self.zchannels = tuple(xs), nz, zchannels
         self.zdim = (zchannels, 16, 16)
         self.compressing = False

@@ -208,8 +208,9 @@ int bsw_rows6_set_lanes_per_row(int lpr);
 /* Launch shape of the tensor-core convolutions, a bit mask: 1 / 2 / 4 = dense 3x3 / dense 5x5 / in-convs and heads on a
  * persistent grid (one CTA per SM, or one four-CTA cluster per four SMs, walking half-image tiles); a clear bit = one
  * CTA per tile.  8 = dense convs and in-convs as single CTAs without TMA multicast (by default each image's four tiles
- * run as one cluster sharing their operand loads); no effect on a model of padded width 64, whose narrow tiles always
- * run as single CTAs.  -1 = default (BSW_TC_PERSIST if set, else 7).  Bit-identical results. */
+ * run as one cluster sharing their operand loads); no effect on a model of padded width 64, 128 or 192, whose tiles
+ * always run as single CTAs.  Bits 1 / 2 split the dense convs by kernel size: <= 3 (1x1, 3x3) / >= 5 (5x5, 7x7).
+ * -1 = default (BSW_TC_PERSIST if set, else 7).  Bit-identical results. */
 int bsw_set_conv_mode(int mode);
 int bsw_rows6_verify_read(uint64_t *out4_host);
 int bsw_logistic_push_2p(bsw_streams *s, int first, int count, const float *mu_dev, int64_t mu_stream_stride,
@@ -272,13 +273,14 @@ typedef struct {
     int32_t nz;
     int32_t zchannels;
     int32_t nprocessing;
-    int32_t kernel_size;   /* 3 */
+    int32_t kernel_size;   /* 1, 3, 5 or 7 (else BSW_E_INVALID): ResNet blocks of the levels, z in-convs, heads;
+                              infer_in and the nprocessing blocks are always 5x5 */
     int32_t resdepth;
     int32_t reswidth;
     int32_t cond_xscale;   /* imagenetcrop: x-scale from a conv head */
     int32_t max_batch;     /* activations are preallocated for this many images */
-    int32_t use_tensor_cores; /* 1: wgmma tensor-core path for the W->W convs (needs padded width 64 or 256, i.e.
-                                 reswidth 1..64 or 193..256); 0: fp32 SIMT */
+    int32_t use_tensor_cores; /* 1: wgmma tensor-core path for the W->W convs (needs a padded width of 64, 128,
+                                 192 or 256, i.e. reswidth 1..256); 0: fp32 SIMT */
 } bsw_model_desc;
 
 int bsw_model_create(bsw_model **out, const bsw_model_desc *desc);

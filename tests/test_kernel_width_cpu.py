@@ -1,0 +1,119 @@
+"""CPU-only checks for models of any kernel size (1, 3, 5, 7) and padded width (64, 128, 192, 256):
+
+1. the new conv instantiations in the built library (cuobjdump -res-usage): the padded-width-128 and -192 tiles of
+   k_conv_wg within the launch shape (<= 128 registers, no spills), k_conv_simt at kernel sizes 1 and 7 without spills;
+2. config validation: an even kernel size, or one outside 1..7, is refused before any device work, by CodecConfig and
+   Model (ValueError) and by bsw_model_create (BSW_E_INVALID);
+3. the float32 / float64 model oracle against the reference Model's outputs for --kernel 5 / 1 / 7 models
+   (tests/golden/make_golden_kw.py).
+"""
+import ctypes
+import json
+import os
+import re
+import subprocess
+
+import numpy as np
+import pytest
+import torch
+
+from bitswap_b200 import _lib, synthetic
+from bitswap_b200.config import CodecConfig
+from bitswap_b200.model import Model, _Desc
+from bitswap_b200.rand import ImageBins
+from oracle import oracle as O
+
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+KW_MODELS = ["kw_k5_w100", "kw_k1_w12", "kw_k7_w16"]
+
+
+@pytest.fixture(scope="module")
+def usage():
+    so = _lib.build()
+    out = subprocess.run(["cuobjdump", "-res-usage", so], stdout=subprocess.PIPE, stderr=subprocess.STDOUT,
+                         text=True).stdout
+    res = {}
+    for name, line in re.findall(r"Function (\S*(?:k_conv_wg|k_conv_simt)I\S*):\s*\n\s*(REG:.*)", out):
+        res[name] = {k: int(v) for k, v in re.findall(r"(\w+):(\d+)", line)}
+    return res
+
+
+@pytest.mark.parametrize("args", ["Tc128Args", "Tc192Args"])
+def test_new_tiles_fit_the_launch_shape(usage, args):
+    u = [v for k, v in usage.items() if re.search(rf"k_conv_wgINS_\d+{args}EEEv", k)]
+    assert len(u) == 1, sorted(usage)
+    assert u[0]["REG"] <= 128, u[0]
+    assert u[0]["LOCAL"] == 0 and u[0]["STACK"] == 0, f"{args} spills: {u[0]}"
+
+
+@pytest.mark.parametrize("ks,tco", [(1, 2), (1, 8), (7, 2), (7, 8)])
+def test_simt_kernel_sizes_1_and_7_do_not_spill(usage, ks, tco):
+    u = [v for k, v in usage.items() if f"k_conv_simtILi{ks}ELi{tco}EE" in k]
+    assert len(u) == 1, sorted(usage)
+    assert u[0]["LOCAL"] == 0 and u[0]["STACK"] == 0, f"k_conv_simt<{ks}, {tco}> spills: {u[0]}"
+
+
+@pytest.mark.parametrize("ks", [1, 3, 5, 7])
+def test_config_accepts_odd_kernels_up_to_7(ks):
+    assert CodecConfig(kernel_size=ks).kernel_size == ks
+
+
+@pytest.mark.parametrize("ks", [-1, 0, 2, 4, 6, 8, 9, 11])
+def test_config_and_model_refuse_other_kernels(ks):
+    with pytest.raises(ValueError):
+        CodecConfig(kernel_size=ks)
+    with pytest.raises(ValueError):
+        Model(xs=(3, 32, 32), nz=2, zchannels=8, kernel_size=ks, reswidth=100)
+
+
+@pytest.mark.parametrize("ks,rc", [(4, 4), (9, 4), (0, 4)])
+def test_model_create_refuses_other_kernels(ks, rc):
+    """The descriptor check comes before any allocation: BSW_E_INVALID, no device needed."""
+    h = ctypes.c_void_p()
+    d = _Desc(3, 2, 8, 1, ks, 2, 100, 0, 1, 1)
+    assert _lib.lib().bsw_model_create(ctypes.byref(h), ctypes.byref(d)) == rc
+    assert not h.value
+    assert "kernel_size" in _lib.lib().bsw_last_error().decode()
+
+
+def _golden(name):
+    g = np.load(os.path.join(GOLDEN, f"model_{name}.npz"))
+    c = json.loads(str(g["cfg"]))
+    c["xs"] = tuple(c["xs"])
+    return CodecConfig(**c), g
+
+
+def model_oracle_vs_golden(name, net, tol):
+    """Runs net(kind, level, given [1, dim] float64) -> (mu, scale) on the golden inputs of `name`; every output within
+    tol(want) of the reference's."""
+    cfg, g = _golden(name)
+    _, zcen = synthetic.synthetic_bins(cfg, seed=0)
+    xcen = ImageBins(torch.float64, "cpu", cfg.xdim).centres()
+    zr = torch.arange(cfg.zdim)
+    worst = 0.0
+    for i in range(cfg.nz):
+        if i == 0:
+            given = xcen[torch.arange(cfg.xdim), torch.from_numpy(g["x"].astype(np.int64))]
+        else:
+            given = zcen[i - 1, zr, torch.from_numpy(g[f"zsym_in_infer{i}"].astype(np.int64))]
+        z = zcen[i, zr, torch.from_numpy(g[f"zsym_in_gen{i}"].astype(np.int64))]
+        for kind, inp, key in (("infer", given, f"infer{i}"), ("generate", z, f"gen{i}")):
+            mu, sc = net(kind, i, inp.unsqueeze(0))
+            for got, want in ((mu, g[key + "_mu"]), (sc, g[key + "_scale"])):
+                err = np.abs(got[0].detach().cpu().double().numpy() - want)
+                worst = max(worst, float(err.max()))
+                assert np.all(err < tol(want)), f"{name} {key}: max |err| {err.max():.3e}"
+    return worst
+
+
+@pytest.mark.parametrize("name", KW_MODELS)
+def test_kw_model_oracle_matches_reference(name):
+    """The oracle builds --kernel 5 / 1 / 7 models as the reference does: float32 within 2e-6 absolute of the golden
+    outputs (measured: identical), float64 within 2e-5 relative to max(1, |output|).  The golden outputs carry the
+    reference's float32 rounding, which grows with the taps summed: measured 9.6e-7 (1x1), 3.2e-6 (5x5) and 6.9e-6
+    (7x7) absolute against the float64 oracle."""
+    cfg, _ = _golden(name)
+    sd = synthetic.synthetic_state_dict(cfg, seed=50, varied=True)
+    for dtype, tol in ((torch.float32, lambda want: 2e-6), (torch.float64, lambda want: 2e-5 * np.maximum(1.0, np.abs(want)))):
+        orc = O.ModelOracle(cfg, sd, dtype=dtype)
+        model_oracle_vs_golden(name, lambda kind, i, g: (orc.infer(i) if kind == "infer" else orc.generate(i))(g), tol)
