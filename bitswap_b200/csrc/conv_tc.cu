@@ -33,7 +33,10 @@
 //     A model of padded width 64 (reswidth 1..64, the MNIST models) has one 64-channel block per pixel half: its dense
 //     convs and in-convs run the narrow tile (NarrowArgs) as single CTAs, one per tile.  Padded width 128 runs the
 //     N = 128 tile with one channel block (Tc128Args), padded width 192 the N = 64 tile with three (Tc192Args), both
-//     as single CTAs.
+//     as single CTAs.  Padded widths 320, 384, 448 and 512 (reswidth 257..512) run the N = 64 tile with Wp / 64 channel
+//     blocks (TcWideArgs<Wp>), single CTAs too.  Their dense convs and heads (HeadWideArgs) fold the main accumulator
+//     into a float32 register accumulator after every tap: K reaches 49 x 512 there, and the tensor core's truncating
+//     accumulate would otherwise lose accuracy in proportion to K.
 //   * the kernel size (1, 3, 5 or 7) is a run-time argument: taps = ks^2 k-blocks per input chunk, TMA's zero fill pads
 //     every shift; a 1x1 in-conv tile is a single k-block.
 //   * fixed k order, no split-K, no atomics: results are bit-identical for any batch size, position in the batch
@@ -302,6 +305,27 @@ struct Tc192Args {
     int A_elu;
 };
 
+// Dense W->W convs and in-convs of a model of padded width WP = 320, 384, 448 or 512 (reswidth 257..512): the N = 64
+// tile with WP / 64 channel blocks per pixel half, single CTAs (tile t -> image t / (2 WP / 64), channel block
+// (t >> 1) % (WP / 64), pixel half t & 1).  Trunk, residual, planes and bias are WP channels wide.  The dense convs fold
+// the main accumulator once per tap (see k_conv_wg), so it never sums more than WP terms.
+template <int WP> struct TcWideArgs {
+    static constexpr int kN = NW, kCoBlocks = WP / NW;
+    int taps, ks;
+    int cchunks;             // 32-channel chunks per tap: WP / 32 for the dense W->W convs, 1 for the in-convs
+    const float *bias;       // [WP]
+    const float *resid;      // [n,256,WP] fp32 or null
+    float *T;                // trunk out or null
+    int T_elu;
+    __nv_bfloat16 *A_hi, *A_lo;   // next conv's input planes [n,256,WP] or null
+    int A_elu;
+};
+
+// Tiles whose consumers fold the main accumulator into a float32 register accumulator after every tap of more than one
+// k-block: the wide dense convs and the wide heads.  Widths <= 256 do not fold (their results stay as they were).
+template <class Args> struct Folds { static constexpr bool value = false; };
+template <int WP> struct Folds<TcWideArgs<WP>> { static constexpr bool value = true; };
+
 // Hand-off tile of the dense convs and in-convs: s = main + cross as fp32 [128 px][N ch] (N = 128, or 64 for NarrowArgs),
 // the 32-byte column chunks of row r XOR-swizzled by r & 3.  A row is a whole number of 128-byte bank lines, so without
 // the swizzle chunk j of rows r..r+3 would sit on the same 8 banks.  The consumers' float2 writes (a half warp covers
@@ -335,6 +359,19 @@ __device__ __forceinline__ void hand_store(const Tc128Args &, float *hand, const
 __device__ __forceinline__ void hand_store(const Tc192Args &, float *hand, const float (&dm)[32], const float (&dc)[32], int row,
                                            int lane) {
     dense_hand_store<NW>(hand, dm, dc, row, lane);
+}
+// Folding tiles: s = (outer + main) + cross, in that order for every element, so the result does not depend on the grid.
+template <int WP>
+__device__ __forceinline__ void hand_store(const TcWideArgs<WP> &, float *hand, const float (&outer)[32], const float (&dm)[32],
+                                           const float (&dc)[32], int row, int lane) {
+#pragma unroll
+    for (int j = 0; j < NW / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int i = 4 * j + 2 * h;
+            *reinterpret_cast<float2 *>(hand + hand_idx<NW>(row + 8 * h, 8 * j + 2 * (lane & 3))) =
+                make_float2((outer[i] + dm[i]) + dc[i], (outer[i + 1] + dm[i + 1]) + dc[i + 1]);
+        }
 }
 
 // Dense / in-conv epilogue, run by the epilogue warps from the hand-off tile: s + bias (+ residual) (-> ELU) -> trunk;
@@ -403,6 +440,10 @@ __device__ __forceinline__ void epilogue(const Tc128Args &a, const float *hand, 
 __device__ __forceinline__ void epilogue(const Tc192Args &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
     dense_epilogue<192, NW, 2>(a, hand, img, mh, co0, ew, lane);
 }
+template <int WP>
+__device__ __forceinline__ void epilogue(const TcWideArgs<WP> &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
+    dense_epilogue<WP, NW, 2>(a, hand, img, mh, co0, ew, lane);
+}
 
 // mu/sigma heads: the 3x3 W -> (n_mu + n_sc <= 32) convolution that ends every net (cifar_train.py:349,368,411,426),
 // with the scale transforms and the UnSqueeze2d index map of the x head in the epilogue.
@@ -438,6 +479,24 @@ __device__ __forceinline__ void hand_store(const HeadArgs &, float *hand, const 
             for (int e = 0; e < 2; ++e) {
                 const int i = 4 * j + 2 * h + e;
                 hand[(8 * j + 2 * (lane & 3) + e) * HD_LD + row + 8 * h] = dm[i] + dc[i];
+            }
+}
+
+// Heads of a model of padded width 320..512: K = taps x Wp (up to 49 x 512), so they fold once per tap like the wide
+// dense convs.  Same fields and epilogue as HeadArgs; a type of its own keeps k_conv_wg<HeadArgs> as it is.
+struct HeadWideArgs : HeadArgs {};
+template <> struct Folds<HeadWideArgs> { static constexpr bool value = true; };
+
+__device__ __forceinline__ void hand_store(const HeadWideArgs &, float *hand, const float (&outer)[16], const float (&dm)[16],
+                                           const float (&dc)[16], int row, int lane) {
+#pragma unroll
+    for (int j = 0; j < HD_N / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int i = 4 * j + 2 * h + e;
+                hand[(8 * j + 2 * (lane & 3) + e) * HD_LD + row + 8 * h] = (outer[i] + dm[i]) + dc[i];
             }
 }
 
@@ -557,12 +616,21 @@ k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ C
         if (mc) { mbar_arrive_cluster(&empty_bar[s], rank); mbar_arrive_cluster(&empty_bar[s], rank ^ 1); mbar_arrive_cluster(&empty_bar[s], rank ^ 2); }
         else mbar_arrive(&empty_bar[s]);
     };
+    // Folding tiles (Folds<Args>): after the last k-block of every tap but the last, the consumers retire the MMAs in
+    // flight, add the main accumulator into `outer` (float32 RNE adds) and restart it from zero, so the tensor core's
+    // truncating accumulate never sums more than one tap's Wp terms into it.  In-convs (one k-block per tap) do not fold.
+    constexpr bool fold = Folds<Args>::value;
+    const bool fold_taps = fold && a.cchunks > 1;
     int stage = 0, phase = 0, it = 0;
     for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++it) {
-        float dm[N / 2], dc[N / 2];
+        float dm[N / 2], dc[N / 2], outer[fold ? N / 2 : 1];
 #pragma unroll
         for (int i = 0; i < N / 2; ++i) { dm[i] = 0.f; dc[i] = 0.f; }
-        int prev = -1;
+        if constexpr (fold) {
+#pragma unroll
+            for (int i = 0; i < N / 2; ++i) outer[i] = 0.f;
+        }
+        int prev = -1, kc = 0;
         for (int kb = 0; kb < nkb; ++kb) {
             mbar_wait(&full_bar[stage], phase);
             const uint32_t sbase = smem_u32(smem + stage * C::STAGE);
@@ -578,9 +646,20 @@ k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ C
                 Wgmma<N>::mma(dc, a_hi, b_lo);
             }
             wg_commit();
-            wg_wait<1>();                                  // the previous k-block's MMAs have read their stage
-            if (prev >= 0) release(prev);
-            prev = stage;
+            if (fold_taps && ++kc == a.cchunks && kb + 1 < nkb) {
+                kc = 0;
+                wg_wait<0>();                              // this tap's MMAs are done: both stages can go
+                fence_regs(dm);
+#pragma unroll
+                for (int i = 0; i < N / 2; ++i) { outer[i] += dm[i]; dm[i] = 0.f; }
+                if (prev >= 0) release(prev);
+                release(stage);
+                prev = -1;
+            } else {
+                wg_wait<1>();                              // the previous k-block's MMAs have read their stage
+                if (prev >= 0) release(prev);
+                prev = stage;
+            }
             if (++stage == C::NSTAGE) { stage = 0; phase ^= 1; }
         }
         wg_wait<0>();
@@ -588,7 +667,8 @@ k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ C
         fence_regs(dc);
         if (prev >= 0) release(prev);
         mbar_wait(acc_empty, (it & 1) ^ 1);            // the epilogue has read the previous tile
-        hand_store(a, hand, dm, dc, row0, lane);
+        if constexpr (fold) hand_store(a, hand, outer, dm, dc, row0, lane);
+        else hand_store(a, hand, dm, dc, row0, lane);
         mbar_arrive(acc_full);
     }
 }
@@ -659,12 +739,12 @@ int encode_map(CUtensorMap *m, void *base, int rank, const cuuint64_t *dims, con
 struct TcSlot { CUtensorMap map_hi, map_lo; };
 
 int bsw_model_tc_prepare(bsw_model *m) {
-    BSW_REQUIRE(m->Wp == 256 || m->Wp == 192 || m->Wp == 128 || m->Wp == NW,
-                "tensor-core conv path needs a padded width of 64, 128, 192 or 256 (reswidth 1..256)");
+    BSW_REQUIRE(m->Wp % 64 == 0 && m->Wp <= 512,
+                "tensor-core conv path needs a padded width of 64, 128, ..., 512 (reswidth 1..512)");
     const int Wp = m->Wp;
-    // output channels per tile of the dense convs and in-convs: the N = 64 tile for padded widths 64 and 192 (one and
-    // three channel blocks), the N = 128 tile for 128 and 256 (one and two)
-    const int dense_n = (Wp == NW || Wp == 192) ? NW : BN;
+    // output channels per tile of the dense convs and in-convs: the N = 128 tile for padded widths 128 and 256 (one and
+    // two channel blocks), the N = 64 tile for every other width (Wp / 64 channel blocks)
+    const int dense_n = (Wp == 128 || Wp == 256) ? BN : NW;
     TcState *ts = new TcState();
     m->tc_state = ts;
     const size_t act_elems = (size_t)m->d.max_batch * 256 * Wp;
@@ -738,6 +818,14 @@ int bsw_model_tc_prepare(bsw_model *m) {
     bsw_prefer_max_shared(k_conv_wg<TcArgs>); bsw_prefer_max_shared(k_conv_wg<HeadArgs>);
     bsw_prefer_max_shared(k_conv_wg<NarrowArgs>);
     bsw_prefer_max_shared(k_conv_wg<Tc128Args>); bsw_prefer_max_shared(k_conv_wg<Tc192Args>);
+    if (Wp > 256) {
+        BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<HeadWideArgs>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<HD_N>::SMEM));
+        bsw_prefer_max_shared(k_conv_wg<HeadWideArgs>);
+        const void *dense = Wp == 320 ? (const void *)k_conv_wg<TcWideArgs<320>> : Wp == 384 ? (const void *)k_conv_wg<TcWideArgs<384>>
+                          : Wp == 448 ? (const void *)k_conv_wg<TcWideArgs<448>> : (const void *)k_conv_wg<TcWideArgs<512>>;
+        BSW_CUDA(cudaFuncSetAttribute(dense, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<NW>::SMEM));
+        bsw_prefer_max_shared(dense);
+    }
     bsw_prefer_max_shared(k_given_to_planes);
     m->tc_ready = true;
     return BSW_OK;
@@ -775,7 +863,7 @@ int bsw_tc_split(bsw_model *m, const float *in, int which, int64_t n, cudaStream
 // 3x3, 7x7 with 5x5), 4 = in-convs and heads on a persistent grid (one CTA or cluster per SM / cluster slot walking the
 // tiles, the TMA ring prefetching across tile boundaries); a clear bit means one CTA per tile.  8 = the dense convs and
 // in-convs without TMA multicast: single CTAs, each loading its whole stage; it has no effect on a model of padded width
-// 64, 128 or 192, whose tiles always run as single CTAs.  Default 7
+// other than 256, whose tiles always run as single CTAs.  Default 7
 // (BSW_TC_PERSIST overrides).  Same tiles, same k order per tile: results are bit-identical in every mode.
 static int g_tc_mode = -1;
 static int tc_mode() {
@@ -839,7 +927,7 @@ static int launch_tc(const CUtensorMap &amap_hi, const CUtensorMap &amap_lo, con
     return BSW_OK;
 }
 
-// Dense convs and in-convs of a model of padded width 64, 128 or 192: single CTAs, one per tile or a persistent grid of
+// Dense convs and in-convs of a model of padded width other than 256: single CTAs, one per tile or a persistent grid of
 // one per SM.
 template <class Args>
 static int launch_tc_single(const CUtensorMap &amap_hi, const CUtensorMap &amap_lo, const TcSlot &s, const Args &t, int64_t n,
@@ -872,6 +960,10 @@ static int launch_dense(bsw_model *m, const CUtensorMap &amap_hi, const CUtensor
         case NW:  return launch_tc_single(amap_hi, amap_lo, s, tc_args<NarrowArgs>(ts, c, a, resid, cchunks), n, persistent, st);
         case 128: return launch_tc_single(amap_hi, amap_lo, s, tc_args<Tc128Args>(ts, c, a, resid, cchunks), n, persistent, st);
         case 192: return launch_tc_single(amap_hi, amap_lo, s, tc_args<Tc192Args>(ts, c, a, resid, cchunks), n, persistent, st);
+        case 320: return launch_tc_single(amap_hi, amap_lo, s, tc_args<TcWideArgs<320>>(ts, c, a, resid, cchunks), n, persistent, st);
+        case 384: return launch_tc_single(amap_hi, amap_lo, s, tc_args<TcWideArgs<384>>(ts, c, a, resid, cchunks), n, persistent, st);
+        case 448: return launch_tc_single(amap_hi, amap_lo, s, tc_args<TcWideArgs<448>>(ts, c, a, resid, cchunks), n, persistent, st);
+        case 512: return launch_tc_single(amap_hi, amap_lo, s, tc_args<TcWideArgs<512>>(ts, c, a, resid, cchunks), n, persistent, st);
         default:  return launch_tc(amap_hi, amap_lo, s, tc_args<TcArgs>(ts, c, a, resid, cchunks), n, persistent, st);
     }
 }
@@ -899,8 +991,13 @@ int bsw_conv_tc_head(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t
     h.taps = c.ks * c.ks; h.ks = c.ks; h.cchunks = m->Wp / BK; h.bias = c.bias; h.mu = a.mu; h.scale = a.scale; h.n_mu = a.n_mu; h.n_sc = a.n_sc;
     h.scale_kind = a.scale_kind; h.out_mode = a.out_mode; h.out_dim = a.out_dim;
     const int ntiles = (int)n * 2;
-    k_conv_wg<HeadArgs><<<tc_grid(ntiles, tc_persistent(4)), WG_THREADS, TileCfg<HD_N>::SMEM, st>>>(
-        ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1], s.map_hi, s.map_lo, h, ntiles);
+    const unsigned grid = tc_grid(ntiles, tc_persistent(4));
+    if (m->Wp > 256)
+        k_conv_wg<HeadWideArgs><<<grid, WG_THREADS, TileCfg<HD_N>::SMEM, st>>>(
+            ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1], s.map_hi, s.map_lo, HeadWideArgs{h}, ntiles);
+    else
+        k_conv_wg<HeadArgs><<<grid, WG_THREADS, TileCfg<HD_N>::SMEM, st>>>(
+            ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1], s.map_hi, s.map_lo, h, ntiles);
     BSW_LAUNCH_CHECK();
     return BSW_OK;
 }

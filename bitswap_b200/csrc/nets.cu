@@ -544,7 +544,7 @@ static int run_net(bsw_model *m, const NetPlan &np, const float *given, int64_t 
 // and net come from the model's plans; a head is named by its mu prefix.  Tensor-core dense convs and heads read plane
 // buffer 0, split from in_dev here by the same RNE split the epilogues use; dense convs write plane buffer 1, in-convs
 // plane buffer 0.  The written buffer is filled with 0xffff first and copied whole ([2][max_batch,256,Wp], Wp = 64, 128,
-// 192 or 256) to planes_dev, so rows the conv must not touch can be checked.
+// ..., 512) to planes_dev, so rows the conv must not touch can be checked.
 extern "C" int bsw_selftest_conv(bsw_model *m, const char *prefix, const float *in_dev, int64_t n, int flags, float *T_dev,
                                  float *A_dev, uint16_t *planes_dev, float *mu_dev, float *scale_dev, void *stream) {
     BSW_REQUIRE(m && prefix && in_dev, "bsw_selftest_conv: null argument");

@@ -208,7 +208,7 @@ int bsw_rows6_set_lanes_per_row(int lpr);
 /* Launch shape of the tensor-core convolutions, a bit mask: 1 / 2 / 4 = dense 3x3 / dense 5x5 / in-convs and heads on a
  * persistent grid (one CTA per SM, or one four-CTA cluster per four SMs, walking half-image tiles); a clear bit = one
  * CTA per tile.  8 = dense convs and in-convs as single CTAs without TMA multicast (by default each image's four tiles
- * run as one cluster sharing their operand loads); no effect on a model of padded width 64, 128 or 192, whose tiles
+ * run as one cluster sharing their operand loads); no effect on a model of padded width other than 256, whose tiles
  * always run as single CTAs.  Bits 1 / 2 split the dense convs by kernel size: <= 3 (1x1, 3x3) / >= 5 (5x5, 7x7).
  * -1 = default (BSW_TC_PERSIST if set, else 7).  Bit-identical results. */
 int bsw_set_conv_mode(int mode);
@@ -280,7 +280,7 @@ typedef struct {
     int32_t cond_xscale;   /* imagenetcrop: x-scale from a conv head */
     int32_t max_batch;     /* activations are preallocated for this many images */
     int32_t use_tensor_cores; /* 1: wgmma tensor-core path for the W->W convs (needs a padded width of 64, 128,
-                                 192 or 256, i.e. reswidth 1..256); 0: fp32 SIMT */
+                                 ..., 512, i.e. reswidth 1..512); 0: fp32 SIMT (any width) */
 } bsw_model_desc;
 
 int bsw_model_create(bsw_model **out, const bsw_model_desc *desc);
