@@ -16,20 +16,23 @@ from .model import Model
 from .streams import StreamSet
 
 BITSWAP, BBANS = 0, 1
+MIN_QUANTBITS = 5           # narrowest latent support of the device codec: 32 bins (every coder kernel owns S/32 bins per lane)
 MAX_QUANTBITS = 12          # widest latent support of the device codec: 4096 bins
 FUSED_MAX_SUPPORT = 1024    # the fused coder keeps a row table in one warp's registers
 
 
 def check_quantbits(q):
-    """ValueError unless 1 <= q <= MAX_QUANTBITS (raised before any device work)."""
-    if not (isinstance(q, (int, np.integer)) and 1 <= int(q) <= MAX_QUANTBITS):
-        raise ValueError(f"quantbits must be an integer in [1, {MAX_QUANTBITS}], got {q!r}")
+    """ValueError unless MIN_QUANTBITS <= q <= MAX_QUANTBITS (raised before any device work)."""
+    if not (isinstance(q, (int, np.integer)) and MIN_QUANTBITS <= int(q) <= MAX_QUANTBITS):
+        raise ValueError(f"quantbits must be an integer in [{MIN_QUANTBITS}, {MAX_QUANTBITS}], got {q!r}: the top latent level "
+                         f"is coded by kernels that own 2^quantbits / 32 bins per lane, so 32 bins is the narrowest support "
+                         f"the codec codes and 4096 the widest")
 
 
 class Bins:
     """Device copy of the discretisation tables (zendpoints [nz,zdim,2^q-1], zcentres [nz,zdim,2^q],
-    the layout discretize() returns, discretization.py:99).  quantbits 1 to 12: up to 4096 bins per latent dimension
-    (at 12, cifar8's bins take 1.07 GB of device memory)."""
+    the layout discretize() returns, discretization.py:99).  quantbits 5 to 12: 32 to 4096 bins per latent dimension
+    (at 12, cifar8's bins take 1.07 GB of device memory); any other quantbits raises ValueError here."""
 
     def __init__(self, cfg: CodecConfig, zendpoints, zcentres, device=None):
         check_quantbits(cfg.quantbits)

@@ -886,7 +886,14 @@ extern "C" int bsw_bins_create(bsw_bins **out, int nz, int zdim, int q, int xdim
                                const double *zcen_host) {
     // q <= 12: supports up to 4096 bins, coded by the two-phase kernels (the fused ones stop at 1024, see
     // bsw_codec_set_two_phase).  At q = 12 the eight 2048-dim levels of cifar8 hold 2 x 8 x 2048 x 4096 doubles: 1.07 GB.
-    BSW_REQUIRE(out && nz > 0 && zdim > 0 && q > 0 && q <= 12 && zend_host && zcen_host, "bsw_bins_create: bad arguments");
+    // q >= 5: the top level (equal-mass bins) takes the generic and fused kernels, which own S/32 bins per lane.
+    if (q < 5 || q > 12) {
+        bsw_set_error("bsw_bins_create: bad arguments: quantbits must be an integer in [5, 12], got %d: the top latent level "
+                      "is coded by kernels that own 2^quantbits / 32 bins per lane, so 32 bins is the narrowest support the "
+                      "codec codes and 4096 the widest", q);
+        return BSW_E_INVALID;
+    }
+    BSW_REQUIRE(out && nz > 0 && zdim > 0 && zend_host && zcen_host, "bsw_bins_create: bad arguments");
     bsw_bins *b = new bsw_bins();
     b->nz = nz; b->zdim = zdim; b->q = q; b->S = 1 << q; b->xdim = xdim;
     const int S = b->S;

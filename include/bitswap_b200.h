@@ -228,8 +228,9 @@ int bsw_logistic_pop_2p(bsw_streams *s, int first, int count, const float *mu_de
  * (utils/torch/rand.py:134-153); the library keeps its own padded copy (each endpoint row padded
  * with +1e300 to S entries so that cdf_{S-1} == 1 falls out of the same formula).
  * ---------------------------------------------------------------------------------------------- */
-/* zendpoints_host [nz, zdim, S-1], zcentres_host [nz, zdim, S] float64 (reference layout); quantbits in [1, 12]
- * (S = 2^quantbits).  Device memory: 16 * nz * zdim * S bytes (padded endpoints + centres), 1.07 GB for cifar8 at 12. */
+/* zendpoints_host [nz, zdim, S-1], zcentres_host [nz, zdim, S] float64 (reference layout); quantbits in [5, 12]
+ * (S = 2^quantbits = 32 ... 4096; BSW_E_INVALID otherwise, before any allocation: the top level's kernels own S/32 bins
+ * per lane).  Device memory: 16 * nz * zdim * S bytes (padded endpoints + centres), 1.07 GB for cifar8 at 12. */
 int bsw_bins_create(bsw_bins **out, int nz, int zdim, int quantbits, int xdim,
                     const double *zendpoints_host, const double *zcentres_host);
 int bsw_bins_destroy(bsw_bins *b);

@@ -606,7 +606,8 @@ def test_gpu_discretize_vs_oracle_nets_on_identical_noise():
         assert (zcen[zi] - c_ref).abs().max().item() <= d.max().item() + 1e-12
     print(f"discretize on identical noise: {100.0 * close / total:.2f} % of endpoints within 1e-3, worst {worst:.2e} of the range")
     assert close >= 0.99 * total and worst <= 4 * 2.0 ** -10
-    # the fit kernels alone, on the samples the GPU run stored: exact (same float16 extrema, same linspace arithmetic)
+    # the top level is rand.Bins on float32 zeros / ones, no sampling: exact.  (The sampling, extrema and fit kernels are
+    # pinned bit for bit on their own, through the C ABI, in test_supports_gpu.py.)
     ref_top, _ = synthetic.synthetic_bins(cfg, seed=0)
     assert torch.equal(zend[-1], ref_top[-1])
 

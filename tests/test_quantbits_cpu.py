@@ -1,6 +1,6 @@
 """quantbits 11 and 12 (2048 and 4096 bins per latent dimension) without a GPU: the oracle and the top-level bins against
 a known-answer test the reference's own classes produced at S = 4096 (tests/golden/make_golden_q12.py), and the
-argument checks that refuse quantbits 13 before any device work."""
+argument checks that refuse quantbits outside [5, 12] before any device work."""
 import ctypes
 import hashlib
 import json
@@ -12,7 +12,7 @@ import torch
 
 from oracle import oracle as O
 from bitswap_b200 import synthetic
-from bitswap_b200.codec import Bins as DeviceBins, check_quantbits, MAX_QUANTBITS
+from bitswap_b200.codec import Bins as DeviceBins, check_quantbits, MIN_QUANTBITS, MAX_QUANTBITS
 from bitswap_b200.config import preset, with_
 from bitswap_b200.rand import Bins
 
@@ -74,28 +74,39 @@ def test_top_level_bins_q12_match_reference():
     assert np.array_equal(b.endpoints().numpy(), g["top_end"]) and np.array_equal(b.centres().numpy(), g["top_cen"])
 
 
-@pytest.mark.parametrize("q", [0, 13, 16, 10.0])
+@pytest.mark.parametrize("q", [0, 1, 4, 13, 16, 10.0])
 def test_out_of_range_quantbits_are_refused_before_device_work(q):
-    with pytest.raises(ValueError):
+    """quantbits 1-4 (2-16 bins) are refused as 0 and 13 are: the top level's coder kernels own 2^q / 32 bins per lane."""
+    with pytest.raises(ValueError, match=r"\[5, 12\]"):
         check_quantbits(q)
     cfg = with_(preset("tiny"), quantbits=q)
-    with pytest.raises(ValueError):       # raised before any CUDA call: this runs on machines without a GPU
-        DeviceBins(cfg, np.zeros((2, 256, 1)), np.zeros((2, 256, 2)))
+    S = 1 << int(q) if int(q) <= 12 else 2
+    with pytest.raises(ValueError, match=r"\[5, 12\]"):   # raised before any CUDA call: this runs on machines without a GPU
+        DeviceBins(cfg, np.zeros((2, 256, S - 1)), np.zeros((2, 256, S)))
 
 
-def test_supported_quantbits_pass_the_check():
-    for q in range(1, MAX_QUANTBITS + 1):
+def test_quantbits_5_to_12_pass_the_check():
+    """Every quantbits the codec codes (32 to 4096 bins) passes; 1-4 are refused by the test above."""
+    assert (MIN_QUANTBITS, MAX_QUANTBITS) == (5, 12)
+    for q in range(MIN_QUANTBITS, MAX_QUANTBITS + 1):
         check_quantbits(q)
+        check_quantbits(np.int64(q))
     assert with_(preset("cifar8"), quantbits=12).zsupport == 4096
+    assert with_(preset("tiny"), quantbits=5).zsupport == 32
 
 
 def test_abi_bins_create_refuses_q13():
-    """bsw_bins_create validates its arguments before allocating anything, so the C ABI answers without a GPU."""
+    """bsw_bins_create validates its arguments before allocating anything, so the C ABI answers without a GPU: quantbits
+    outside [5, 12] (13, 0, and 1-4, whose 2-16 bins the top level's kernels cannot code) is BSW_E_INVALID, with the
+    supported range in the message."""
     from bitswap_b200 import _lib
     _lib.build()
     L = _lib.lib()
-    h = ctypes.c_void_p()
-    one = np.zeros(8, dtype=np.float64)
-    assert L.bsw_bins_create(ctypes.byref(h), 1, 1, 13, 1024, one.ctypes.data, one.ctypes.data) == 4
-    assert b"bad arguments" in L.bsw_last_error() and not h.value
-    assert L.bsw_bins_create(ctypes.byref(h), 1, 1, 0, 1024, one.ctypes.data, one.ctypes.data) == 4
+    for q in (13, 0, 1, 4):
+        h = ctypes.c_void_p()
+        S = 1 << q
+        ends = np.zeros(max(S - 1, 1), dtype=np.float64)
+        cens = np.zeros(S, dtype=np.float64)
+        assert L.bsw_bins_create(ctypes.byref(h), 1, 1, q, 1024, ends.ctypes.data, cens.ctypes.data) == 4, q
+        msg = L.bsw_last_error()
+        assert b"bad arguments" in msg and b"[5, 12]" in msg and not h.value, (q, msg)

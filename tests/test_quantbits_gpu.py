@@ -22,7 +22,7 @@ from bitswap_b200._lib import lib, check, cuda_stream_ptr, BswError   # noqa: E4
 from test_quantbits_cpu import KAT, kat_inputs                         # noqa: E402
 
 dev = "cuda"
-WIDE = [(2048, 11), (4096, 12)]
+WIDE = [(1 << q, q) for q in range(5, 13)]              # every support the codec codes: 32 ... 4096 bins
 
 
 def test_kat_q12_dropin_ans():
@@ -126,7 +126,8 @@ def _check_vs_oracle(res, tabs, states, sym, check_streams):
 @pytest.mark.parametrize("family", ["generic", "affine", "forced_affine"])
 def test_two_phase_wide_support_vs_oracle(S, q, family):
     """pop then push of one level through bsw_logistic_pop_2p / push_2p, against our exported pmfs -> oracle ANS.__init__ ->
-    oracle coder.  generic = k_rows_wide / k_pop_coarse_wide, affine = k_rows6 / k_pop6 on uniform grids, forced_affine =
+    oracle coder, at every power of two from 32 to 4096 bins.  generic = k_rows<S/32> / k_pop_coarse<S/32> (k_rows_wide /
+    k_pop_coarse_wide above 1024), affine = k_rows6 / k_pop6 on uniform grids, forced_affine =
     the affine kernels on the equal-mass top-level rows (every bin takes the exact path).  B = 64 streams, L = 99 rows (not
     a multiple of the 8 rows per warp); ordinary, needle-sharp, all-bins-live and off-grid rows."""
     B, L = 64, 99
@@ -209,9 +210,12 @@ def _oracle_with(cfg, m, sd, zend, zcen, cls=O.BitSwapOracle):
     return orc
 
 
-@pytest.mark.parametrize("q", [11, 12])
+@pytest.mark.parametrize("q", [5, 8, 9, 11, 12])
 @pytest.mark.parametrize("name,scheme", [("tiny", BITSWAP), ("tiny3", BITSWAP), ("tiny", BBANS), ("tiny3", BBANS)])
 def test_p4_wide_support_vs_oracle_with_injected_nets(name, scheme, q):
+    """The codec end to end at quantbits 5, 8, 9, 11 and 12 (q = 6, 7 and 10 are the presets' own): every stream equals the
+    oracle recursion driven with the same nets, and decoding restores images and states.  The prior pop on the shared
+    table (k_pop_full<S/32>, and the cdf-table pop at S = 32) runs only here and in the tests of test_supports_gpu.py."""
     B, nimg = 4, 2
     cfg, m, sd, zend, zcen, bins, codec = _setup(name, q, B)
     assert cfg.zsupport == 1 << q
