@@ -31,12 +31,12 @@
 //     bound by L2 -> SM bytes, not by their MMAs).  A stage is refilled only after all three CTAs writing into it
 //     released it.
 //     A model of padded width 64 (reswidth 1..64, the MNIST models) has one 64-channel block per pixel half: its dense
-//     convs and in-convs run the narrow tile (NarrowArgs) as single CTAs, one per tile.  Padded width 128 runs the
-//     N = 128 tile with one channel block (Tc128Args), padded width 192 the N = 64 tile with three (Tc192Args), both
-//     as single CTAs.  Padded widths 320, 384, 448 and 512 (reswidth 257..512) run the N = 64 tile with Wp / 64 channel
-//     blocks (TcWideArgs<Wp>), single CTAs too.  Their dense convs and heads (HeadWideArgs) fold the main accumulator
-//     into a float32 register accumulator after every tap: K reaches 49 x 512 there, and the tensor core's truncating
-//     accumulate would otherwise lose accuracy in proportion to K.
+//     convs and in-convs run the narrow tile (DenseArgs<64>) as single CTAs, one per tile.  Padded width 128 runs the
+//     N = 128 tile with one channel block (DenseArgs<128>), padded width 192 the N = 64 tile with three
+//     (DenseArgs<192>), both as single CTAs.  Padded widths 320, 384, 448 and 512 (reswidth 257..512) run the N = 64
+//     tile with Wp / 64 channel blocks (DenseArgs<Wp>), single CTAs too.  Their dense convs and heads (HeadArgs<true>)
+//     fold the main accumulator into a float32 register accumulator after every tap: K reaches 49 x 512 there, and the
+//     tensor core's truncating accumulate would otherwise lose accuracy in proportion to K.
 //   * the kernel size (1, 3, 5 or 7) is a run-time argument: taps = ks^2 k-blocks per input chunk, TMA's zero fill pads
 //     every shift; a 1x1 in-conv tile is a single k-block.
 //   * fixed k order, no split-K, no atomics: results are bit-identical for any batch size, position in the batch
@@ -249,68 +249,14 @@ __device__ __forceinline__ uint32_t pack_bf16x2(__nv_bfloat16 a, __nv_bfloat16 b
     return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
 }
 
-struct TcArgs {
-    static constexpr int kN = BN, kCoBlocks = 256 / BN;
-    int taps, ks;
-    int cchunks;             // 32-channel chunks per tap: 8 for the dense W->W convs, 1 for the in-convs
-    const float *bias;       // [256]
-    const float *resid;      // [n,256,256] fp32 or null
-    float *T;                // trunk out or null
-    int T_elu;
-    __nv_bfloat16 *A_hi, *A_lo;   // next conv's input planes or null
-    int A_elu;
-};
-
-// Dense W->W convs and in-convs of a model of padded width 64: one 64-channel block per pixel half (kCoBlocks = 1, so
-// single CTAs; tile t -> image t / 2, pixel half t & 1).  Trunk, residual, planes and bias are 64 channels wide.
-struct NarrowArgs {
-    static constexpr int kN = NW, kCoBlocks = 1;
-    int taps, ks;
-    int cchunks;             // 32-channel chunks per tap: 2 for the dense W->W convs, 1 for the in-convs
-    const float *bias;       // [64]
-    const float *resid;      // [n,256,64] fp32 or null
-    float *T;                // trunk out or null
-    int T_elu;
-    __nv_bfloat16 *A_hi, *A_lo;   // next conv's input planes [n,256,64] or null
-    int A_elu;
-};
-
-// Dense W->W convs and in-convs of a model of padded width 128 (reswidth 65..128): the N = 128 tile with one channel
-// block per pixel half, single CTAs (tile t -> image t / 2, pixel half t & 1).  Trunk, residual, planes and bias are 128
-// channels wide.
-struct Tc128Args {
-    static constexpr int kN = BN, kCoBlocks = 1;
-    int taps, ks;
-    int cchunks;             // 32-channel chunks per tap: 4 for the dense W->W convs, 1 for the in-convs
-    const float *bias;       // [128]
-    const float *resid;      // [n,256,128] fp32 or null
-    float *T;                // trunk out or null
-    int T_elu;
-    __nv_bfloat16 *A_hi, *A_lo;   // next conv's input planes [n,256,128] or null
-    int A_elu;
-};
-
-// Dense W->W convs and in-convs of a model of padded width 192 (reswidth 129..192): the N = 64 tile with three channel
-// blocks per pixel half, single CTAs (tile t -> image t / 6, channel block (t >> 1) % 3, pixel half t & 1).  Trunk,
-// residual, planes and bias are 192 channels wide.
-struct Tc192Args {
-    static constexpr int kN = NW, kCoBlocks = 3;
-    int taps, ks;
-    int cchunks;             // 32-channel chunks per tap: 6 for the dense W->W convs, 1 for the in-convs
-    const float *bias;       // [192]
-    const float *resid;      // [n,256,192] fp32 or null
-    float *T;                // trunk out or null
-    int T_elu;
-    __nv_bfloat16 *A_hi, *A_lo;   // next conv's input planes [n,256,192] or null
-    int A_elu;
-};
-
-// Dense W->W convs and in-convs of a model of padded width WP = 320, 384, 448 or 512 (reswidth 257..512): the N = 64
-// tile with WP / 64 channel blocks per pixel half, single CTAs (tile t -> image t / (2 WP / 64), channel block
-// (t >> 1) % (WP / 64), pixel half t & 1).  Trunk, residual, planes and bias are WP channels wide.  The dense convs fold
-// the main accumulator once per tap (see k_conv_wg), so it never sums more than WP terms.
-template <int WP> struct TcWideArgs {
-    static constexpr int kN = NW, kCoBlocks = WP / NW;
+// Dense W->W convs and in-convs of a model of padded width WP = 64, 128, ..., 512 (reswidth 1..512): the N = kN tile
+// with kCoBlocks channel blocks per pixel half (tile t -> image t / (2 kCoBlocks), channel block (t >> 1) % kCoBlocks,
+// pixel half t & 1).  Padded widths 128 and 256 take the N = 128 tile, every other width the N = 64 tile.  Trunk,
+// residual, planes and bias are WP channels wide.  Above 256 the dense convs fold the main accumulator once per tap (see
+// k_conv_wg), so it never sums more than WP terms; widths <= 256 do not fold.
+template <int WP> struct DenseArgs {
+    static constexpr int kN = (WP == 128 || WP == 256) ? BN : NW, kCoBlocks = WP / kN;
+    static constexpr bool kFold = WP > 256;
     int taps, ks;
     int cchunks;             // 32-channel chunks per tap: WP / 32 for the dense W->W convs, 1 for the in-convs
     const float *bias;       // [WP]
@@ -321,75 +267,49 @@ template <int WP> struct TcWideArgs {
     int A_elu;
 };
 
-// Tiles whose consumers fold the main accumulator into a float32 register accumulator after every tap of more than one
-// k-block: the wide dense convs and the wide heads.  Widths <= 256 do not fold (their results stay as they were).
-template <class Args> struct Folds { static constexpr bool value = false; };
-template <int WP> struct Folds<TcWideArgs<WP>> { static constexpr bool value = true; };
-
-// Hand-off tile of the dense convs and in-convs: s = main + cross as fp32 [128 px][N ch] (N = 128, or 64 for NarrowArgs),
-// the 32-byte column chunks of row r XOR-swizzled by r & 3.  A row is a whole number of 128-byte bank lines, so without
+// Hand-off tile of the dense convs and in-convs: s = main + cross as fp32 [128 px][N ch] (N = kN, 128 or 64), the
+// 32-byte column chunks of row r XOR-swizzled by r & 3.  A row is a whole number of 128-byte bank lines, so without
 // the swizzle chunk j of rows r..r+3 would sit on the same 8 banks.  The consumers' float2 writes (a half warp covers
 // chunk j of 4 consecutive rows) go to chunks j ^ 0..3, and the epilogue's float4 reads (a quarter warp covers 4
 // consecutive chunks of one row) to 4 chunks; either way the low two chunk bits differ -> 32 distinct banks.
 template <int N> __device__ __forceinline__ int hand_idx(int r, int c) { return r * N + (((c >> 3) ^ (r & 3)) << 3) + (c & 7); }
 
-template <int N>
-__device__ __forceinline__ void dense_hand_store(float *hand, const float (&dm)[N / 2], const float (&dc)[N / 2], int row, int lane) {
+// Folding tiles: s = (outer + main) + cross, in that order for every element, so the result does not depend on the grid.
+// The other tiles pass a one-element `outer` that is never read.
+template <int WP, int O>
+__device__ __forceinline__ void hand_store(const DenseArgs<WP> &, float *hand, const float (&outer)[O],
+                                           const float (&dm)[DenseArgs<WP>::kN / 2], const float (&dc)[DenseArgs<WP>::kN / 2],
+                                           int row, int lane) {
+    constexpr int N = DenseArgs<WP>::kN;
 #pragma unroll
     for (int j = 0; j < N / 8; ++j)
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int i = 4 * j + 2 * h;
-            *reinterpret_cast<float2 *>(hand + hand_idx<N>(row + 8 * h, 8 * j + 2 * (lane & 3))) =
-                make_float2(dm[i] + dc[i], dm[i + 1] + dc[i + 1]);
-        }
-}
-__device__ __forceinline__ void hand_store(const TcArgs &, float *hand, const float (&dm)[64], const float (&dc)[64], int row,
-                                           int lane) {
-    dense_hand_store<BN>(hand, dm, dc, row, lane);
-}
-__device__ __forceinline__ void hand_store(const NarrowArgs &, float *hand, const float (&dm)[32], const float (&dc)[32], int row,
-                                           int lane) {
-    dense_hand_store<NW>(hand, dm, dc, row, lane);
-}
-__device__ __forceinline__ void hand_store(const Tc128Args &, float *hand, const float (&dm)[64], const float (&dc)[64], int row,
-                                           int lane) {
-    dense_hand_store<BN>(hand, dm, dc, row, lane);
-}
-__device__ __forceinline__ void hand_store(const Tc192Args &, float *hand, const float (&dm)[32], const float (&dc)[32], int row,
-                                           int lane) {
-    dense_hand_store<NW>(hand, dm, dc, row, lane);
-}
-// Folding tiles: s = (outer + main) + cross, in that order for every element, so the result does not depend on the grid.
-template <int WP>
-__device__ __forceinline__ void hand_store(const TcWideArgs<WP> &, float *hand, const float (&outer)[32], const float (&dm)[32],
-                                           const float (&dc)[32], int row, int lane) {
-#pragma unroll
-    for (int j = 0; j < NW / 8; ++j)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int i = 4 * j + 2 * h;
-            *reinterpret_cast<float2 *>(hand + hand_idx<NW>(row + 8 * h, 8 * j + 2 * (lane & 3))) =
-                make_float2((outer[i] + dm[i]) + dc[i], (outer[i + 1] + dm[i + 1]) + dc[i + 1]);
+            float2 s;
+            if constexpr (DenseArgs<WP>::kFold) s = make_float2((outer[i] + dm[i]) + dc[i], (outer[i + 1] + dm[i + 1]) + dc[i + 1]);
+            else s = make_float2(dm[i] + dc[i], dm[i + 1] + dc[i + 1]);
+            *reinterpret_cast<float2 *>(hand + hand_idx<N>(row + 8 * h, 8 * j + 2 * (lane & 3))) = s;
         }
 }
 
 // Dense / in-conv epilogue, run by the epilogue warps from the hand-off tile: s + bias (+ residual) (-> ELU) -> trunk;
-// (-> ELU) -> bf16 hi/lo planes of the next conv.  Tensors are NHWC with LD channels per pixel and the hand-off tile has
-// N channels per row; ROWS tile rows are stored per warp step, 32 / ROWS lanes per row, 4 channels per lane (TcArgs:
-// one 128-channel half row per step; NarrowArgs: two 64-channel rows).  Warp ew takes row steps ew, ew + 3, ..., so a
-// warp stores 512 contiguous bytes of the trunk and 256 of each plane per step.  The residual is the trunk itself
-// (updated in place: resid == T): each element is read and then written by the same thread, and the loads of the next
-// RD steps are issued before the current step's stores.
-template <int LD, int N, int ROWS, class Args>
-__device__ __forceinline__ void dense_epilogue(const Args &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
+// (-> ELU) -> bf16 hi/lo planes of the next conv.  Tensors are NHWC with WP channels per pixel and the hand-off tile has
+// N channels per row; ROWS = 128 / N tile rows are stored per warp step, 32 / ROWS lanes per row, 4 channels per lane
+// (N = 128: 128 channels of one row per step; N = 64: two 64-channel rows), at channel block co0.  Warp ew takes row
+// steps ew, ew + 3, ..., so a warp stores 512 contiguous bytes of the trunk and 256 of each plane per step.  The
+// residual is the trunk itself (updated in place: resid == T): each element is read and then written by the same
+// thread, and the loads of the next RD steps are issued before the current step's stores.
+template <int WP>
+__device__ __forceinline__ void epilogue(const DenseArgs<WP> &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
+    constexpr int N = DenseArgs<WP>::kN, ROWS = 128 / N;
     constexpr int RD = 3, LPR = 32 / ROWS;
     const int hl = lane % LPR, sub = lane / LPR;
     const float4 bq = __ldg(reinterpret_cast<const float4 *>(a.bias + co0) + hl);
-    const int64_t base = ((int64_t)img * 256 + mh * 128 + sub) * LD + co0 + 4 * hl;     // + ROWS * step * LD
+    const int64_t base = ((int64_t)img * 256 + mh * 128 + sub) * WP + co0 + 4 * hl;     // + ROWS * step * WP
     const int nr = (MT / ROWS - ew + EPI_WARPS - 1) / EPI_WARPS;
     auto resid = [&](int k) {
-        return (a.resid && k < nr) ? *reinterpret_cast<const float4 *>(a.resid + base + ROWS * (ew + EPI_WARPS * k) * LD)
+        return (a.resid && k < nr) ? *reinterpret_cast<const float4 *>(a.resid + base + ROWS * (ew + EPI_WARPS * k) * WP)
                                    : make_float4(0.f, 0.f, 0.f, 0.f);
     };
     float4 q[RD];
@@ -408,7 +328,7 @@ __device__ __forceinline__ void dense_epilogue(const Args &a, const float *hand,
             if (a.T_elu)
 #pragma unroll
                 for (int e = 0; e < 4; ++e) x[e] = elu1(x[e]);
-            const int64_t off = base + ROWS * rs * LD;
+            const int64_t off = base + ROWS * rs * WP;
             if (a.T) *reinterpret_cast<float4 *>(a.T + off) = make_float4(x[0], x[1], x[2], x[3]);
             if (a.A_hi) {
                 __nv_bfloat16 hi[4], lo[4];
@@ -424,33 +344,15 @@ __device__ __forceinline__ void dense_epilogue(const Args &a, const float *hand,
         }
     }
 }
-__device__ __forceinline__ void epilogue(const TcArgs &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
-    dense_epilogue<256, BN, 1>(a, hand, img, mh, co0, ew, lane);
-}
-
-__device__ __forceinline__ void epilogue(const NarrowArgs &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
-    dense_epilogue<NW, NW, 2>(a, hand, img, mh, co0, ew, lane);
-}
-
-// Padded widths 128 and 192: the trunk and planes are the model's Wp channels wide; each row step of the N = 64 tile
-// stores 64 of a pixel's 192 channels, at channel block co0.
-__device__ __forceinline__ void epilogue(const Tc128Args &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
-    dense_epilogue<128, BN, 1>(a, hand, img, mh, co0, ew, lane);
-}
-__device__ __forceinline__ void epilogue(const Tc192Args &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
-    dense_epilogue<192, NW, 2>(a, hand, img, mh, co0, ew, lane);
-}
-template <int WP>
-__device__ __forceinline__ void epilogue(const TcWideArgs<WP> &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
-    dense_epilogue<WP, NW, 2>(a, hand, img, mh, co0, ew, lane);
-}
 
 // mu/sigma heads: the 3x3 W -> (n_mu + n_sc <= 32) convolution that ends every net (cifar_train.py:349,368,411,426),
-// with the scale transforms and the UnSqueeze2d index map of the x head in the epilogue.
-struct HeadArgs {
+// with the scale transforms and the UnSqueeze2d index map of the x head in the epilogue.  FOLD: the heads of a model of
+// padded width 320..512, where K = taps x Wp (up to 49 x 512), fold once per tap like the dense convs of that width.
+template <bool FOLD> struct HeadArgs {
     static constexpr int kN = HD_N, kCoBlocks = 1;
+    static constexpr bool kFold = FOLD;
     int taps, ks;
-    int cchunks;             // 8: K = taps x 256
+    int cchunks;             // Wp / 32: K = taps x Wp
     const float *bias;       // [>= n_mu + n_sc]
     float *mu, *scale;
     int n_mu, n_sc, scale_kind, out_mode, out_dim;
@@ -468,9 +370,11 @@ __device__ __forceinline__ float hd_scale(float r, int kind) {      // same expr
 }
 
 // Heads' hand-off tile: channel-major [32 ch][HD_LD], so the epilogue's lanes read consecutive pixels of one channel; the
-// row stride of 132 floats also spreads the consumers' writes (8 rows x 4 channels per register) over 32 banks.
-__device__ __forceinline__ void hand_store(const HeadArgs &, float *hand, const float (&dm)[16], const float (&dc)[16], int row,
-                                           int lane) {
+// row stride of 132 floats also spreads the consumers' writes (8 rows x 4 channels per register) over 32 banks.  The sum
+// is the dense tiles': (outer + main) + cross when folding, main + cross otherwise.
+template <bool FOLD, int O>
+__device__ __forceinline__ void hand_store(const HeadArgs<FOLD> &, float *hand, const float (&outer)[O], const float (&dm)[HD_N / 2],
+                                           const float (&dc)[HD_N / 2], int row, int lane) {
 #pragma unroll
     for (int j = 0; j < HD_N / 8; ++j)
 #pragma unroll
@@ -478,30 +382,16 @@ __device__ __forceinline__ void hand_store(const HeadArgs &, float *hand, const 
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
                 const int i = 4 * j + 2 * h + e;
-                hand[(8 * j + 2 * (lane & 3) + e) * HD_LD + row + 8 * h] = dm[i] + dc[i];
-            }
-}
-
-// Heads of a model of padded width 320..512: K = taps x Wp (up to 49 x 512), so they fold once per tap like the wide
-// dense convs.  Same fields and epilogue as HeadArgs; a type of its own keeps k_conv_wg<HeadArgs> as it is.
-struct HeadWideArgs : HeadArgs {};
-template <> struct Folds<HeadWideArgs> { static constexpr bool value = true; };
-
-__device__ __forceinline__ void hand_store(const HeadWideArgs &, float *hand, const float (&outer)[16], const float (&dm)[16],
-                                           const float (&dc)[16], int row, int lane) {
-#pragma unroll
-    for (int j = 0; j < HD_N / 8; ++j)
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                const int i = 4 * j + 2 * h + e;
-                hand[(8 * j + 2 * (lane & 3) + e) * HD_LD + row + 8 * h] = (outer[i] + dm[i]) + dc[i];
+                float s;
+                if constexpr (FOLD) s = (outer[i] + dm[i]) + dc[i];
+                else s = dm[i] + dc[i];
+                hand[(8 * j + 2 * (lane & 3) + e) * HD_LD + row + 8 * h] = s;
             }
 }
 
 // Heads' epilogue: lane = pixel, so the flat CHW stores dst[o * 256 + p] of a warp are coalesced.
-__device__ __forceinline__ void epilogue(const HeadArgs &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
+template <bool FOLD>
+__device__ __forceinline__ void epilogue(const HeadArgs<FOLD> &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
     float *mu_row = a.mu + (int64_t)img * a.out_dim;
     float *sc_row = a.scale ? a.scale + (int64_t)img * a.out_dim : nullptr;
     for (int r = ew * 32 + lane; r < MT; r += EPI_WARPS * 32) {
@@ -520,8 +410,8 @@ __device__ __forceinline__ void epilogue(const HeadArgs &a, const float *hand, i
 
 // Tile t -> image t / (2 * kCoBlocks), output-channel block, pixel half (t & 1): the tiles of one image run on
 // neighbouring SMs at about the same time, so the activation planes they share come out of L2.
-// Launched as four-CTA clusters (TcArgs only, see the file comment), gridDim.x is a multiple of 4: t & 3 is the CTA's
-// cluster rank and the four CTAs of a cluster walk the same images in step.
+// Launched as four-CTA clusters (DenseArgs<256> only, see the file comment), gridDim.x is a multiple of 4: t & 3 is the
+// CTA's cluster rank and the four CTAs of a cluster walk the same images in step.
 // Each tile's accumulators go through the shared-memory hand-off tile to the epilogue warps, so the consumers start the
 // next tile's MMAs while its epilogue runs: acc_full (256 consumer threads arrive) publishes the tile, acc_empty (96
 // epilogue threads arrive after their last read of it) frees it.
@@ -616,10 +506,10 @@ k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ C
         if (mc) { mbar_arrive_cluster(&empty_bar[s], rank); mbar_arrive_cluster(&empty_bar[s], rank ^ 1); mbar_arrive_cluster(&empty_bar[s], rank ^ 2); }
         else mbar_arrive(&empty_bar[s]);
     };
-    // Folding tiles (Folds<Args>): after the last k-block of every tap but the last, the consumers retire the MMAs in
+    // Folding tiles (Args::kFold): after the last k-block of every tap but the last, the consumers retire the MMAs in
     // flight, add the main accumulator into `outer` (float32 RNE adds) and restart it from zero, so the tensor core's
     // truncating accumulate never sums more than one tap's Wp terms into it.  In-convs (one k-block per tap) do not fold.
-    constexpr bool fold = Folds<Args>::value;
+    constexpr bool fold = Args::kFold;
     const bool fold_taps = fold && a.cchunks > 1;
     int stage = 0, phase = 0, it = 0;
     for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++it) {
@@ -667,8 +557,7 @@ k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ C
         fence_regs(dc);
         if (prev >= 0) release(prev);
         mbar_wait(acc_empty, (it & 1) ^ 1);            // the epilogue has read the previous tile
-        if constexpr (fold) hand_store(a, hand, outer, dm, dc, row0, lane);
-        else hand_store(a, hand, dm, dc, row0, lane);
+        hand_store(a, hand, outer, dm, dc, row0, lane);
         mbar_arrive(acc_full);
     }
 }
@@ -734,17 +623,42 @@ int encode_map(CUtensorMap *m, void *base, int rank, const cuuint64_t *dims, con
     return BSW_OK;
 }
 
+// Calls f(DenseArgs<Wp>{}) for the run-time padded width Wp: the one list of the widths the tensor-core convs run.
+template <class F> int with_width(int Wp, F &&f) {
+    switch (Wp) {
+        case 64:  return f(DenseArgs<64>{});
+        case 128: return f(DenseArgs<128>{});
+        case 192: return f(DenseArgs<192>{});
+        case 256: return f(DenseArgs<256>{});
+        case 320: return f(DenseArgs<320>{});
+        case 384: return f(DenseArgs<384>{});
+        case 448: return f(DenseArgs<448>{});
+        case 512: return f(DenseArgs<512>{});
+    }
+    BSW_REQUIRE(false, "tensor-core conv path needs a padded width of 64, 128, ..., 512 (reswidth 1..512)");
+}
+
 }  // namespace
 
 struct TcSlot { CUtensorMap map_hi, map_lo; };
 
 int bsw_model_tc_prepare(bsw_model *m) {
-    BSW_REQUIRE(m->Wp % 64 == 0 && m->Wp <= 512,
-                "tensor-core conv path needs a padded width of 64, 128, ..., 512 (reswidth 1..512)");
     const int Wp = m->Wp;
-    // output channels per tile of the dense convs and in-convs: the N = 128 tile for padded widths 128 and 256 (one and
-    // two channel blocks), the N = 64 tile for every other width (Wp / 64 channel blocks)
-    const int dense_n = (Wp == 128 || Wp == 256) ? BN : NW;
+    // The dense / in-conv and head kernels of the model's width, with one SM-wide L1/shared split for every kernel of
+    // the path (see bsw_prefer_max_shared).  dense_n: output channels per tile of the dense convs and in-convs.
+    int dense_n = 0;
+    if (int rc = with_width(Wp, [&](auto t) {
+            using Args = decltype(t);
+            using Head = HeadArgs<Args::kFold>;
+            dense_n = Args::kN;
+            BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<Args>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<Args::kN>::SMEM));
+            BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<Head>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<HD_N>::SMEM));
+            bsw_prefer_max_shared(k_conv_wg<Args>);
+            bsw_prefer_max_shared(k_conv_wg<Head>);
+            return BSW_OK;
+        }))
+        return rc;
+    bsw_prefer_max_shared(k_given_to_planes);
     TcState *ts = new TcState();
     m->tc_state = ts;
     const size_t act_elems = (size_t)m->d.max_batch * 256 * Wp;
@@ -809,24 +723,6 @@ int bsw_model_tc_prepare(bsw_model *m) {
         slots->push_back(s);
     }
     m->tc_slots = slots;
-    BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<TcArgs>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<BN>::SMEM));
-    BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<HeadArgs>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<HD_N>::SMEM));
-    BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<NarrowArgs>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<NW>::SMEM));
-    BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<Tc128Args>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<BN>::SMEM));
-    BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<Tc192Args>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<NW>::SMEM));
-    // one SM-wide L1/shared split for every kernel of the path (see bsw_prefer_max_shared)
-    bsw_prefer_max_shared(k_conv_wg<TcArgs>); bsw_prefer_max_shared(k_conv_wg<HeadArgs>);
-    bsw_prefer_max_shared(k_conv_wg<NarrowArgs>);
-    bsw_prefer_max_shared(k_conv_wg<Tc128Args>); bsw_prefer_max_shared(k_conv_wg<Tc192Args>);
-    if (Wp > 256) {
-        BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<HeadWideArgs>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<HD_N>::SMEM));
-        bsw_prefer_max_shared(k_conv_wg<HeadWideArgs>);
-        const void *dense = Wp == 320 ? (const void *)k_conv_wg<TcWideArgs<320>> : Wp == 384 ? (const void *)k_conv_wg<TcWideArgs<384>>
-                          : Wp == 448 ? (const void *)k_conv_wg<TcWideArgs<448>> : (const void *)k_conv_wg<TcWideArgs<512>>;
-        BSW_CUDA(cudaFuncSetAttribute(dense, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<NW>::SMEM));
-        bsw_prefer_max_shared(dense);
-    }
-    bsw_prefer_max_shared(k_given_to_planes);
     m->tc_ready = true;
     return BSW_OK;
 }
@@ -894,78 +790,55 @@ static unsigned tc_grid(int ntiles, bool persistent) {   // one CTA per tile, or
     return (unsigned)(ntiles < sms[dev] ? ntiles : sms[dev]);
 }
 
-// Dense convs and in-convs: one four-CTA cluster per image (TMA multicast, see k_conv_wg), or single CTAs with mode bit 8.
-// The persistent grid is as many clusters as the device holds at once (GPCs of 16-18 SMs leave some SMs out), cluster c
-// walking images c, c + C, ...
-static int launch_tc(const CUtensorMap &amap_hi, const CUtensorMap &amap_lo, const TcSlot &s, const TcArgs &t, int64_t n,
-                     bool persistent, cudaStream_t st) {
-    static int clusters[64] = {0};
-    const int ntiles = (int)n * 2 * TcArgs::kCoBlocks;
-    const bool mc = (tc_mode() & 8) == 0;
-    cudaLaunchAttribute attr;
-    attr.id = cudaLaunchAttributeClusterDimension;
-    attr.val.clusterDim.x = 4; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)ntiles);
-    cfg.blockDim = dim3(WG_THREADS);
-    cfg.dynamicSmemBytes = TileCfg<BN>::SMEM;
-    cfg.stream = st;
-    cfg.attrs = &attr;
-    cfg.numAttrs = mc ? 1 : 0;
-    if (persistent && !mc) cfg.gridDim = dim3(tc_grid(ntiles, true));
-    if (persistent && mc) {
-        const int dev = cur_device();
-        if (!clusters[dev]) {
-            int v = 0;
-            BSW_CUDA(cudaOccupancyMaxActiveClusters(&v, k_conv_wg<TcArgs>, &cfg));
-            BSW_REQUIRE(v > 0, "launch_tc: a cluster of four conv CTAs does not fit this device");
-            clusters[dev] = v;
-        }
-        cfg.gridDim = dim3(4u * (unsigned)(n < clusters[dev] ? n : clusters[dev]));
-    }
-    BSW_CUDA(cudaLaunchKernelEx(&cfg, k_conv_wg<TcArgs>, amap_hi, amap_lo, s.map_hi, s.map_lo, t, ntiles));
-    return BSW_OK;
-}
-
-// Dense convs and in-convs of a model of padded width other than 256: single CTAs, one per tile or a persistent grid of
-// one per SM.
-template <class Args>
-static int launch_tc_single(const CUtensorMap &amap_hi, const CUtensorMap &amap_lo, const TcSlot &s, const Args &t, int64_t n,
-                            bool persistent, cudaStream_t st) {
-    const int ntiles = (int)n * 2 * Args::kCoBlocks;
-    k_conv_wg<Args><<<tc_grid(ntiles, persistent), WG_THREADS, TileCfg<Args::kN>::SMEM, st>>>(amap_hi, amap_lo, s.map_hi,
-                                                                                              s.map_lo, t, ntiles);
-    BSW_LAUNCH_CHECK();
-    return BSW_OK;
-}
-
-// Fills the fields the dense Args types share; cchunks = 32-channel chunks per tap of the input planes.
-template <class Args>
-static Args tc_args(TcState *ts, const ConvSlot &c, const ConvArgs &a, const float *resid, int cchunks) {
-    Args t;
-    t.taps = c.ks * c.ks; t.ks = c.ks; t.cchunks = cchunks;
-    t.bias = c.bias; t.resid = resid; t.T = a.T; t.T_elu = a.T_elu;
-    t.A_hi = a.A_planes >= 0 ? ts->act[a.A_planes][0] : nullptr;
-    t.A_lo = a.A_planes >= 0 ? ts->act[a.A_planes][1] : nullptr;
-    t.A_elu = a.A_elu;
-    return t;
-}
-
-// One dense conv or in-conv on the tile of the model's padded width, reading the planes behind amap_hi / amap_lo.
+// One dense conv or in-conv on the tile of the model's padded width, reading the planes behind amap_hi / amap_lo;
+// cchunks = 32-channel chunks per tap of those planes.  The tile with two channel blocks (padded width 256) runs one
+// four-CTA cluster per image (TMA multicast, see k_conv_wg), or single CTAs with mode bit 8; its persistent grid is as
+// many clusters as the device holds at once (GPCs of 16-18 SMs leave some SMs out), cluster c walking images c, c + C,
+// ...  Every other tile runs single CTAs, one per tile or a persistent grid of one per SM.
 static int launch_dense(bsw_model *m, const CUtensorMap &amap_hi, const CUtensorMap &amap_lo, const TcSlot &s,
                         const ConvSlot &c, const ConvArgs &a, const float *resid, int cchunks, int64_t n, bool persistent,
                         cudaStream_t st) {
     TcState *ts = (TcState *)m->tc_state;
-    switch (m->Wp) {
-        case NW:  return launch_tc_single(amap_hi, amap_lo, s, tc_args<NarrowArgs>(ts, c, a, resid, cchunks), n, persistent, st);
-        case 128: return launch_tc_single(amap_hi, amap_lo, s, tc_args<Tc128Args>(ts, c, a, resid, cchunks), n, persistent, st);
-        case 192: return launch_tc_single(amap_hi, amap_lo, s, tc_args<Tc192Args>(ts, c, a, resid, cchunks), n, persistent, st);
-        case 320: return launch_tc_single(amap_hi, amap_lo, s, tc_args<TcWideArgs<320>>(ts, c, a, resid, cchunks), n, persistent, st);
-        case 384: return launch_tc_single(amap_hi, amap_lo, s, tc_args<TcWideArgs<384>>(ts, c, a, resid, cchunks), n, persistent, st);
-        case 448: return launch_tc_single(amap_hi, amap_lo, s, tc_args<TcWideArgs<448>>(ts, c, a, resid, cchunks), n, persistent, st);
-        case 512: return launch_tc_single(amap_hi, amap_lo, s, tc_args<TcWideArgs<512>>(ts, c, a, resid, cchunks), n, persistent, st);
-        default:  return launch_tc(amap_hi, amap_lo, s, tc_args<TcArgs>(ts, c, a, resid, cchunks), n, persistent, st);
-    }
+    return with_width(m->Wp, [&](auto t) {
+        using Args = decltype(t);
+        t.taps = c.ks * c.ks; t.ks = c.ks; t.cchunks = cchunks;
+        t.bias = c.bias; t.resid = resid; t.T = a.T; t.T_elu = a.T_elu;
+        t.A_hi = a.A_planes >= 0 ? ts->act[a.A_planes][0] : nullptr;
+        t.A_lo = a.A_planes >= 0 ? ts->act[a.A_planes][1] : nullptr;
+        t.A_elu = a.A_elu;
+        const int ntiles = (int)n * 2 * Args::kCoBlocks;
+        if constexpr (Args::kCoBlocks == 2) {
+            static int clusters[64] = {0};
+            const bool mc = (tc_mode() & 8) == 0;
+            cudaLaunchAttribute attr;
+            attr.id = cudaLaunchAttributeClusterDimension;
+            attr.val.clusterDim.x = 4; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+            cudaLaunchConfig_t cfg = {};
+            cfg.gridDim = dim3((unsigned)ntiles);
+            cfg.blockDim = dim3(WG_THREADS);
+            cfg.dynamicSmemBytes = TileCfg<Args::kN>::SMEM;
+            cfg.stream = st;
+            cfg.attrs = &attr;
+            cfg.numAttrs = mc ? 1 : 0;
+            if (persistent && !mc) cfg.gridDim = dim3(tc_grid(ntiles, true));
+            if (persistent && mc) {
+                const int dev = cur_device();
+                if (!clusters[dev]) {
+                    int v = 0;
+                    BSW_CUDA(cudaOccupancyMaxActiveClusters(&v, k_conv_wg<Args>, &cfg));
+                    BSW_REQUIRE(v > 0, "launch_dense: a cluster of four conv CTAs does not fit this device");
+                    clusters[dev] = v;
+                }
+                cfg.gridDim = dim3(4u * (unsigned)(n < clusters[dev] ? n : clusters[dev]));
+            }
+            BSW_CUDA(cudaLaunchKernelEx(&cfg, k_conv_wg<Args>, amap_hi, amap_lo, s.map_hi, s.map_lo, t, ntiles));
+        } else {
+            k_conv_wg<Args><<<tc_grid(ntiles, persistent), WG_THREADS, TileCfg<Args::kN>::SMEM, st>>>(amap_hi, amap_lo, s.map_hi,
+                                                                                                      s.map_lo, t, ntiles);
+            BSW_LAUNCH_CHECK();
+        }
+        return BSW_OK;
+    });
 }
 
 // a.in must be one of the plane buffers: a.in_planes = 0/1 selects it; outputs a.A_planes = 0/1/-1.
@@ -987,19 +860,18 @@ int bsw_conv_tc_head(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t
     TcState *ts = (TcState *)m->tc_state;
     BSW_REQUIRE(ts && c.tc_index >= 0 && a.n_mu + a.n_sc <= HD_N, "bsw_conv_tc_head: conv has no tensor-core head weights");
     const TcSlot &s = (*(std::vector<TcSlot> *)m->tc_slots)[c.tc_index];
-    HeadArgs h;
-    h.taps = c.ks * c.ks; h.ks = c.ks; h.cchunks = m->Wp / BK; h.bias = c.bias; h.mu = a.mu; h.scale = a.scale; h.n_mu = a.n_mu; h.n_sc = a.n_sc;
-    h.scale_kind = a.scale_kind; h.out_mode = a.out_mode; h.out_dim = a.out_dim;
     const int ntiles = (int)n * 2;
     const unsigned grid = tc_grid(ntiles, tc_persistent(4));
-    if (m->Wp > 256)
-        k_conv_wg<HeadWideArgs><<<grid, WG_THREADS, TileCfg<HD_N>::SMEM, st>>>(
-            ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1], s.map_hi, s.map_lo, HeadWideArgs{h}, ntiles);
-    else
-        k_conv_wg<HeadArgs><<<grid, WG_THREADS, TileCfg<HD_N>::SMEM, st>>>(
-            ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1], s.map_hi, s.map_lo, h, ntiles);
-    BSW_LAUNCH_CHECK();
-    return BSW_OK;
+    return with_width(m->Wp, [&](auto t) {
+        using Head = HeadArgs<decltype(t)::kFold>;      // the heads fold where the model's dense convs do
+        Head h;
+        h.taps = c.ks * c.ks; h.ks = c.ks; h.cchunks = m->Wp / BK; h.bias = c.bias; h.mu = a.mu; h.scale = a.scale; h.n_mu = a.n_mu; h.n_sc = a.n_sc;
+        h.scale_kind = a.scale_kind; h.out_mode = a.out_mode; h.out_dim = a.out_dim;
+        k_conv_wg<Head><<<grid, WG_THREADS, TileCfg<HD_N>::SMEM, st>>>(ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1],
+                                                                        s.map_hi, s.map_lo, h, ntiles);
+        BSW_LAUNCH_CHECK();
+        return BSW_OK;
+    });
 }
 
 // In-conv on the tensor cores: `given` (flat CHW float32) -> 32-channel bf16 planes -> k_conv_wg with one channel chunk

@@ -1,7 +1,8 @@
-"""CPU-only checks for models of any kernel size (1, 3, 5, 7) and padded width (64, 128, 192, 256):
+"""CPU-only checks for models of any kernel size (1, 3, 5, 7) and padded width (64, 128, ..., 512):
 
-1. the new conv instantiations in the built library (cuobjdump -res-usage): the padded-width-128 and -192 tiles of
-   k_conv_wg within the launch shape (<= 128 registers, no spills), k_conv_simt at kernel sizes 1 and 7 without spills;
+1. the conv instantiations in the built library (cuobjdump -res-usage): exactly one k_conv_wg tile per padded width and
+   one per head kind and no other, each within the launch shape (<= 128 registers, no spills), the width-256 dense tile and the
+   non-folding head at their pinned counts; k_conv_simt at kernel sizes 1 and 7 without spills;
 2. config validation: an even kernel size, or one outside 1..7, is refused before any device work, by CodecConfig and
    Model (ValueError) and by bsw_model_create (BSW_E_INVALID);
 3. the float32 / float64 model oracle against the reference Model's outputs for --kernel 5 / 1 / 7 models
@@ -38,12 +39,37 @@ def usage():
     return res
 
 
-@pytest.mark.parametrize("args", ["Tc128Args", "Tc192Args"])
-def test_new_tiles_fit_the_launch_shape(usage, args):
-    u = [v for k, v in usage.items() if re.search(rf"k_conv_wgINS_\d+{args}EEEv", k)]
+# Every k_conv_wg instantiation, as (test id, mangled template argument): the dense tile at each padded width and the
+# heads without and with the per-tap fold.
+CONV_WG_TILES = [(f"dense{w}", f"DenseArgsILi{w}E") for w in (64, 128, 192, 256, 320, 384, 448, 512)] + \
+                [("head", "HeadArgsILb0E"), ("head_fold", "HeadArgsILb1E")]
+# k_conv_wg runs 384 threads under __maxnreg__(128): 48 K registers, so a coder CTA still fits beside a conv CTA
+# (DESIGN 5.2).  SHARED is the static part only; the stages and hand-off tile are dynamic.
+PINNED_USAGE = {"dense256": {"REG": 128, "SHARED": 1024, "LOCAL": 0, "STACK": 0},
+                "head": {"REG": 128, "SHARED": 1024, "LOCAL": 0, "STACK": 0}}
+
+
+def _is_tile(name, args):
+    return re.search(rf"k_conv_wgINS_\d+{args}EEEEv", name) is not None
+
+
+def test_conv_wg_instantiations_are_exactly_the_tiles(usage):
+    """The library holds one k_conv_wg per padded width and head kind, and no other: a width missing from the
+    dispatcher, or a tile type left behind, changes the set."""
+    names = [k for k in usage if "k_conv_wg" in k]
+    tiles = [t for n in names for t, args in CONV_WG_TILES if _is_tile(n, args)]
+    assert len(tiles) == len(names), names
+    assert sorted(tiles) == sorted(t for t, _ in CONV_WG_TILES), names
+
+
+@pytest.mark.parametrize("tile,args", CONV_WG_TILES, ids=[t for t, _ in CONV_WG_TILES])
+def test_conv_wg_tiles_fit_the_launch_shape(usage, tile, args):
+    u = [v for k, v in usage.items() if _is_tile(k, args)]
     assert len(u) == 1, sorted(usage)
     assert u[0]["REG"] <= 128, u[0]
-    assert u[0]["LOCAL"] == 0 and u[0]["STACK"] == 0, f"{args} spills: {u[0]}"
+    assert u[0]["LOCAL"] == 0 and u[0]["STACK"] == 0, f"{tile} spills: {u[0]}"
+    if tile in PINNED_USAGE:
+        assert {k: u[0][k] for k in PINNED_USAGE[tile]} == PINNED_USAGE[tile]
 
 
 @pytest.mark.parametrize("ks,tco", [(1, 2), (1, 8), (7, 2), (7, 8)])
