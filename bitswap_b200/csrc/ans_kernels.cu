@@ -115,7 +115,8 @@ extern "C" int bsw_streams_min_words(bsw_streams *s, int64_t *min_host) {
     for (int i = 0; i < s->B; ++i) min_host[i] = n[i];
     return BSW_OK;
 }
-// a12 accounting: the word count right after a chain's first pop, the reference's len(restbits) - 1 (cifar_compress.py:190-192,254)
+// a12 accounting: the reference's len(restbits) - 1, the word count after the first image's first pop (Bit-Swap,
+// cifar_compress.py:190-192) or after all its nz pops (BB-ANS, :224-226); the encoder calls this at that point (codec.cu)
 __global__ void k_mark_rest(bsw_streams sv, int first, int count) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < count && sv.restwords[first + i] < 0) sv.restwords[first + i] = sv.nwords[first + i];
@@ -201,6 +202,7 @@ __global__ void k_unpack_words(bsw_streams sv, int first, const int64_t *__restr
     for (int i = threadIdx.x; i < n; i += blockDim.x) dst[i] = in[o + i];
     if (threadIdx.x == 0) {
         sv.nwords[first + b] = lo + n; sv.minwords[first + b] = base ? lo : n; sv.heads[first + b] = heads_in[b]; sv.flags[first + b] = 0;
+        sv.restwords[first + b] = -1;                     // a new chain starts here, as after import / fill
     }
 }
 static int pack_impl(bsw_streams *s, int first, int count, uint32_t *words_dev, int64_t *offsets_dev, uint64_t *heads_dev,

@@ -410,7 +410,7 @@ extern "C" int bsw_codec_encode_ext(bsw_codec *c, bsw_streams *s, int first, int
             RC(k.net(true, zi));
             k.hop(k.conv, k.rows);
             RC(k.level(true, zi, true, c->zs[zi]));
-            if (zi == 0) { RC(bsw_streams_mark_rest(s, first, count, k.ser)); ++k.nl; }     // :224-226 restbits
+            if (zi == nz - 1) { RC(bsw_streams_mark_rest(s, first, count, k.ser)); ++k.nl; }  // :224-226 restbits (after all nz pops)
             k.hop(k.ser, k.conv);
         }
         for (int zi = 0; zi < nz; ++zi) {

@@ -89,7 +89,8 @@ class StreamSet:
 
     @_on_own_device
     def rest_words(self):
-        """Word count right after the first pop of each chain (reference: len(restbits) - 1, cifar_compress.py:190-192)."""
+        """The reference's len(restbits) - 1 per stream (-1 until the chain reaches it): the word count after the first
+        image's first pop for Bit-Swap (cifar_compress.py:190-192), after all its nz pops for BB-ANS (:224-226)."""
         n = np.zeros(self.n, dtype=np.int64)
         check(lib().bsw_streams_rest_words(self._h, n.ctypes.data))
         return n
@@ -98,7 +99,7 @@ class StreamSet:
         """The reference's per-chain bookkeeping (cifar_compress.py:253-259) from the current stream sizes:
         net = totaladdedbits / (xdim * images)  with totaladdedbits = (len(state) - len(initialstate)) * 32,
         cma = totalbits / (xdim * images)       with totalbits = (len(state) - (len(restbits) - 1)) * 32 -- the
-        cumulative average INCLUDING the initial bits the first pop consumed."""
+        cumulative average INCLUDING the initial bits the first image's pops consumed up to restbits (rest_words)."""
         n, _, _ = self.sizes()
         rest = self.rest_words()
         added = (n - int(initial_words)) * 32.0
@@ -193,7 +194,9 @@ class StreamSet:
         import torch
         count = len(heads)
         total = int(offsets[count])
-        assert int(np.max(np.diff(offsets))) + (int(np.max(base)) if base is not None else 0) <= self.capacity
+        sent = np.diff(np.asarray(offsets[:count + 1], dtype=np.int64))
+        if count and int(np.max(sent + (np.asarray(base[:count], dtype=np.int64) if base is not None else 0))) > self.capacity:
+            raise OverflowError(f"import_packed_fast: a stream's base + packed length exceeds the capacity of {self.capacity} words")
         st = self._staging(count)
         if words.ctypes.data != st["words_h"].data_ptr():
             st["words_h"][:total].copy_(torch.from_numpy(np.ascontiguousarray(words).view(np.int32)))

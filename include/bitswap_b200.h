@@ -93,15 +93,17 @@ int bsw_streams_sizes(bsw_streams *s, int64_t *nwords_host, uint64_t *heads_host
 /* Lowest word count each stream has reached since import/fill: the part of the initial random words that was never
  * borrowed and can be trimmed from a stored bitstream (demo_compress.py:137,160 `excess_state_len`). Synchronous. */
 int bsw_streams_min_words(bsw_streams *s, int64_t *min_host);
-/* Word count of each stream right after the FIRST pop of its chain since import/fill (-1: none yet): the reference's
- * len(restbits) - 1, from which it reports `totalbits` and the cumulative moving average (cifar_compress.py:190-192,254,259).
- * Recorded by bsw_codec_encode.  Synchronous. */
+/* The reference's len(restbits) - 1 for each stream's chain since import/fill/unpack (-1: not reached yet), from which it
+ * reports `totalbits` and the cumulative moving average (cifar_compress.py:253-259): the word count after the first
+ * image's first pop for Bit-Swap (:190-192), after all nz pops of the first image for BB-ANS (:224-226).  Recorded by
+ * bsw_codec_encode.  Synchronous. */
 int bsw_streams_rest_words(bsw_streams *s, int64_t *rest_host);
 /* Packed export: stream i's words go to words_host[offsets_host[i] ...). Synchronous. */
 int bsw_streams_export(bsw_streams *s, int first, int count, uint32_t *words_host, const int64_t *offsets_host);
 /* Device-side packed (de)serialisation, async on `stream`: all streams' words gathered into one contiguous device
  * buffer (capacity >= total words; offsets_dev holds count+1 int64 prefix sums, heads_dev count uint64), or scattered back
- * (unpack requires every stream's length <= capacity; it also resets flags).  A host export is then three memcpys. */
+ * (unpack resets flags and rest words like import; a stream whose packed length exceeds its capacity is flagged
+ * BSW_E_OVERFLOW and left otherwise untouched).  A host export is then three memcpys. */
 int bsw_streams_pack(bsw_streams *s, int first, int count, uint32_t *words_dev, int64_t *offsets_dev, uint64_t *heads_dev,
                      void *stream);
 int bsw_streams_unpack(bsw_streams *s, int first, int count, const uint32_t *words_dev, const int64_t *offsets_dev,

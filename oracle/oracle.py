@@ -353,9 +353,18 @@ class BitSwapOracle:
     """One chain (= one reference 'experiment'): images are pushed one after
     another onto a single ANS state.  `coder` is AnsPort (list state) or AnsC
     (CState); pmf = "torch" (the reference's expression on torch CPU), "cuda" (the same
-    expression on torch CUDA -- how the reference itself runs it) or "c" (libm, ans_oracle.c)."""
+    expression on torch CUDA -- how the reference itself runs it) or "c" (libm, ans_oracle.c).
 
-    def __init__(self, cfg, model, zendpoints, zcentres, coder="c", pmf="torch", trace=None):
+    record: optional dict, the reference's per-chain bookkeeping, filled by every encode of the chain.  All lengths are
+    len(state) of the reference's list (words + head, = CState.n + 1):
+      init_len    length of the state the chain's first image was coded onto (len(initialstate), cifar_compress.py:159)
+      rest_len    len(restbits): the length after the first image's first pop for Bit-Swap (:190-192), after the last of
+                  its nz pops for BB-ANS (:224-226); None before that point
+      excess_len  demo_compress.py:137 `excess_state_len`: the least length after any pop, starting from init_len
+      push_lens   [(trace tag, length)] after every push, in order: the chain's peak depth and the push that reaches it
+      images      images coded so far"""
+
+    def __init__(self, cfg, model, zendpoints, zcentres, coder="c", pmf="torch", trace=None, record=None):
         self.cfg, self.model = cfg, model
         self.zend, self.zcen = zendpoints.double(), zcentres.double()
         # ImageBins (utils/torch/rand.py:146-152): 255 inner endpoints, 256 centres, identical for every dimension
@@ -363,7 +372,7 @@ class BitSwapOracle:
         self.xend = (((k - 127.5) / 127.5) - 1. / 255.)[None,].expand([cfg.xdim, -1])
         k = torch.arange(0, 256, dtype=torch.float64)
         self.xcen = ((k - 127.5) / 127.5)[None,].expand([cfg.xdim, -1])
-        self.coder_kind, self.pmf_kind, self.trace = coder, pmf, trace
+        self.coder_kind, self.pmf_kind, self.trace, self.record = coder, pmf, trace, record
         self.zr, self.xr = torch.arange(cfg.zdim), torch.arange(cfg.xdim)
         self.mu_hook = None     # optional: callable(kind, level, mu, scale) -> (mu, scale) to inject GPU nets
         self.timers = None      # optional dict: seconds per phase {net, cdf, tables, pop, push} (bench.py's 5-way split, BASELINE.md 3)
@@ -414,12 +423,34 @@ class BitSwapOracle:
             mu, sc = self.mu_hook(kind, level, mu, sc)
         return mu, sc
 
-    def _note(self, tag, st, sym=None):
+    def _note(self, tag, st, rest=False):
+        """Trace entry and accounting after one pop or push.  rest: this pop is where the reference takes restbits if the
+        chain has not taken it yet."""
+        n = len(st) if isinstance(st, list) else st.n + 1
         if self.trace is not None:
             if isinstance(st, list):
-                self.trace.append((tag, len(st), state_digest(np.array(st[:-1], dtype=np.uint64).astype(np.uint32), st[-1])))
+                self.trace.append((tag, n, state_digest(np.array(st[:-1], dtype=np.uint64).astype(np.uint32), st[-1])))
             else:
-                self.trace.append((tag, st.n + 1, st.digest()))
+                self.trace.append((tag, n, st.digest()))
+        r = self.record
+        if r is not None:
+            if tag.startswith("pop"):
+                r["excess_len"] = min(r["excess_len"], n)
+                if rest and r["rest_len"] is None:
+                    r["rest_len"] = n
+            else:
+                r["push_lens"].append((tag, n))
+
+    def _begin(self, st):
+        """A chain's first encode sets up its record (see the class docstring)."""
+        r = self.record
+        if r is not None and "init_len" not in r:
+            n = len(st) if isinstance(st, list) else st.n + 1
+            r.update(init_len=n, rest_len=None, excess_len=n, push_lens=[], images=0)
+
+    def _end(self):
+        if self.record is not None:
+            self.record["images"] += 1
 
     def _prior(self):
         c = self.cfg
@@ -431,12 +462,13 @@ class BitSwapOracle:
         x = torch.as_tensor(np.asarray(x).reshape(-1).astype(np.int64))
         q = c.quantbits
         zsym = None
+        self._begin(state)
         for zi in range(c.nz):
             given = self.zcen[zi - 1, self.zr, zsym] if zi > 0 else self.xcen[self.xr, x]           # :180
             mu, sc = self._net("infer", zi, given)                                                  # :181
             state, zsymtop = self._pop(self.zend[zi], mu, sc, q, state)                             # :182-187
             zsymtop = torch.as_tensor(np.asarray(zsymtop))
-            self._note(f"pop z{zi+1}", state)
+            self._note(f"pop z{zi+1}", state, rest=zi == 0)                                         # :190-192 restbits
             z = self.zcen[zi, self.zr, zsymtop]                                                     # :195
             mu, sc = self._net("generate", zi, z)                                                   # :196
             ends = self.zend[zi - 1] if zi > 0 else self.xend                                       # :197
@@ -445,6 +477,7 @@ class BitSwapOracle:
             zsym = zsymtop                                                                          # :204
         state = self._timed("push", self._timed("tables", self._coder, self._timed("cdf", self._prior), q).encode, state, zsym.numpy())   # :245-250
         self._note("push prior", state)
+        self._end()
         return state
 
     # -- Bit-Swap receiver, one image (cifar_compress.py:283-317) -------------------------------
@@ -471,12 +504,14 @@ class BitSwapOracle:
         x = torch.as_tensor(np.asarray(x).reshape(-1).astype(np.int64))
         q = c.quantbits
         zs, zsym = [], None
+        self._begin(state)
         for zi in range(c.nz):                                                                      # :209-221
             given = self.zcen[zi - 1, self.zr, zsym] if zi > 0 else self.xcen[self.xr, x]
             mu, sc = self._net("infer", zi, given)
             state, zsym = self._coder(self._pmfs(self.zend[zi], mu, sc), q).decode(state)
             zsym = torch.as_tensor(np.asarray(zsym))
             zs.append(zsym)
+            self._note(f"pop z{zi+1}", state, rest=zi == c.nz - 1)                                 # :224-226 restbits
         zsym = None
         for zi in range(c.nz):                                                                      # :228-240
             zsymtop = zs[zi]
@@ -485,8 +520,12 @@ class BitSwapOracle:
             ends = self.zend[zi - 1] if zi > 0 else self.xend
             state = self._coder(self._pmfs(ends, mu, sc), q if zi > 0 else 8).encode(
                 state, (zsym if zi > 0 else x).numpy())
+            self._note(f"push {'z%d' % zi if zi > 0 else 'x'}", state)
             zsym = zsymtop
-        return self._coder(self._prior(), q).encode(state, zsym.numpy())
+        state = self._coder(self._prior(), q).encode(state, zsym.numpy())                          # :245-250
+        self._note("push prior", state)
+        self._end()
+        return state
 
     def decode_image_bbans(self, state):
         c = self.cfg
