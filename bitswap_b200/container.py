@@ -17,13 +17,26 @@ whole image: it is tiled into ceil(H/32) x ceil(W/32) blocks, and a block on the
 pixels inside its valid extent (vh, vw) = (min(32, H - 32 by), min(32, W - 32 bx)) (bsw_codec_encode_ext).  The tail then
 holds the true H and W; an image whose sides are multiples of 32 gives the same container in both modes, and a header
 with a side off a multiple of 32 (which the crop mode never writes) is what marks an edge-coded container.
+
+Chains: one chain is serial (block t+1 starts from the state block t left), so coding time grows with an image's block
+count.  `chain_blocks=L` splits an image of n blocks into K = ceil(n / L) contiguous runs of its row-major blocks and codes
+each run as its own chain from the reference's seeded initial state; the K chains run side by side as K streams.  Each
+chain is exactly what the demo procedure writes for its run of blocks, and each keeps its own borrowed initial words, so
+more chains cost more bits.  K = 1 is the reference layout above; K >= 2 is written as
+    [ words_0 ... | ... | words_{K-1} ... | (nwords_k, head_lo_k, head_hi_k, nblocks_k) for k < K | K, h, w, CHAIN_MARK ]
+CHAIN_MARK >= 2^31 sits where the reference layout has w, so a reader of that layout alone sees an impossible header.
 """
+import numbers
+
 import numpy as np
 import torch
 
 from .codec import BITSWAP
 from .streams import StreamSet
 from .synthetic import initial_words
+
+CHAIN_MARK = 0x8043484E                  # bit 31 | "CHN": last word of a multi-chain container
+MAX_BLOCKS = 1 << 20                     # blocks per image a container may declare
 
 
 def extract_blocks(arr, block_size=(32, 32)):
@@ -85,65 +98,105 @@ def _model_to_blocks(x, hwc_quirk):
     return np.ascontiguousarray(x).reshape(n, bh, bw, c) if hwc_quirk else np.ascontiguousarray(x.transpose(0, 2, 3, 1))
 
 
+def chain_sizes(nblocks, chain_blocks=None):
+    """Block counts of the chains an image of `nblocks` row-major blocks is coded as, in block order: K = ceil(nblocks /
+    chain_blocks) contiguous runs whose sizes differ by at most one, larger runs first.  None, or chain_blocks >= nblocks:
+    one chain (the reference layout)."""
+    if chain_blocks is None or chain_blocks >= nblocks:
+        return [nblocks]
+    k = -(-nblocks // chain_blocks)
+    q, r = divmod(nblocks, k)
+    return [q + 1] * r + [q] * (k - r)
+
+
+def _check_chain_blocks(chain_blocks):
+    if chain_blocks is None:
+        return None
+    if isinstance(chain_blocks, bool) or not isinstance(chain_blocks, numbers.Integral) or chain_blocks < 1:
+        raise ValueError(f"chain_blocks must be None or a positive int, got {chain_blocks!r}")
+    return int(chain_blocks)
+
+
+def _sub_ranges(active, max_batch):
+    """(first, count) calls covering streams [0, active) with at most max_batch streams each.  The boundaries are multiples
+    of max_batch whatever `active` is, so a stream always lands at the same offset of a call: a free-running
+    PipelinedCodec then codes it on the same lane at every step."""
+    return [(b, min(max_batch, active - b)) for b in range(0, active, max_batch)]
+
+
+def _active(nblk):
+    """Streams still coding at each step t, for block counts sorted largest first: the active streams are a prefix."""
+    return np.searchsorted(-np.asarray(nblk), -np.arange(max(nblk)), side="left")
+
+
 def compress_images(codec, images, excess_state_len=10000, seed=100, scheme=BITSWAP, hwc_quirk=False, words_per_block=1400,
-                    edges="crop"):
+                    edges="crop", chain_blocks=None):
     """images: list of HWC uint8 arrays.  Returns one container array per image.
     Every chain starts from the reference's initial state: `excess_state_len` random words drawn with
     np.random.seed(100) (demo_compress.py:113-115, :202).
     edges="crop" (the reference's behaviour): every image is cropped down to multiples of 32 and must be at least 32x32.
     edges="code": the whole image (any H, W >= 1) is coded, with partial blocks at the bottom and right edges;
-    decompress_images returns it exactly."""
+    decompress_images returns it exactly.
+    chain_blocks: None (the reference's one chain per image) or a positive int L: an image of n > L blocks is coded as
+    ceil(n / L) chains of contiguous blocks (chain_sizes), which run side by side.  Fewer serial steps, more initial bits."""
     if edges not in ("crop", "code"):
         raise ValueError(f"edges must be 'crop' or 'code', got {edges!r}")
     if edges == "code" and hwc_quirk:
         raise ValueError("edges='code' needs the CHW block layout: hwc_quirk scrambles the rows and columns the extents refer to")
+    chain_blocks = _check_chain_blocks(chain_blocks)
     images = [np.asarray(im) for im in images]
     if edges == "code":
         tiled = [extract_edge_blocks(im) for im in images]
     else:
         tiled = [(b, None, h, w) for b, h, w in (extract_blocks(im) for im in images)]
-    order = sorted(range(len(images)), key=lambda i: (-tiled[i][0].shape[0], i))
-    nblk = [tiled[i][0].shape[0] for i in order]
-    n = len(images)
+    # chains (image, first block, blocks) in image and block order; streams hold them largest first
+    chains = []
+    for i, t in enumerate(tiled):
+        sizes = chain_sizes(t[0].shape[0], chain_blocks)
+        chains += [(i, s, nb) for s, nb in zip(np.cumsum([0] + sizes[:-1]).tolist(), sizes)]
+    order = sorted(range(len(chains)), key=lambda c: (-chains[c][2], c))
+    nblk = [chains[c][2] for c in order]
     w, head = initial_words(excess_state_len, seed=seed)
-    # capacity: `words_per_block` words per 32x32 block (1400 = 14.6 bits/dim; 8 bits/dim of raw pixels is 768).  A chain
-    # that still overflows is retried with twice the room instead of failing after the whole chain was coded.
+    # capacity: `words_per_block` words per 32x32 block of the longest chain (1400 = 14.6 bits/dim; 8 bits/dim of raw pixels
+    # is 768).  A chain that still overflows is retried with twice the room instead of failing after it was coded.
     for attempt in range(4):
-        ss = StreamSet(n, excess_state_len + (words_per_block << attempt) * max(nblk) + 64, device=codec.device)
+        ss = StreamSet(len(chains), excess_state_len + (words_per_block << attempt) * max(nblk) + 64, device=codec.device)
         ss.fill(w, head)
         try:
-            return _compress_chains(codec, ss, tiled, order, nblk, scheme, hwc_quirk)
+            return _compress_chains(codec, ss, tiled, chains, order, nblk, scheme, hwc_quirk)
         except OverflowError:
             if attempt == 3:
                 raise
     raise AssertionError("unreachable")
 
 
-def _compress_chains(codec, ss, tiled, order, nblk, scheme, hwc_quirk):
+def _compress_chains(codec, ss, tiled, chains, order, nblk, scheme, hwc_quirk):
     n = len(order)
-    # all blocks to the device once: [step t, stream j] = block t of the j-th largest image (CHW, demo_compress.py:120)
-    C = tiled[order[0]][0].shape[-1]
+    # all blocks to the device once: [step t, stream j] = block t of the j-th largest chain (CHW, demo_compress.py:120)
+    C = tiled[chains[order[0]][0]][0].shape[-1]
     host = np.zeros((max(nblk), n, C, 32, 32), dtype=np.uint8)
-    for j, i in enumerate(order):
-        host[:nblk[j], j] = _blocks_to_model(tiled[i][0], hwc_quirk)
+    model = [_blocks_to_model(t[0], hwc_quirk) for t in tiled]
+    for j, c in enumerate(order):
+        i, s, nb = chains[c]
+        host[:nb, j] = model[i][s:s + nb]
     dev = torch.from_numpy(host).to(torch.device("cuda", codec.device))
-    ext = _extents_to_device(codec, [tiled[i][1] for i in order], nblk)
+    ext = _extents_to_device(codec, [None if tiled[i][1] is None else tiled[i][1][s:s + nb] for i, s, nb in
+                                     (chains[c] for c in order)], nblk)
+    active = _active(nblk)
     for t in range(max(nblk)):
-        active = sum(1 for b in nblk if b > t)
-        codec.encode(ss, dev[t, :active].contiguous(), first=0, scheme=scheme,
-                     extent=None if ext is None else ext[t, :active].contiguous())
+        for b, cnt in _sub_ranges(int(active[t]), codec.max_batch):
+            codec.encode(ss, dev[t, b:b + cnt], first=b, scheme=scheme, extent=None if ext is None else ext[t, b:b + cnt])
     torch.cuda.synchronize()
     ss.raise_on_error()
     words, offs, heads, _ = ss.export()
     lo = ss.min_words()                                       # never-borrowed initial words (demo_compress.py:137,160)
-    out = [None] * n
-    for j, i in enumerate(order):
-        ws = words[offs[j] + lo[j]:offs[j + 1]]
-        hd = int(heads[j])
-        _, _, h, wd = tiled[i]
-        tail = np.array([hd & 0xffffffff, hd >> 32, nblk[j], h, wd], dtype=np.uint32)           # demo_compress.py:272-279
-        out[i] = np.concatenate([ws.astype(np.uint32), tail])
-    return out
+    mine = [[] for _ in tiled]                                # each image's streams, in block order
+    stream = np.empty(n, dtype=np.int64)
+    stream[order] = np.arange(n)
+    for c, (i, _, _) in enumerate(chains):
+        mine[i].append(int(stream[c]))
+    return [pack_container([(words[offs[j] + lo[j]:offs[j + 1]], int(heads[j]), nblk[j]) for j in js], h, wd)
+            for js, (_, _, h, wd) in zip(mine, tiled)]
 
 
 def _extents_to_device(codec, extents, nblk):
@@ -158,42 +211,95 @@ def _extents_to_device(codec, extents, nblk):
     return torch.from_numpy(host).to(torch.device("cuda", codec.device))
 
 
+def pack_container(chains, h, w):
+    """One image's container from its chains in block order, [(words uint32 [m], head int, nblocks)]: the reference layout
+    for one chain (demo_compress.py:272-279), the multi-chain layout (module docstring) for two or more."""
+    if len(chains) == 1:
+        ws, hd, nb = chains[0]
+        return np.concatenate([np.asarray(ws, dtype=np.uint32),
+                               np.array([hd & 0xffffffff, hd >> 32, nb, h, w], dtype=np.uint32)])
+    table = np.array([(len(ws), hd & 0xffffffff, hd >> 32, nb) for ws, hd, nb in chains], dtype=np.uint32)
+    return np.concatenate([np.asarray(ws, dtype=np.uint32) for ws, _, _ in chains]
+                          + [table.reshape(-1), np.array([len(chains), h, w, CHAIN_MARK], dtype=np.uint32)])
+
+
+def _check_header(nblocks, h, w, hwc_quirk):
+    if h <= 0 or w <= 0 or nblocks != np.prod(block_grid(h, w)) or nblocks > MAX_BLOCKS:
+        raise ValueError(f"inconsistent container header: nblocks={nblocks}, h={h}, w={w}")
+    if hwc_quirk and (h % 32 or w % 32):
+        raise ValueError(f"edge-coded container (h={h}, w={w}) cannot be decoded with hwc_quirk")
+
+
+def unpack_container(c, hwc_quirk=False):
+    """Inverse of pack_container: (words uint32, offsets int64 [K+1], heads uint64 [K], nblocks int64 [K], h, w), chain k's
+    words being words[offsets[k]:offsets[k+1]].  Every field is checked here, before anything is sized from it: a truncated
+    or inconsistent container is a ValueError."""
+    c = np.asarray(c, dtype=np.uint32)
+    if c.ndim != 1 or c.size < 5:
+        raise ValueError(f"container too short ({c.size} words): needs at least head_lo, head_hi, nblocks, h, w")
+    if int(c[-1]) != CHAIN_MARK:
+        nblocks, h, w = int(c[-3]), int(c[-2]), int(c[-1])                                      # demo_decompress.py:216-219
+        _check_header(nblocks, h, w, hwc_quirk)
+        head = (int(c[-4]) << 32) | int(c[-5])                                                  # :222
+        return (c[:-5], np.array([0, c.size - 5], dtype=np.int64), np.array([head], dtype=np.uint64),
+                np.array([nblocks], dtype=np.int64), h, w)
+    k, h, w = int(c[-4]), int(c[-3]), int(c[-2])
+    if k < 2 or c.size < 4 * k + 4:
+        raise ValueError(f"multi-chain container of {c.size} words cannot hold the table of its {k} chains")
+    table = c[c.size - 4 * k - 4:-4].reshape(k, 4).astype(np.int64)
+    nwords, nblocks = table[:, 0], table[:, 3]
+    if (nblocks < 1).any():
+        raise ValueError("multi-chain container: a chain with no blocks")
+    _check_header(int(nblocks.sum()), h, w, hwc_quirk)                 # (so also K <= blocks, as each chain has one)
+    body = c.size - 4 * k - 4
+    if int(nwords.sum()) != body:
+        raise ValueError(f"multi-chain container: the chains claim {int(nwords.sum())} words, the container holds {body}")
+    offsets = np.zeros(k + 1, dtype=np.int64)
+    np.cumsum(nwords, out=offsets[1:])
+    heads = (table[:, 2].astype(np.uint64) << np.uint64(32)) | table[:, 1].astype(np.uint64)
+    return c[:body], offsets, heads, nblocks, h, w
+
+
 def decompress_images(codec, containers, channels=3, scheme=BITSWAP, hwc_quirk=False, headroom_words=None):
     """Inverse of compress_images: list of container arrays -> list of HWC uint8 images (the cropped size for a crop-mode
-    container, the full size for an edge-coded one: a header whose h or w is not a multiple of 32)."""
-    meta = []
-    for c in containers:
-        c = np.asarray(c, dtype=np.uint32)
-        if c.ndim != 1 or c.size < 5:
-            raise ValueError(f"container too short ({c.size} words): needs at least head_lo, head_hi, nblocks, h, w")
-        nblocks, h, w = int(c[-3]), int(c[-2]), int(c[-1])                                      # demo_decompress.py:216-219
-        if h <= 0 or w <= 0 or nblocks != np.prod(block_grid(h, w)) or nblocks > (1 << 20):
-            raise ValueError(f"inconsistent container header: nblocks={nblocks}, h={h}, w={w}")
-        if hwc_quirk and (h % 32 or w % 32):
-            raise ValueError(f"edge-coded container (h={h}, w={w}) cannot be decoded with hwc_quirk")
-        head = (int(c[-4]) << 32) | int(c[-5])                                                  # :222
-        meta.append((c[:-5], head, nblocks, h, w))
-    order = sorted(range(len(containers)), key=lambda i: (-meta[i][2], i))
-    nblk = [meta[i][2] for i in order]
-    n = len(containers)
+    container, the full size for an edge-coded one: a header whose h or w is not a multiple of 32).  Single- and
+    multi-chain containers can be mixed in one call."""
+    parsed = [unpack_container(c, hwc_quirk) for c in containers]
+    # chains in image and block order: image, index within the image, first block, blocks
+    cimg = np.concatenate([np.full(len(p[3]), i) for i, p in enumerate(parsed)])
+    ck = np.concatenate([np.arange(len(p[3])) for p in parsed])
+    cstart = np.concatenate([np.cumsum(p[3]) - p[3] for p in parsed])
+    cnb = np.concatenate([p[3] for p in parsed])
+    order = np.argsort(-cnb, kind="stable")                                                   # streams: largest chain first
+    pieces = [parsed[i][0][parsed[i][1][k]:parsed[i][1][k + 1]] for i, k in zip(cimg[order], ck[order])]
+    nblk = cnb[order].tolist()
+    n = len(nblk)
     # The receiver pushes too (it returns the borrowed bits, cifar_compress.py:306-313): one block's worth of latents,
-    # nz * zdim symbols at <= 31 bits each, can sit on the stack above the container's own length.
+    # nz * zdim symbols at <= 31 bits each, can sit on the stack above the chain's own length.
     if headroom_words is None:
         headroom_words = codec.cfg.nz * codec.cfg.zdim + 64
-    ss = StreamSet(n, max(len(meta[i][0]) for i in order) + headroom_words, device=codec.device)
-    ss.import_lists([[int(v) for v in meta[i][0]] + [meta[i][1]] for i in order])
+    ss = StreamSet(n, max(len(p) for p in pieces) + headroom_words, device=codec.device)
+    offs = np.zeros(n + 1, dtype=np.int64)
+    np.cumsum([len(p) for p in pieces], out=offs[1:])
+    ss.import_packed(np.concatenate(pieces), offs, np.array([parsed[i][2][k] for i, k in zip(cimg[order], ck[order])],
+                                                              dtype=np.uint64))
     dev = torch.zeros((max(nblk), n, channels, 32, 32), dtype=torch.uint8, device=torch.device("cuda", codec.device))
-    ext = _extents_to_device(codec, [block_extents(meta[i][3], meta[i][4]) for i in order], nblk)
+    extents = [block_extents(p[4], p[5]) for p in parsed]
+    ext = _extents_to_device(codec, [extents[i][s:s + nb] for i, s, nb in zip(cimg[order], cstart[order], nblk)], nblk)
+    active = _active(nblk)
     for t in reversed(range(max(nblk))):
-        active = sum(1 for b in nblk if b > t)
-        codec.decode(ss, active, first=0, scheme=scheme, out=dev[t, :active],
-                     extent=None if ext is None else ext[t, :active].contiguous())
+        for b, cnt in _sub_ranges(int(active[t]), codec.max_batch):
+            codec.decode(ss, cnt, first=b, scheme=scheme, out=dev[t, b:b + cnt],
+                         extent=None if ext is None else ext[t, b:b + cnt])
     if hasattr(codec, "join"):                                             # (free-running multi-lane codec: lanes -> current stream)
         codec.join()
     host = dev.cpu().numpy()                                               # one transfer for every block of every image
-    blocks = [_model_to_blocks(host[:nblk[j], j], hwc_quirk) for j in range(n)]
     ss.raise_on_error()
-    out = [None] * n
-    for j, i in enumerate(order):
-        out[i] = unextract_edge_blocks(blocks[j], meta[i][3], meta[i][4])
+    stream = np.empty(n, dtype=np.int64)
+    stream[order] = np.arange(n)
+    out = []
+    for i, p in enumerate(parsed):
+        js = stream[cimg == i]                                             # this image's chains in block order
+        blocks = np.concatenate([host[:nblk[j], j] for j in js])
+        out.append(unextract_edge_blocks(_model_to_blocks(blocks, hwc_quirk), p[4], p[5]))
     return out
