@@ -25,7 +25,13 @@ chain is exactly what the demo procedure writes for its run of blocks, and each 
 more chains cost more bits.  K = 1 is the reference layout above; K >= 2 is written as
     [ words_0 ... | ... | words_{K-1} ... | (nwords_k, head_lo_k, head_hi_k, nblocks_k) for k < K | K, h, w, CHAIN_MARK ]
 CHAIN_MARK >= 2^31 sits where the reference layout has w, so a reader of that layout alone sees an impossible header.
+
+Regions: a chain is a stack, so decoding pops its blocks last to first; to reach block j of a chain of n blocks the decoder
+pops n - j blocks and no further, and a chain none of whose blocks is wanted is not imported at all.  decompress_regions
+decodes only that (plan_regions says how much), and decompress_images is the same path with one whole-image region per
+container.
 """
+import collections
 import numbers
 
 import numpy as np
@@ -260,20 +266,89 @@ def unpack_container(c, hwc_quirk=False):
     return c[:body], offsets, heads, nblocks, h, w
 
 
+RegionPlan = collections.namedtuple("RegionPlan", "first depth needed")
+RegionPlan.__doc__ = """What decoding a container's regions costs.  first, depth: int64 [K], per chain in block order, the
+earliest block the regions need counted from the chain's first block (the chain's block count when it holds none of them)
+and the blocks to pop to reach it, nblocks - first (0: the chain is skipped).  needed: bool [nblocks], the row-major
+blocks the regions cover."""
+
+
+def _check_region(r, parsed):
+    try:
+        fields = tuple(r)
+    except TypeError:
+        raise ValueError(f"a region is (i, y, x, h, w), got {r!r}") from None
+    if len(fields) != 5 or not all(isinstance(v, numbers.Integral) and not isinstance(v, bool) for v in fields):
+        raise ValueError(f"a region is five ints (i, y, x, h, w), got {r!r}")
+    i, y, x, h, w = (int(v) for v in fields)
+    if not 0 <= i < len(parsed):
+        raise ValueError(f"region {r!r}: no container {i} among {len(parsed)}")
+    H, W = parsed[i][4], parsed[i][5]
+    if h < 1 or w < 1 or y < 0 or x < 0 or y + h > H or x + w > W:
+        raise ValueError(f"region {r!r} is empty or leaves the {H} x {W} image of container {i}")
+    return i, y, x, h, w
+
+
+def _plan(parsed, regions):
+    """(regions as int tuples, one RegionPlan per container) for unpack_container results.  Every region is checked here."""
+    regions = [_check_region(r, parsed) for r in regions]
+    boxes = collections.defaultdict(list)
+    for i, y, x, h, w in regions:
+        boxes[i].append((y, x, h, w))
+    plans = []
+    for i, (_, _, _, nblocks, H, W) in enumerate(parsed):
+        gw = block_grid(H, W)[1]
+        needed = np.zeros(int(nblocks.sum()), dtype=bool)
+        grid = needed.reshape(-1, gw)
+        for y, x, h, w in boxes[i]:
+            grid[y // 32:(y + h - 1) // 32 + 1, x // 32:(x + w - 1) // 32 + 1] = True
+        starts = np.cumsum(nblocks) - nblocks
+        earliest = np.minimum.reduceat(np.where(needed, np.arange(needed.size), needed.size), starts)
+        first = np.minimum(earliest - starts, nblocks)
+        plans.append(RegionPlan(first, nblocks - first, needed))
+    return regions, plans
+
+
+def plan_regions(containers, regions, hwc_quirk=False):
+    """The decode plan of decompress_regions, computed on the host alone: one RegionPlan per container.  regions: list of
+    (i, y, x, h, w) in pixels of container i's decoded image (the cropped size for a crop-mode container).  A malformed
+    container, or a region that is empty, leaves the image, has a non-int field or names no container, is a ValueError."""
+    parsed = [unpack_container(c, hwc_quirk) for c in containers]
+    return _plan(parsed, regions)[1]
+
+
+def decompress_regions(codec, containers, regions, channels=3, scheme=BITSWAP, hwc_quirk=False, headroom_words=None):
+    """regions: list of (i, y, x, h, w) -> one HWC uint8 array per region, equal to decompress_images(...)[i][y:y+h, x:x+w].
+    Only the chains holding a wanted block are imported, and each is popped only down to the earliest block any region on
+    its container wants (plan_regions): a chain of n blocks whose earliest wanted block is j costs n - j block decodes.
+    Blocks are row-major, so a window near an image's bottom is cheapest, and a single-chain container gains only there."""
+    parsed = [unpack_container(c, hwc_quirk) for c in containers]
+    return _decode_regions(codec, parsed, regions, channels, scheme, hwc_quirk, headroom_words)
+
+
 def decompress_images(codec, containers, channels=3, scheme=BITSWAP, hwc_quirk=False, headroom_words=None):
     """Inverse of compress_images: list of container arrays -> list of HWC uint8 images (the cropped size for a crop-mode
     container, the full size for an edge-coded one: a header whose h or w is not a multiple of 32).  Single- and
     multi-chain containers can be mixed in one call."""
     parsed = [unpack_container(c, hwc_quirk) for c in containers]
-    # chains in image and block order: image, index within the image, first block, blocks
+    return _decode_regions(codec, parsed, [(i, 0, 0, p[4], p[5]) for i, p in enumerate(parsed)], channels, scheme,
+                           hwc_quirk, headroom_words)
+
+
+def _decode_regions(codec, parsed, regions, channels, scheme, hwc_quirk, headroom_words):
+    regions, plans = _plan(parsed, regions)
+    if not regions:
+        return []
+    # chains in image and block order: image, index within the image, first block, blocks, blocks to pop
     cimg = np.concatenate([np.full(len(p[3]), i) for i, p in enumerate(parsed)])
     ck = np.concatenate([np.arange(len(p[3])) for p in parsed])
     cstart = np.concatenate([np.cumsum(p[3]) - p[3] for p in parsed])
     cnb = np.concatenate([p[3] for p in parsed])
-    order = np.argsort(-cnb, kind="stable")                                                   # streams: largest chain first
+    cdepth = np.concatenate([pl.depth for pl in plans])
+    order = np.argsort(-cdepth, kind="stable")[:np.count_nonzero(cdepth)]   # streams: deepest chain first, skipped ones out
     pieces = [parsed[i][0][parsed[i][1][k]:parsed[i][1][k + 1]] for i, k in zip(cimg[order], ck[order])]
-    nblk = cnb[order].tolist()
-    n = len(nblk)
+    depth = cdepth[order].tolist()
+    n = len(depth)
     # The receiver pushes too (it returns the borrowed bits, cifar_compress.py:306-313): one block's worth of latents,
     # nz * zdim symbols at <= 31 bits each, can sit on the stack above the chain's own length.
     if headroom_words is None:
@@ -283,23 +358,38 @@ def decompress_images(codec, containers, channels=3, scheme=BITSWAP, hwc_quirk=F
     np.cumsum([len(p) for p in pieces], out=offs[1:])
     ss.import_packed(np.concatenate(pieces), offs, np.array([parsed[i][2][k] for i, k in zip(cimg[order], ck[order])],
                                                               dtype=np.uint64))
-    dev = torch.zeros((max(nblk), n, channels, 32, 32), dtype=torch.uint8, device=torch.device("cuda", codec.device))
+    # Steps are aligned at the chains' ends: step s pops block n - 1 - s of every stream deeper than s, so the active
+    # streams stay a prefix and [s, stream] holds that block, in the output and in the extents alike.
+    dev = torch.empty((max(depth), n, channels, 32, 32), dtype=torch.uint8, device=torch.device("cuda", codec.device))
     extents = [block_extents(p[4], p[5]) for p in parsed]
-    ext = _extents_to_device(codec, [extents[i][s:s + nb] for i, s, nb in zip(cimg[order], cstart[order], nblk)], nblk)
-    active = _active(nblk)
-    for t in reversed(range(max(nblk))):
-        for b, cnt in _sub_ranges(int(active[t]), codec.max_batch):
-            codec.decode(ss, cnt, first=b, scheme=scheme, out=dev[t, b:b + cnt],
-                         extent=None if ext is None else ext[t, b:b + cnt])
+    ext = _extents_to_device(codec, [extents[i][s + nb - d:s + nb][::-1] for i, s, nb, d in
+                                     zip(cimg[order], cstart[order], cnb[order], depth)], depth)
+    active = _active(depth)
+    for s in range(max(depth)):
+        for b, cnt in _sub_ranges(int(active[s]), codec.max_batch):
+            codec.decode(ss, cnt, first=b, scheme=scheme, out=dev[s, b:b + cnt],
+                         extent=None if ext is None else ext[s, b:b + cnt])
     if hasattr(codec, "join"):                                             # (free-running multi-lane codec: lanes -> current stream)
         codec.join()
-    host = dev.cpu().numpy()                                               # one transfer for every block of every image
-    ss.raise_on_error()
-    stream = np.empty(n, dtype=np.int64)
+    # the needed blocks of every image, gathered on the device into one transfer; pos[i][b]: block b's row in it
+    stream = np.full(len(cnb), -1, dtype=np.int64)
     stream[order] = np.arange(n)
+    first_chain = np.cumsum([0] + [len(p[3]) for p in parsed])
+    rows, pos, m = [], [], 0
+    for i, (p, pl) in enumerate(zip(parsed, plans)):
+        b = np.flatnonzero(pl.needed)
+        c = first_chain[i] + np.searchsorted(np.cumsum(p[3]), b, side="right")
+        rows.append((cstart[c] + cnb[c] - 1 - b) * n + stream[c])
+        pos.append(np.full(pl.needed.size, -1, dtype=np.int64))
+        pos[i][b] = m + np.arange(b.size)
+        m += b.size
+    idx = torch.from_numpy(np.concatenate(rows)).to(dev.device)
+    host = _model_to_blocks(dev.view(-1, channels, 32, 32).index_select(0, idx).cpu().numpy(), hwc_quirk)
+    ss.raise_on_error()
     out = []
-    for i, p in enumerate(parsed):
-        js = stream[cimg == i]                                             # this image's chains in block order
-        blocks = np.concatenate([host[:nblk[j], j] for j in js])
-        out.append(unextract_edge_blocks(_model_to_blocks(blocks, hwc_quirk), p[4], p[5]))
+    for i, y, x, h, w in regions:
+        gw = block_grid(parsed[i][4], parsed[i][5])[1]
+        by, bx = np.arange(y // 32, (y + h - 1) // 32 + 1), np.arange(x // 32, (x + w - 1) // 32 + 1)
+        tile = unextract_blocks(host[pos[i][by[:, None] * gw + bx[None, :]].reshape(-1)], 32 * by.size, 32 * bx.size)
+        out.append(np.ascontiguousarray(tile[y - 32 * by[0]:y - 32 * by[0] + h, x - 32 * bx[0]:x - 32 * bx[0] + w]))
     return out
