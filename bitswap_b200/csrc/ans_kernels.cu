@@ -11,7 +11,7 @@
 #include <stdarg.h>
 #include <string.h>
 #include <vector>
-#include "bsw_common.cuh"
+#include "coder.cuh"
 
 static thread_local char g_err[512] = "";
 void bsw_set_error(const char *fmt, ...) {
@@ -22,8 +22,6 @@ void bsw_set_error(const char *fmt, ...) {
 }
 extern "C" const char *bsw_last_error(void) { return g_err; }
 extern "C" int bsw_version(void) { return 100; }
-
-#define FULL 0xffffffffu
 
 // ================================================================================================
 // Stream sets
@@ -268,87 +266,10 @@ extern "C" int bsw_streams_total_words(bsw_streams *s, int64_t *total_dev, void 
 }
 
 // ================================================================================================
-// Warp-level helpers shared by the coder kernels
+// Warp reductions of the table kernels
 // ================================================================================================
-// Per-warp view of one stream with a 32-word register window over the top of the stack, so that the
-// renormalisation words move to/from HBM as whole 128-byte lines.
-struct WarpStream {
-    uint32_t *words;   // this stream's row
-    uint64_t x;        // head (replicated in all lanes)
-    int len, cap;
-    int wbase;         // index of the word lane 0 holds (multiple of 32), or -1
-    uint32_t wbuf;     // lane j holds words[wbase + j]
-    int err;
-
-    __device__ __forceinline__ void open(const bsw_streams &sv, int b) {
-        words = sv.words + (int64_t)b * sv.cap;
-        x = sv.heads[b];
-        len = sv.nwords[b];
-        cap = (int)sv.cap;
-        err = sv.flags[b];
-        wbase = -1;
-        wbuf = 0;
-    }
-    __device__ __forceinline__ void close(const bsw_streams &sv, int b, int lane) {
-        if (lane == 0) { sv.heads[b] = x; sv.nwords[b] = len; sv.flags[b] = err; if (len < sv.minwords[b]) sv.minwords[b] = len; }
-    }
-    // ---- pop side: window slides downward -------------------------------------------------------
-    __device__ __forceinline__ uint32_t pop_word(int lane) {     // caller guarantees len > 0
-        int idx = len - 1;
-        if (wbase < 0 || idx < wbase) {
-            wbase = idx & ~31;
-            wbuf = words[wbase + lane];
-        }
-        len = idx;
-        return __shfl_sync(FULL, wbuf, idx - wbase);
-    }
-    // ---- push side: window slides upward --------------------------------------------------------
-    __device__ __forceinline__ void push_begin(int lane) {
-        wbase = len & ~31;
-        wbuf = (wbase + lane < len) ? words[wbase + lane] : 0u;
-    }
-    __device__ __forceinline__ void push_word(uint32_t w, int lane) {   // caller guarantees len < cap
-        if (lane == len - wbase) wbuf = w;
-        ++len;
-        if (len - wbase == 32) {
-            words[wbase + lane] = wbuf;
-            wbase += 32;
-        }
-    }
-    __device__ __forceinline__ void push_end(int lane) {
-        if (lane < len - wbase) words[wbase + lane] = wbuf;
-    }
-    // ---- the integer recurrences (cifar_compress.py:51-54 and :60-65) -------------------------------
-    __device__ __forceinline__ void encode(uint32_t p, uint32_t c, int bits, int lane) {
-        uint64_t lim = ((((uint64_t)1 << 32) >> bits) << 32) * (uint64_t)p;
-        if (x >= lim) {
-            if (len >= cap) { err = BSW_E_OVERFLOW; return; }
-            push_word((uint32_t)x, lane);
-            x >>= 32;
-        }
-        uint64_t qd = x / p;
-        uint64_t rm = x - qd * p;
-        x = (qd << bits) + rm + c;
-    }
-    __device__ __forceinline__ void decode(uint32_t p, uint32_t c, uint32_t m, int bits, int lane) {
-        x = (uint64_t)p * (x >> bits) + m - c;
-        if (x < ((uint64_t)1 << 32)) {
-            if (len <= 0) { err = BSW_E_UNDERFLOW; return; }
-            uint32_t w = pop_word(lane);
-            x = (x << 32) | w;
-        }
-    }
-};
-
 __device__ __forceinline__ uint32_t warp_sum_u32(uint32_t v) {
     for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
-    return v;
-}
-__device__ __forceinline__ uint32_t warp_incl_scan_u32(uint32_t v, int lane) {
-    for (int o = 1; o < 32; o <<= 1) {
-        uint32_t t = __shfl_up_sync(FULL, v, o);
-        if (lane >= o) v += t;
-    }
     return v;
 }
 // argmax with the reference's tie rule (first index wins, cifar_compress.py:35 / torch.argmax)
@@ -852,16 +773,8 @@ static int dispatch_fused(bool push, bsw_streams *s, int first, int count, const
     BSW_REQUIRE(bits > 0 && bits <= 31 && q >= 0 && q < bits, "fused coder: bits/quantbits out of range");
     BSW_REQUIRE((ers == 0 || ers >= S) && (((uintptr_t)endp) & 7) == 0, "fused coder: endpoint rows must hold S doubles (+inf padded)");
     cudaStream_t st = (cudaStream_t)stream;
-    switch (S) {
-        case 32:   return launch_fused<1>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext, st);
-        case 64:   return launch_fused<2>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext, st);
-        case 128:  return launch_fused<4>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext, st);
-        case 256:  return launch_fused<8>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext, st);
-        case 512:  return launch_fused<16>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext, st);
-        case 1024: return launch_fused<32>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext, st);
-    }
-    bsw_set_error("fused coder: support must be one of 32,64,...,1024 (got %d; wider supports need the two-phase coder)", S);
-    return BSW_E_INVALID;
+    return with_support<1, 32>(S, "fused coder: support must be one of 32,64,...,1024 (wider supports need the two-phase coder)",
+                               [&](auto nb) { return launch_fused<decltype(nb)::value>(push, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, ext, st); });
 }
 extern "C" int bsw_logistic_push(bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
                                  int64_t sss, const double *endp, int64_t ers, const int16_t *sym, int64_t L, int S,
@@ -883,7 +796,6 @@ int bsw_logistic_fused_ext(bool push, bsw_streams *s, int first, int count, cons
 // ================================================================================================
 // Bin tables + centre gathers (a5, a6, a7 data)
 // ================================================================================================
-int bsw_rows6_build_meta(const double *endp, int64_t ers, int64_t L, int S, void *meta_dev, int *n_affine_host, cudaStream_t st);   // ans_rows6.cu
 extern "C" int bsw_bins_create(bsw_bins **out, int nz, int zdim, int q, int xdim, const double *zend_host,
                                const double *zcen_host) {
     // q <= 12: supports up to 4096 bins, coded by the two-phase kernels (the fused ones stop at 1024, see

@@ -4,86 +4,22 @@
 // the FP64 pipe 27 % utilised at 1024 streams (7 warps per SM, long
 // dependent DFMA chains).  The table of a row does not depend on the ANS head, only the *search* does, so:
 //
-//   phase A  (k_rows_push / k_rows_pop)   one warp per (stream,row), fully parallel over count x L rows:
+//   phase A  (k_rows / k_rows_wide)  one warp per (stream,row), fully parallel over count x L rows:
 //            float64 logistic cdf -> trunc -> remnant at the row argmax (ANS.__init__ semantics,
 //            cifar_compress.py:28-39).  Streaming reductions only, so few registers and high occupancy.
 //            push: emits the (P_s, C_s) pair of the symbol being coded            ->  8 B per row
-//            pop : emits the integer cdf at every 32nd bin ("coarse cdf", 32 x 4 B) and (argmax, remnant)
+//            pop : emits the integer cdf at the start of every chunk (up to 32 x 4 B) and (argmax, remnant)
 //   phase B  (k_push_pairs / k_pop_coarse) one warp per stream, serial in the head as the reference is
-//            (cifar_compress.py:48-67): push consumes the pairs; pop finds the 32-bin chunk containing
-//            m = head & mask in the coarse cdf, recomputes just that chunk's 33 cdf values with the same
+//            (cifar_compress.py:48-67): push consumes the pairs; pop finds the chunk containing
+//            m = head & mask from the chunk bases, recomputes just that chunk's cdf values with the same
 //            float64 function (bit-identical by construction) and finishes the search with a warp scan.
 //
 // Results are bit-identical to the fused kernels (integer sums are associative; the cdf function is shared).
 #include <stdlib.h>
-#include <type_traits>
 #include <string.h>
-#include "bsw_common.cuh"
-
-#define FULL 0xffffffffu
+#include "coder.cuh"
 
 namespace {
-
-struct WarpStream2 {          // same state handling as ans_kernels.cu's WarpStream
-    uint32_t *words;
-    uint64_t x;
-    int len, cap, wbase, err;
-    uint32_t wbuf;
-    __device__ __forceinline__ void open(const bsw_streams &sv, int b) {
-        words = sv.words + (int64_t)b * sv.cap; x = sv.heads[b]; len = sv.nwords[b]; cap = (int)sv.cap;
-        err = sv.flags[b]; wbase = -1; wbuf = 0;
-    }
-    __device__ __forceinline__ void close(const bsw_streams &sv, int b, int lane) {
-        if (lane == 0) { sv.heads[b] = x; sv.nwords[b] = len; sv.flags[b] = err; if (len < sv.minwords[b]) sv.minwords[b] = len; }
-    }
-    __device__ __forceinline__ uint32_t pop_word(int lane) {
-        int idx = len - 1;
-        if (wbase < 0 || idx < wbase) { wbase = idx & ~31; wbuf = words[wbase + lane]; }
-        len = idx;
-        return __shfl_sync(FULL, wbuf, idx - wbase);
-    }
-    __device__ __forceinline__ void push_begin(int lane) {
-        wbase = len & ~31;
-        wbuf = (wbase + lane < len) ? words[wbase + lane] : 0u;
-    }
-    __device__ __forceinline__ void push_word(uint32_t w, int lane) {
-        if (lane == len - wbase) wbuf = w;
-        ++len;
-        if (len - wbase == 32) { words[wbase + lane] = wbuf; wbase += 32; }
-    }
-    __device__ __forceinline__ void push_end(int lane) { if (lane < len - wbase) words[wbase + lane] = wbuf; }
-    __device__ __forceinline__ void encode(uint32_t p, uint32_t c, int bits, int lane) {      // cifar_compress.py:51-54
-        uint64_t lim = ((((uint64_t)1 << 32) >> bits) << 32) * (uint64_t)p;
-        if (x >= lim) {
-            if (len >= cap) { err = BSW_E_OVERFLOW; return; }
-            push_word((uint32_t)x, lane);
-            x >>= 32;
-        }
-        uint64_t qd = x / p;
-        x = (qd << bits) + (x - qd * p) + c;
-    }
-    // same recurrence with the division replaced by a multiply with M = floor((2^64-1)/p) computed in the parallel phase:
-    // floor(x*M / 2^64) is floor(x/p) or one less, so a single correction makes it exact
-    __device__ __forceinline__ void encode_magic(uint32_t p, uint32_t c, uint64_t M, int bits, int lane) {
-        uint64_t lim = ((((uint64_t)1 << 32) >> bits) << 32) * (uint64_t)p;
-        if (x >= lim) {
-            if (len >= cap) { err = BSW_E_OVERFLOW; return; }
-            push_word((uint32_t)x, lane);
-            x >>= 32;
-        }
-        uint64_t qd = __umul64hi(x, M);
-        uint64_t rm = x - qd * p;
-        if (rm >= p) { rm -= p; ++qd; }
-        x = (qd << bits) + rm + c;
-    }
-    __device__ __forceinline__ void decode(uint32_t p, uint32_t c, uint32_t m, int bits, int lane) {   // :63-65
-        x = (uint64_t)p * (x >> bits) + m - c;
-        if (x < ((uint64_t)1 << 32)) {
-            if (len <= 0) { err = BSW_E_UNDERFLOW; return; }
-            x = (x << 32) | pop_word(lane);
-        }
-    }
-};
 
 constexpr int RW = 16;       // warps per CTA in phase A: 512 threads x <=64 registers = half an SM's register file, so two
                              // of these CTAs fill an SM, or one of them sits beside one k_conv_wg CTA (codec.cu overlap)
@@ -114,13 +50,18 @@ __device__ __noinline__ uint32_t rows_exact_pm(const double *tile, int lane, int
     else if (lane > 0) p = bsw_cdf_fast(tile[(lane - 1) * STRIDE + NB - 1], m, s, rs);
     return __double2uint_rz(__dmul_rn(__dsub_rn(c, p), mult));
 }
+// the same for bin k of the row, endpoints read from global memory: the rare path of k_rows_wide
+__device__ __noinline__ uint32_t rows_exact_pm_g(const double *__restrict__ e, int k, int S, double m, double s, double rs, double mult) {
+    const double c = (k == S - 1) ? 1.0 : bsw_cdf_fast(__ldg(e + k), m, s, rs);    // (the row's last bin: cdf = 1, :184)
+    const double p = (k == 0) ? 0.0 : bsw_cdf_fast(__ldg(e + k - 1), m, s, rs);
+    return __double2uint_rz(__dmul_rn(__dsub_rn(c, p), mult));
+}
 
-// APX = true (default): every cdf value comes from the 15-instruction screening function bsw_cdf_apx; the pmf is formed
-// in 2^-20 fixed point with one FMA against a 2^52-type magic constant, and any bin whose scaled pmf lands within
-// BSW_APX_WINDOW of an integer boundary (about 1.2e-4 of them) is recomputed with the exact bsw_cdf_fast.  The integers
-// this kernel emits are therefore those of the exact function, which is what k_pop_coarse re-evaluates and what the
-// fused kernels produce.  APX = false (BSW_ROWS_EXACT=1) evaluates the exact function for every bin.
-template <int NB, bool POP, bool APX>
+// Every cdf value comes from the 15-instruction screening function bsw_cdf_apx; the pmf is formed in 2^-20 fixed point
+// with one FMA against a 2^52-type magic constant, and any bin whose scaled pmf lands within BSW_APX_WINDOW of an integer
+// boundary (about 1.2e-4 of them) is recomputed with the exact bsw_cdf_fast.  The integers this kernel emits are therefore
+// those of the exact function, which is what k_pop_coarse re-evaluates and what the fused kernels produce.
+template <int NB, bool POP>
 __global__ void __launch_bounds__(RW * 32, 2) k_rows(int count, int64_t L, const float *__restrict__ mu, int64_t mss,
         const float *__restrict__ sc, int64_t sss, const double *__restrict__ endp, int64_t ers,
         const int16_t *__restrict__ sym, int bits, int q, uint4 *__restrict__ pairs, uint32_t *__restrict__ coarse,
@@ -128,12 +69,12 @@ __global__ void __launch_bounds__(RW * 32, 2) k_rows(int count, int64_t L, const
     constexpr int S = 32 * NB;
     using RT = RowTile<NB>;
     __shared__ __align__(16) double tile[RT::DOUBLES];
-    __shared__ __align__(16) double t32[APX ? BSW_APX_TABLE_DOUBLES : 2];
+    __shared__ __align__(16) double t32[BSW_APX_TABLE_DOUBLES];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t row = blockIdx.x;                      // row index i within the level
     const int si = blockIdx.y * RW + warp;               // stream
     const double *e = endp + row * ers;
-    if (APX) bsw_apx_table_fill(t32, threadIdx.x, RW * 32);
+    bsw_apx_table_fill(t32, threadIdx.x, RW * 32);
     for (int k = threadIdx.x; k < S; k += RW * 32) tile[(k / NB) * RT::STRIDE + (k % NB)] = __ldg(e + k);
     __syncthreads();
     if (si >= count) return;
@@ -145,23 +86,16 @@ __global__ void __launch_bounds__(RW * 32, 2) k_rows(int count, int64_t L, const
     int sy = 0;
     if (!POP) sy = (int)sym[(int64_t)si * L + row];
     const int owner = sy / NB, js = sy - owner * NB;     // push: lane and in-lane position of the coded symbol
-
-    BswExpRegs K;
-    if (!APX) K.load();
     const double *my = tile + lane * RT::STRIDE;
     const uint32_t tl = smem_u32r(t32) + 8u * lane;
     // The screening cdf needs |t| <= 690 (its exponent arithmetic has no range checks).  Rows are sorted, so if both ends
     // of the row are inside that range for this stream's (mu, sigma) every bin is, and the three clamp instructions per
     // value are skipped (warp-uniform: a warp is one stream).  Needle-sharp x rows take the clamped loop.
-    bool wide = true;
-    if (APX && S > 2) {
-        const double t_lo = __dmul_rn(__dsub_rn(tile[0], m), rs);
-        const double t_hi = __dmul_rn(__dsub_rn(tile[((S - 2) / NB) * RT::STRIDE + ((S - 2) % NB)], m), rs);
-        wide = !(fabs(t_lo) <= 690.0 && fabs(t_hi) <= 690.0);
-    }
+    const double t_lo = __dmul_rn(__dsub_rn(tile[0], m), rs);
+    const double t_hi = __dmul_rn(__dsub_rn(tile[((S - 2) / NB) * RT::STRIDE + ((S - 2) % NB)], m), rs);
+    const bool wide = !(fabs(t_lo) <= 690.0 && fabs(t_hi) <= 690.0);
     auto cdf_at = [&](int j, auto clampc) -> double {
-        if (APX) return bsw_cdf_apx<decltype(clampc)::value>(my[j], m, rs, tl, KA);
-        return bsw_cdf_fast_regs(my[j], m, s, rs, K);
+        return bsw_cdf_apx<decltype(clampc)::value>(my[j], m, rs, tl, KA);
     };
     // cdf at my last endpoint first: the next lane needs it as the lower neighbour of its first bin.  The row's very
     // last entry is the +1e300 pad: t clamps to +690 and the cdf comes out as exactly 1.0, the reference's
@@ -184,23 +118,19 @@ __global__ void __launch_bounds__(RW * 32, 2) k_rows(int count, int64_t L, const
 #pragma unroll
         for (int t = 0; t < G; ++t) {
             const double c = (decltype(last_group)::value && t == G - 1) ? c_last : cdf_at(j0 + t, clampc);
-            if (APX) {
-                // z = 1.5*2^52 + WINDOW + pmf*2^20: the mantissa of z holds the fixed-point pmf, shifted by WINDOW so that
-                // "low 20 bits < 2*WINDOW" means "within WINDOW of a truncation boundary".  The funnel shift drops the low
-                // 20 bits; what remains is the integer pmf with the 2^51 magic bit on top (bit 31).
-                const double z = __fma_rn(__dsub_rn(c, prev), mult2, magic2);
-                const uint32_t raw = __funnelshift_r((uint32_t)__double2loint(z), (uint32_t)__double2hiint(z), 20);
-                // a pmf that truncates to 0 needs no second look: the exact value then lies in (-1, 1) as well
-                doubt[t] = ((uint32_t)__double2loint(z) & (0xfffffu & ~(2u * BSW_APX_WINDOW - 1u))) == 0u && raw != 0x80000000u;
-                any |= doubt[t];
-                all_hi &= raw;                            // bit 31 clear = negative pmf (unsorted endpoints): exact path
-                vv[t] = raw + 0x80000001u;                                                 // :29 trunc, :32 +1
-            } else {
-                vv[t] = __double2uint_rz(__dmul_rn(__dsub_rn(c, prev), mult)) + 1u;
-            }
+            // z = 1.5*2^52 + WINDOW + pmf*2^20: the mantissa of z holds the fixed-point pmf, shifted by WINDOW so that
+            // "low 20 bits < 2*WINDOW" means "within WINDOW of a truncation boundary".  The funnel shift drops the low
+            // 20 bits; what remains is the integer pmf with the 2^51 magic bit on top (bit 31).
+            const double z = __fma_rn(__dsub_rn(c, prev), mult2, magic2);
+            const uint32_t raw = __funnelshift_r((uint32_t)__double2loint(z), (uint32_t)__double2hiint(z), 20);
+            // a pmf that truncates to 0 needs no second look: the exact value then lies in (-1, 1) as well
+            doubt[t] = ((uint32_t)__double2loint(z) & (0xfffffu & ~(2u * BSW_APX_WINDOW - 1u))) == 0u && raw != 0x80000000u;
+            any |= doubt[t];
+            all_hi &= raw;                                // bit 31 clear = negative pmf (unsorted endpoints): exact path
+            vv[t] = raw + 0x80000001u;                                                     // :29 trunc, :32 +1
             prev = c;
         }
-        if (APX && (any || !(all_hi & 0x80000000u))) {
+        if (any || !(all_hi & 0x80000000u)) {
             const bool all = !(all_hi & 0x80000000u);
 #pragma unroll
             for (int t = 0; t < G; ++t)
@@ -238,11 +168,7 @@ __global__ void __launch_bounds__(RW * 32, 2) k_rows(int count, int64_t L, const
     int lbi = bestj0;                                     // first position of the maximum inside its group
 #pragma unroll
     for (int t = G - 1; t >= 0; --t) if (bestv[t] == lbest) lbi = bestj0 + t;
-    uint32_t incl = lsum;
-    for (int o = 1; o < 32; o <<= 1) {
-        uint32_t t = __shfl_up_sync(FULL, incl, o);
-        if (lane >= o) incl += t;
-    }
+    const uint32_t incl = warp_incl_scan_u32(lsum, lane);
     const uint32_t total = __shfl_sync(FULL, incl, 31);
     // :35 first maximum of the row: lanes own ascending blocks, so it is the lowest lane that holds the row maximum
     const uint32_t rowmax = __reduce_max_sync(FULL, lbest);
@@ -267,141 +193,14 @@ __global__ void __launch_bounds__(RW * 32, 2) k_rows(int count, int64_t L, const
     }
 }
 
-// ---- phase B: push -------------------------------------------------------------------------------------------------
-constexpr int BW = 4;
-// MASK: pixel level with block extents (bsw_x_live); the 32 rows of a block are one image row, so the coded ones are a prefix
-template <bool MASK>
-__global__ void __launch_bounds__(BW * 32) k_push_pairs(bsw_streams sv, int first, int count, const uint4 *__restrict__ pairs,
-                                                        int64_t L, int bits, const int16_t *__restrict__ ext) {
-    const int lane = threadIdx.x & 31;
-    const int si = blockIdx.x * BW + (threadIdx.x >> 5);
-    if (si >= count) return;
-    const int b = first + si;
-    WarpStream2 ws;
-    ws.open(sv, b);
-    if (ws.err) return;
-    int vh = 32, vw = 32;
-    if (MASK) { vh = ext[2 * si]; vw = ext[2 * si + 1]; }
-    ws.push_begin(lane);
-    const uint4 *pp = pairs + (int64_t)si * L;
-    uint4 nxt = (lane < L) ? __ldg(pp + lane) : make_uint4(1, 0, 0xffffffffu, 0xffffffffu);
-    for (int64_t i0 = 0; i0 < L && !ws.err; i0 += 32) {
-        uint4 cur = nxt;
-        int64_t r = i0 + 32 + lane;
-        if (r < L) nxt = __ldg(pp + r);                   // prefetch the next 32 rows
-        int n = (int)min((int64_t)32, L - i0);
-        if (MASK) n = (int)((i0 >> 5) & 31) < vh ? min(n, vw) : 0;
-        for (int j = 0; j < n && !ws.err; ++j) {
-            uint64_t M = ((uint64_t)__shfl_sync(FULL, cur.w, j) << 32) | __shfl_sync(FULL, cur.z, j);
-            const uint32_t pj = __shfl_sync(FULL, cur.x, j);
-            if (pj == 0u) { ws.err = BSW_E_INVALID; break; }     // phase A saw a symbol outside the support (reference: IndexError)
-            ws.encode_magic(pj, __shfl_sync(FULL, cur.y, j), M, bits, lane);
-        }
-    }
-    ws.push_end(lane);
-    ws.close(sv, b, lane);
-}
-
-// ---- phase B: pop ----------------------------------------------------------------------------------------------------
-template <int NB, bool MASK>
-__global__ void __launch_bounds__(BW * 32) k_pop_coarse(bsw_streams sv, int first, int count, const float *__restrict__ mu,
-        int64_t mss, const float *__restrict__ sc, int64_t sss, const double *__restrict__ endp, int64_t ers,
-        const uint32_t *__restrict__ coarse, const uint2 *__restrict__ fix, int16_t *__restrict__ sym, int64_t L,
-        int bits, int q, const int16_t *__restrict__ ext) {
-    const int lane = threadIdx.x & 31;
-    const int si = blockIdx.x * BW + (threadIdx.x >> 5);
-    if (si >= count) return;
-    const int b = first + si;
-    WarpStream2 ws;
-    ws.open(sv, b);
-    if (ws.err) return;
-    int vh = 32, vw = 32;
-    if (MASK) { vh = ext[2 * si]; vw = ext[2 * si + 1]; }
-    constexpr int S = 32 * NB;
-    const float *mub = mu + (int64_t)si * mss, *scb = sc + (int64_t)si * sss;
-    const uint32_t *cb = coarse + (int64_t)si * L * NB;
-    const uint2 *fb = fix + (int64_t)si * L;
-    int16_t *sy = sym + (int64_t)si * L;
-    const double mult = (double)(((int64_t)1 << bits) - ((int64_t)1 << q));
-    const uint32_t mask = (uint32_t)(((uint64_t)1 << bits) - 1);
-
-    float mu_w = 0.f, sc_w = 1.f;
-    uint2 fx_w = make_uint2(0, 0);
-    int my_sym = 0;
-    // per-row scalars (mu, sigma, argmax, remnant) of a block of 32 rows, loaded one block ahead of their use
-    float mu_nx, sc_nx;
-    uint2 fx_nx;
-    {
-        int64_t r = ((L - 1) & ~(int64_t)31) + lane;
-        mu_nx = r < L ? mub[r] : 0.f;
-        sc_nx = r < L ? scb[r] : 1.f;
-        fx_nx = r < L ? __ldg(fb + r) : make_uint2(0, 0);
-    }
-    // coarse cdf rows are independent of the head: keep the loads two rows ahead of their use.  (They are issued AFTER
-    // the per-row shuffles below: the first version issued the load first and ncu showed every row stalling ~700 cycles
-    // on that load's scoreboard at the first shuffle.)
-    uint32_t base_n1 = (lane < NB) ? __ldg(cb + (L - 1) * NB + lane) : 0xffffffffu;
-    uint32_t base_n2 = (lane < NB && L > 1) ? __ldg(cb + (L - 2) * NB + lane) : 0xffffffffu;
-    for (int64_t i = L - 1; i >= 0; --i) {
-        const int j32 = (int)(i & 31);
-        const bool new_block = (j32 == 31 || i == L - 1);
-        if (new_block) { mu_w = mu_nx; sc_w = sc_nx; fx_w = fx_nx; }
-        const double m_ = (double)__shfl_sync(FULL, mu_w, j32), s_ = (double)__shfl_sync(FULL, sc_w, j32);
-        const int bi = (int)__shfl_sync(FULL, fx_w.x, j32);
-        const uint32_t rem = __shfl_sync(FULL, fx_w.y, j32);
-        if (new_block) {                                  // the block below this one
-            int64_t r = (i & ~(int64_t)31) - 32 + lane;
-            mu_nx = r >= 0 ? mub[r] : 0.f;
-            sc_nx = r >= 0 ? scb[r] : 1.f;
-            fx_nx = r >= 0 ? __ldg(fb + r) : make_uint2(0, 0);
-        }
-        const uint32_t base = base_n1;
-        base_n1 = base_n2;
-        if (i > 1) base_n2 = (lane < NB) ? __ldg(cb + (i - 2) * NB + lane) : 0xffffffffu;
-        if (!MASK || bsw_x_live(i, vh, vw)) {             // a masked dim leaves the head alone; its symbol is padded later
-            const double rs = __ddiv_rn(1.0, s_);
-            const uint32_t mm = (uint32_t)ws.x & mask;                                   // cifar_compress.py:60
-            const int chunk = 31 - __clz(__ballot_sync(FULL, base <= mm));               // base of lanes >= NB is UINT_MAX
-            const int k = chunk * 32 + lane;
-            const double *e = endp + i * ers;
-            // two independent cdf evaluations per lane (upper and lower endpoint of my bin)
-            double c_hi = (k == S - 1) ? 1.0 : bsw_cdf_fast(__ldg(e + k), m_, s_, rs);
-            double c_lo = (k == 0) ? 0.0 : bsw_cdf_fast(__ldg(e + k - 1), m_, s_, rs);
-            uint32_t v = __double2uint_rz(__dmul_rn(__dsub_rn(c_hi, c_lo), mult)) + 1u + (k == bi ? rem : 0u);
-            uint32_t incl = v;
-            for (int o = 1; o < 32; o <<= 1) {
-                uint32_t t = __shfl_up_sync(FULL, incl, o);
-                if (lane >= o) incl += t;
-            }
-            const uint32_t cex = __shfl_sync(FULL, base, chunk) + incl - v;              // integer cdf at my bin
-            const int js = 31 - __clz(__ballot_sync(FULL, cex <= mm));                   // :61 searchsorted 'right' - 1
-            const uint32_t ps = __shfl_sync(FULL, v, js), cs = __shfl_sync(FULL, cex, js);
-            if (lane == j32) my_sym = chunk * 32 + js;                                   // :62
-            ws.decode(ps, cs, mm, bits, lane);                                           // :63-65
-        }
-        if (j32 == 0 || ws.err) {
-            int64_t r = (i & ~(int64_t)31) + lane;
-            if (r < L && r >= i) sy[r] = (int16_t)my_sym;
-            if (ws.err) break;
-        }
-    }
-    ws.close(sv, b, lane);
-}
-
 // ---- wide supports (S = 32 * 32 * NP = 2048 or 4096: quantbits 11 and 12) ----------------------------------------------
 // A lane cannot keep NB = S/32 = 64 or 128 float64 endpoints in registers, and 128 chunk bases per row would make the pop
 // scratch four times larger.  So lane l owns the pop chunk l -- the CH = S/32 consecutive bins [l*CH, l*CH + CH) -- and walks
 // it in NP passes of 32 bins.  Pass p stages the 32 x 32 endpoints {l*CH + p*32 + j} into the same padded tile as k_rows<32>,
 // runs the same 4-bin groups on them and carries the lane's running sum, its first maximum and (push) its prefix below the
 // symbol into the next pass.  The screening test and the exact fallback are those of k_rows; the chunk bases are the
-// lane-exclusive prefix sums, 32 per row as for S <= 1024.
-__device__ __noinline__ uint32_t rows_exact_pm_g(const double *__restrict__ e, int k, int S, double m, double s, double rs, double mult) {
-    const double c = (k == S - 1) ? 1.0 : bsw_cdf_fast(__ldg(e + k), m, s, rs);    // (the row's last bin: cdf = 1, :184)
-    const double p = (k == 0) ? 0.0 : bsw_cdf_fast(__ldg(e + k - 1), m, s, rs);
-    return __double2uint_rz(__dmul_rn(__dsub_rn(c, p), mult));
-}
-
-template <int NP, bool POP, bool APX>
+// lane-exclusive prefix sums, 32 per row as for S = 1024.
+template <int NP, bool POP>
 __global__ void __launch_bounds__(RW * 32, 2) k_rows_wide(int count, int64_t L, const float *__restrict__ mu, int64_t mss,
         const float *__restrict__ sc, int64_t sss, const double *__restrict__ endp, int64_t ers,
         const int16_t *__restrict__ sym, int bits, int q, uint4 *__restrict__ pairs, uint32_t *__restrict__ coarse,
@@ -412,13 +211,13 @@ __global__ void __launch_bounds__(RW * 32, 2) k_rows_wide(int count, int64_t L, 
     constexpr int G = 4;
     using RT = RowTile<NB>;
     __shared__ __align__(16) double tile[RT::DOUBLES];
-    __shared__ __align__(16) double t32[APX ? BSW_APX_TABLE_DOUBLES : 2];
+    __shared__ __align__(16) double t32[BSW_APX_TABLE_DOUBLES];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t row = blockIdx.x;
     const int si = blockIdx.y * RW + warp;
     const bool live = si < count;                        // every warp stages every pass: no warp leaves before the last barrier
     const double *e = endp + row * ers;
-    if (APX) bsw_apx_table_fill(t32, threadIdx.x, RW * 32);
+    bsw_apx_table_fill(t32, threadIdx.x, RW * 32);
     const double m = live ? (double)mu[(int64_t)si * mss + row] : 0.0, s = live ? (double)sc[(int64_t)si * sss + row] : 1.0;
     const double rs = __ddiv_rn(1.0, s);
     const double mult = (double)(((int64_t)1 << bits) - ((int64_t)1 << q));
@@ -427,24 +226,18 @@ __global__ void __launch_bounds__(RW * 32, 2) k_rows_wide(int count, int64_t L, 
     int sy = 0;
     if (!POP && live) sy = (int)sym[(int64_t)si * L + row];
     const int owner = sy / CH, js = sy - owner * CH;     // push: lane and in-chunk position of the coded symbol
-
-    BswExpRegs K;
-    if (!APX) K.load();
     const double *my = tile + lane * RT::STRIDE;
     const uint32_t tl = smem_u32r(t32) + 8u * lane;
-    bool wide = true;                                    // (|t| > 690 somewhere in the row: the clamped loop, as in k_rows)
-    if (APX) {
-        const double t_lo = __dmul_rn(__dsub_rn(__ldg(e), m), rs);
-        const double t_hi = __dmul_rn(__dsub_rn(__ldg(e + S - 2), m), rs);
-        wide = !(fabs(t_lo) <= 690.0 && fabs(t_hi) <= 690.0);
-    }
+    // |t| > 690 somewhere in the row: the clamped loop, as in k_rows
+    const double t_lo = __dmul_rn(__dsub_rn(__ldg(e), m), rs);
+    const double t_hi = __dmul_rn(__dsub_rn(__ldg(e + S - 2), m), rs);
+    const bool wide = !(fabs(t_lo) <= 690.0 && fabs(t_hi) <= 690.0);
     auto cdf_at = [&](int j, auto clampc) -> double {
-        if (APX) return bsw_cdf_apx<decltype(clampc)::value>(my[j], m, rs, tl, KA);
-        return bsw_cdf_fast_regs(my[j], m, s, rs, K);
+        return bsw_cdf_apx<decltype(clampc)::value>(my[j], m, rs, tl, KA);
     };
     // lower edge of my first bin: the upper endpoint of the previous lane's chunk, evaluated from global memory
     double prev = 0.0;
-    if (lane > 0) prev = APX ? bsw_cdf_apx<true>(__ldg(e + lane * CH - 1), m, rs, tl, KA) : bsw_cdf_fast_regs(__ldg(e + lane * CH - 1), m, s, rs, K);
+    if (lane > 0) prev = bsw_cdf_apx<true>(__ldg(e + lane * CH - 1), m, rs, tl, KA);
     uint32_t lsum = 0, lbest = 0, pre = 0, pv = 0;
     uint32_t bestv[G];
     int bestj0 = 0;
@@ -468,19 +261,15 @@ __global__ void __launch_bounds__(RW * 32, 2) k_rows_wide(int count, int64_t L, 
             for (int t = 0; t < G; ++t) {
                 double c = cdf_at(j0 + t, clampc);
                 if (t == G - 1 && row_end && j0 + t == NB - 1) c = 1.0;
-                if (APX) {
-                    const double z = __fma_rn(__dsub_rn(c, prev), mult2, magic2);
-                    const uint32_t raw = __funnelshift_r((uint32_t)__double2loint(z), (uint32_t)__double2hiint(z), 20);
-                    doubt[t] = ((uint32_t)__double2loint(z) & (0xfffffu & ~(2u * BSW_APX_WINDOW - 1u))) == 0u && raw != 0x80000000u;
-                    any |= doubt[t];
-                    all_hi &= raw;
-                    vv[t] = raw + 0x80000001u;                                             // :29 trunc, :32 +1
-                } else {
-                    vv[t] = __double2uint_rz(__dmul_rn(__dsub_rn(c, prev), mult)) + 1u;
-                }
+                const double z = __fma_rn(__dsub_rn(c, prev), mult2, magic2);
+                const uint32_t raw = __funnelshift_r((uint32_t)__double2loint(z), (uint32_t)__double2hiint(z), 20);
+                doubt[t] = ((uint32_t)__double2loint(z) & (0xfffffu & ~(2u * BSW_APX_WINDOW - 1u))) == 0u && raw != 0x80000000u;
+                any |= doubt[t];
+                all_hi &= raw;
+                vv[t] = raw + 0x80000001u;                                                 // :29 trunc, :32 +1
                 prev = c;
             }
-            if (APX && (any || !(all_hi & 0x80000000u))) {
+            if (any || !(all_hi & 0x80000000u)) {
                 const bool all = !(all_hi & 0x80000000u);
 #pragma unroll
                 for (int t = 0; t < G; ++t)
@@ -518,11 +307,7 @@ __global__ void __launch_bounds__(RW * 32, 2) k_rows_wide(int count, int64_t L, 
     int lbi = bestj0;
 #pragma unroll
     for (int t = G - 1; t >= 0; --t) if (bestv[t] == lbest) lbi = bestj0 + t;
-    uint32_t incl = lsum;
-    for (int o = 1; o < 32; o <<= 1) {
-        uint32_t t = __shfl_up_sync(FULL, incl, o);
-        if (lane >= o) incl += t;
-    }
+    const uint32_t incl = warp_incl_scan_u32(lsum, lane);
     const uint32_t total = __shfl_sync(FULL, incl, 31);
     const uint32_t rowmax = __reduce_max_sync(FULL, lbest);
     const int wl = __ffs(__ballot_sync(FULL, lbest == rowmax)) - 1;
@@ -544,32 +329,78 @@ __global__ void __launch_bounds__(RW * 32, 2) k_rows_wide(int count, int64_t L, 
     }
 }
 
-// Pop of the wide generic rows: the ballot over the 32 chunk bases picks the chunk, which is then walked in sub-chunks of
-// 32 bins with the cdf carried between them (same per-bin arithmetic as k_pop_coarse).
-template <int NP, bool MASK>
-__global__ void __launch_bounds__(BW * 32) k_pop_coarse_wide(bsw_streams sv, int first, int count, const float *__restrict__ mu,
-        int64_t mss, const float *__restrict__ sc, int64_t sss, const double *__restrict__ endp, int64_t ers,
-        const uint32_t *__restrict__ coarse, const uint2 *__restrict__ fix, int16_t *__restrict__ sym, int64_t L,
-        int bits, int q, const int16_t *__restrict__ ext) {
-    constexpr int CH = 32 * NP, S = 32 * CH;
+
+template <int NB, bool POP>
+auto rows_kernel() {
+    if constexpr (NB <= 32) return k_rows<NB, POP>;
+    else return k_rows_wide<NB / 32, POP>;
+}
+
+// ---- phase B: push -------------------------------------------------------------------------------------------------
+constexpr int BW = 4;
+// MASK: pixel level with block extents (bsw_x_live); the 32 rows of a block are one image row, so the coded ones are a prefix
+template <bool MASK>
+__global__ void __launch_bounds__(BW * 32) k_push_pairs(bsw_streams sv, int first, int count, const uint4 *__restrict__ pairs,
+                                                        int64_t L, int bits, const int16_t *__restrict__ ext) {
     const int lane = threadIdx.x & 31;
     const int si = blockIdx.x * BW + (threadIdx.x >> 5);
     if (si >= count) return;
     const int b = first + si;
-    WarpStream2 ws;
+    WarpStream ws;
+    ws.open(sv, b);
+    if (ws.err) return;
+    int vh = 32, vw = 32;
+    if (MASK) { vh = ext[2 * si]; vw = ext[2 * si + 1]; }
+    ws.push_begin(lane);
+    const uint4 *pp = pairs + (int64_t)si * L;
+    uint4 nxt = (lane < L) ? __ldg(pp + lane) : make_uint4(1, 0, 0xffffffffu, 0xffffffffu);
+    for (int64_t i0 = 0; i0 < L && !ws.err; i0 += 32) {
+        uint4 cur = nxt;
+        int64_t r = i0 + 32 + lane;
+        if (r < L) nxt = __ldg(pp + r);                   // prefetch the next 32 rows
+        int n = (int)min((int64_t)32, L - i0);
+        if (MASK) n = (int)((i0 >> 5) & 31) < vh ? min(n, vw) : 0;
+        for (int j = 0; j < n && !ws.err; ++j) {
+            uint64_t M = ((uint64_t)__shfl_sync(FULL, cur.w, j) << 32) | __shfl_sync(FULL, cur.z, j);
+            const uint32_t pj = __shfl_sync(FULL, cur.x, j);
+            if (pj == 0u) { ws.err = BSW_E_INVALID; break; }     // phase A saw a symbol outside the support (reference: IndexError)
+            ws.encode_magic(pj, __shfl_sync(FULL, cur.y, j), M, bits, lane);
+        }
+    }
+    ws.push_end(lane);
+    ws.close(sv, b, lane);
+}
+
+// ---- phase B: pop ----------------------------------------------------------------------------------------------------
+// Rows of S = 32 NB bins are searched in chunks: 32 chunks of NB bins from 1024 bins up, NB chunks of 32 bins below.
+template <int NB> __host__ __device__ constexpr int chunks_per_row() { return NB < 32 ? NB : 32; }
+
+template <int NB, bool MASK>
+__global__ void __launch_bounds__(BW * 32) k_pop_coarse(bsw_streams sv, int first, int count, const float *__restrict__ mu,
+        int64_t mss, const float *__restrict__ sc, int64_t sss, const double *__restrict__ endp, int64_t ers,
+        const uint32_t *__restrict__ coarse, const uint2 *__restrict__ fix, int16_t *__restrict__ sym, int64_t L,
+        int bits, int q, const int16_t *__restrict__ ext) {
+    constexpr int S = 32 * NB, NBASE = chunks_per_row<NB>(), CH = S / NBASE, NP = CH / 32;  // chunks, bins per chunk, sub-chunks
+    const int lane = threadIdx.x & 31;
+    const int si = blockIdx.x * BW + (threadIdx.x >> 5);
+    if (si >= count) return;
+    const int b = first + si;
+    WarpStream ws;
     ws.open(sv, b);
     if (ws.err) return;
     int vh = 32, vw = 32;
     if (MASK) { vh = ext[2 * si]; vw = ext[2 * si + 1]; }
     const float *mub = mu + (int64_t)si * mss, *scb = sc + (int64_t)si * sss;
-    const uint32_t *cb = coarse + (int64_t)si * L * 32;
+    const uint32_t *cb = coarse + (int64_t)si * L * NBASE;
     const uint2 *fb = fix + (int64_t)si * L;
     int16_t *sy = sym + (int64_t)si * L;
     const double mult = (double)(((int64_t)1 << bits) - ((int64_t)1 << q));
     const uint32_t mask = (uint32_t)(((uint64_t)1 << bits) - 1);
+
     float mu_w = 0.f, sc_w = 1.f;
     uint2 fx_w = make_uint2(0, 0);
     int my_sym = 0;
+    // per-row scalars (mu, sigma, argmax, remnant) of a block of 32 rows, loaded one block ahead of their use
     float mu_nx, sc_nx;
     uint2 fx_nx;
     {
@@ -578,8 +409,11 @@ __global__ void __launch_bounds__(BW * 32) k_pop_coarse_wide(bsw_streams sv, int
         sc_nx = r < L ? scb[r] : 1.f;
         fx_nx = r < L ? __ldg(fb + r) : make_uint2(0, 0);
     }
-    uint32_t base_n1 = __ldg(cb + (L - 1) * 32 + lane);
-    uint32_t base_n2 = L > 1 ? __ldg(cb + (L - 2) * 32 + lane) : 0xffffffffu;
+    // chunk bases are independent of the head: keep the loads two rows ahead of their use.  (They are issued AFTER the
+    // per-row shuffles below: the first version issued the load first and ncu showed every row stalling ~700 cycles on
+    // that load's scoreboard at the first shuffle.)
+    uint32_t base_n1 = (lane < NBASE) ? __ldg(cb + (L - 1) * NBASE + lane) : 0xffffffffu;
+    uint32_t base_n2 = (lane < NBASE && L > 1) ? __ldg(cb + (L - 2) * NBASE + lane) : 0xffffffffu;
     for (int64_t i = L - 1; i >= 0; --i) {
         const int j32 = (int)(i & 31);
         const bool new_block = (j32 == 31 || i == L - 1);
@@ -587,7 +421,7 @@ __global__ void __launch_bounds__(BW * 32) k_pop_coarse_wide(bsw_streams sv, int
         const double m_ = (double)__shfl_sync(FULL, mu_w, j32), s_ = (double)__shfl_sync(FULL, sc_w, j32);
         const int bi = (int)__shfl_sync(FULL, fx_w.x, j32);
         const uint32_t rem = __shfl_sync(FULL, fx_w.y, j32);
-        if (new_block) {
+        if (new_block) {                                  // the block below this one
             int64_t r = (i & ~(int64_t)31) - 32 + lane;
             mu_nx = r >= 0 ? mub[r] : 0.f;
             sc_nx = r >= 0 ? scb[r] : 1.f;
@@ -595,39 +429,52 @@ __global__ void __launch_bounds__(BW * 32) k_pop_coarse_wide(bsw_streams sv, int
         }
         const uint32_t base = base_n1;
         base_n1 = base_n2;
-        if (i > 1) base_n2 = __ldg(cb + (i - 2) * 32 + lane);
-        if (!MASK || bsw_x_live(i, vh, vw)) {
+        if (i > 1) base_n2 = (lane < NBASE) ? __ldg(cb + (i - 2) * NBASE + lane) : 0xffffffffu;
+        if (!MASK || bsw_x_live(i, vh, vw)) {             // a masked dim leaves the head alone; its symbol is padded later
             const double rs = __ddiv_rn(1.0, s_);
             const uint32_t mm = (uint32_t)ws.x & mask;                                   // cifar_compress.py:60
-            const int chunk = 31 - __clz(__ballot_sync(FULL, base <= mm));
-            const double *e = endp + i * ers;
-            uint32_t carry = __shfl_sync(FULL, base, chunk), ps = 1u, cs = 0u;
-            int s = 0;
+            const int chunk = 31 - __clz(__ballot_sync(FULL, base <= mm));               // base of lanes >= NBASE is UINT_MAX
+            if constexpr (NP == 1) {
+                const int k = chunk * 32 + lane;
+                const double *e = endp + i * ers;
+                // two independent cdf evaluations per lane (upper and lower endpoint of my bin)
+                double c_hi = (k == S - 1) ? 1.0 : bsw_cdf_fast(__ldg(e + k), m_, s_, rs);
+                double c_lo = (k == 0) ? 0.0 : bsw_cdf_fast(__ldg(e + k - 1), m_, s_, rs);
+                uint32_t v = __double2uint_rz(__dmul_rn(__dsub_rn(c_hi, c_lo), mult)) + 1u + (k == bi ? rem : 0u);
+                uint32_t incl = warp_incl_scan_u32(v, lane);
+                const uint32_t cex = __shfl_sync(FULL, base, chunk) + incl - v;          // integer cdf at my bin
+                const int js = 31 - __clz(__ballot_sync(FULL, cex <= mm));               // :61 searchsorted 'right' - 1
+                const uint32_t ps = __shfl_sync(FULL, v, js), cs = __shfl_sync(FULL, cex, js);
+                if (lane == j32) my_sym = chunk * 32 + js;                               // :62
+                ws.decode(ps, cs, mm, bits, lane);                                       // :63-65
+            } else {
+                // the chunk is walked in sub-chunks of 32 bins with the cdf carried between them: the symbol lies in the
+                // first sub-chunk whose successor starts above mm (or in the chunk's last one)
+                const double *e = endp + i * ers;
+                uint32_t carry = __shfl_sync(FULL, base, chunk), ps = 1u, cs = 0u;
+                int s = 0;
 #pragma unroll 1
-            for (int sub = 0; sub < NP; ++sub) {
-                const int k = chunk * CH + sub * 32 + lane;
-                const double c_hi = (k == S - 1) ? 1.0 : bsw_cdf_fast(__ldg(e + k), m_, s_, rs);
-                const double c_lo = (k == 0) ? 0.0 : bsw_cdf_fast(__ldg(e + k - 1), m_, s_, rs);
-                const uint32_t v = __double2uint_rz(__dmul_rn(__dsub_rn(c_hi, c_lo), mult)) + 1u + (k == bi ? rem : 0u);
-                uint32_t incl = v;
-                for (int o = 1; o < 32; o <<= 1) {
-                    uint32_t t = __shfl_up_sync(FULL, incl, o);
-                    if (lane >= o) incl += t;
+                for (int sub = 0; sub < NP; ++sub) {
+                    const int k = chunk * CH + sub * 32 + lane;
+                    const double c_hi = (k == S - 1) ? 1.0 : bsw_cdf_fast(__ldg(e + k), m_, s_, rs);
+                    const double c_lo = (k == 0) ? 0.0 : bsw_cdf_fast(__ldg(e + k - 1), m_, s_, rs);
+                    const uint32_t v = __double2uint_rz(__dmul_rn(__dsub_rn(c_hi, c_lo), mult)) + 1u + (k == bi ? rem : 0u);
+                    uint32_t incl = warp_incl_scan_u32(v, lane);
+                    const uint32_t cex = carry + incl - v;
+                    const uint32_t next = carry + __shfl_sync(FULL, incl, 31);
+                    if (sub == NP - 1 || next > mm) {
+                        const int js = 31 - __clz(__ballot_sync(FULL, cex <= mm));       // :61 searchsorted 'right' - 1
+                        ps = __shfl_sync(FULL, v, js); cs = __shfl_sync(FULL, cex, js);
+                        s = chunk * CH + sub * 32 + js;
+                        break;
+                    }
+                    carry = next;
                 }
-                const uint32_t cex = carry + incl - v;
-                const uint32_t next = carry + __shfl_sync(FULL, incl, 31);
-                if (sub == NP - 1 || next > mm) {                                        // the symbol is in this sub-chunk
-                    const int js = 31 - __clz(__ballot_sync(FULL, cex <= mm));           // :61 searchsorted 'right' - 1
-                    ps = __shfl_sync(FULL, v, js); cs = __shfl_sync(FULL, cex, js);
-                    s = chunk * CH + sub * 32 + js;
-                    break;
-                }
-                carry = next;
+                if (lane == j32) my_sym = s;                                             // :62
+                ws.decode(ps, cs, mm, bits, lane);                                       // :63-65
             }
-            if (lane == j32) my_sym = s;                                                 // :62
-            ws.decode(ps, cs, mm, bits, lane);                                           // :63-65
         }
-        if (j32 == 0 || ws.err) {
+        if (j32 == 0 || ws.err) {                         // block of rows done: coalesced symbol store
             int64_t r = (i & ~(int64_t)31) + lane;
             if (r < L && r >= i) sy[r] = (int16_t)my_sym;
             if (ws.err) break;
@@ -648,7 +495,7 @@ __global__ void __launch_bounds__(BW * 32) k_pop_full(bsw_streams sv, int first,
     const int si = blockIdx.x * BW + (threadIdx.x >> 5);
     if (si >= count) return;
     const int b = first + si;
-    WarpStream2 ws;
+    WarpStream ws;
     ws.open(sv, b);
     if (ws.err) return;
     constexpr int S = 32 * NB;
@@ -683,11 +530,7 @@ __global__ void __launch_bounds__(BW * 32) k_pop_full(bsw_streams sv, int first,
         const int chunk = 31 - __clz(__ballot_sync(FULL, base <= mm));
         const int k = chunk * 32 + lane;
         uint32_t v = __ldg(pb + i * S + k) + (k == bi ? rem : 0u);
-        uint32_t incl = v;
-        for (int o = 1; o < 32; o <<= 1) {
-            uint32_t t = __shfl_up_sync(FULL, incl, o);
-            if (lane >= o) incl += t;
-        }
+        uint32_t incl = warp_incl_scan_u32(v, lane);
         const uint32_t cex = __shfl_sync(FULL, base, chunk) + incl - v;
         const int js = 31 - __clz(__ballot_sync(FULL, cex <= mm));                       // :61
         const uint32_t ps = __shfl_sync(FULL, v, js), cs = __shfl_sync(FULL, cex, js);
@@ -702,14 +545,6 @@ __global__ void __launch_bounds__(BW * 32) k_pop_full(bsw_streams sv, int first,
     ws.close(sv, b, lane);
 }
 
-template <int NB>
-int launch_pop_full(bsw_streams *s, int first, int count, const uint32_t *pfull, const uint32_t *coarse, const uint2 *fix,
-                    int16_t *sym, int64_t L, int bits, int shared_tables, cudaStream_t st) {
-    k_pop_full<NB><<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, pfull, coarse, fix, sym, L, bits, shared_tables);
-    BSW_LAUNCH_CHECK();
-    return BSW_OK;
-}
-
 int launch_push_pairs(bsw_streams *s, int first, int count, const void *scratch, int64_t L, int bits, const int16_t *ext,
                       cudaStream_t st) {
     BSW_MAX_SHARED_ONCE(k_push_pairs<false>); BSW_MAX_SHARED_ONCE(k_push_pairs<true>);
@@ -719,66 +554,22 @@ int launch_push_pairs(bsw_streams *s, int first, int count, const void *scratch,
     return BSW_OK;
 }
 
+// S = 32 NB for NB = 1, 2, ..., 128
 template <int NB>
 int launch_rows(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
                 int64_t sss, const double *endp, int64_t ers, int16_t *sym, int64_t L, int bits, int q, void *scratch,
                 const int16_t *ext, cudaStream_t st) {
-    dim3 grid((unsigned)L, (count + RW - 1) / RW);
-    // pop scratch layout: [coarse: count*L*NB u32, rounded up to 8 bytes] [fix: count*L uint2]
-    uint4 *pairs = (uint4 *)scratch;
-    uint32_t *coarse = (uint32_t *)scratch;
-    uint2 *fix = (uint2 *)((uint8_t *)scratch + (((size_t)count * L * NB * 4 + 7) & ~(size_t)7));
-    const BswApxRegs kp = bsw_apx_params();
-    // BSW_ROWS_EXACT=1: evaluate the exact cdf for every bin instead of screening with bsw_cdf_apx (A/B switch; same output)
-    static const bool env_exact = getenv("BSW_ROWS_EXACT") && getenv("BSW_ROWS_EXACT")[0] == '1';
-    const bool exact = bits > 31 || env_exact;
-    BSW_MAX_SHARED_ONCE((k_rows<NB, true, false>)); BSW_MAX_SHARED_ONCE((k_rows<NB, true, true>));
-    BSW_MAX_SHARED_ONCE((k_rows<NB, false, false>)); BSW_MAX_SHARED_ONCE((k_rows<NB, false, true>));
+    const RowsScratch scr(scratch, count, L);
+    BSW_MAX_SHARED_ONCE((rows_kernel<NB, true>())); BSW_MAX_SHARED_ONCE((rows_kernel<NB, false>()));
     BSW_MAX_SHARED_ONCE((k_pop_coarse<NB, false>)); BSW_MAX_SHARED_ONCE((k_pop_coarse<NB, true>));
     if (phase == 0) {
-        if (pop) {
-            if (exact) k_rows<NB, true, false><<<grid, RW * 32, 0, st>>>(count, L, mu, mss, sc, sss, endp, ers, nullptr, bits, q, nullptr, coarse, fix, kp);
-            else k_rows<NB, true, true><<<grid, RW * 32, 0, st>>>(count, L, mu, mss, sc, sss, endp, ers, nullptr, bits, q, nullptr, coarse, fix, kp);
-        } else {
-            if (exact) k_rows<NB, false, false><<<grid, RW * 32, 0, st>>>(count, L, mu, mss, sc, sss, endp, ers, sym, bits, q, pairs, nullptr, nullptr, kp);
-            else k_rows<NB, false, true><<<grid, RW * 32, 0, st>>>(count, L, mu, mss, sc, sss, endp, ers, sym, bits, q, pairs, nullptr, nullptr, kp);
-        }
+        const dim3 grid((unsigned)L, (count + RW - 1) / RW);
+        auto *k = pop ? rows_kernel<NB, true>() : rows_kernel<NB, false>();
+        k<<<grid, RW * 32, 0, st>>>(count, L, mu, mss, sc, sss, endp, ers, sym, bits, q, scr.pairs, scr.bases, scr.fix, bsw_apx_params());
     } else {
-        if (!pop) return launch_push_pairs(s, first, count, pairs, L, bits, ext, st);
-        if (ext) k_pop_coarse<NB, true><<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, coarse, fix, sym, L, bits, q, ext);
-        else k_pop_coarse<NB, false><<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, coarse, fix, sym, L, bits, q, nullptr);
-    }
-    BSW_LAUNCH_CHECK();
-    return BSW_OK;
-}
-
-// S = 2048 (NP = 2) or 4096 (NP = 4); same scratch layout as launch_rows<32>: 32 chunk bases per row, then the fix words
-template <int NP>
-int launch_rows_wide(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
-                     int64_t sss, const double *endp, int64_t ers, int16_t *sym, int64_t L, int bits, int q, void *scratch,
-                     const int16_t *ext, cudaStream_t st) {
-    dim3 grid((unsigned)L, (count + RW - 1) / RW);
-    uint4 *pairs = (uint4 *)scratch;
-    uint32_t *coarse = (uint32_t *)scratch;
-    uint2 *fix = (uint2 *)((uint8_t *)scratch + (size_t)count * L * 32 * 4);
-    const BswApxRegs kp = bsw_apx_params();
-    static const bool env_exact = getenv("BSW_ROWS_EXACT") && getenv("BSW_ROWS_EXACT")[0] == '1';
-    const bool exact = bits > 31 || env_exact;
-    BSW_MAX_SHARED_ONCE((k_rows_wide<NP, true, false>)); BSW_MAX_SHARED_ONCE((k_rows_wide<NP, true, true>));
-    BSW_MAX_SHARED_ONCE((k_rows_wide<NP, false, false>)); BSW_MAX_SHARED_ONCE((k_rows_wide<NP, false, true>));
-    BSW_MAX_SHARED_ONCE((k_pop_coarse_wide<NP, false>)); BSW_MAX_SHARED_ONCE((k_pop_coarse_wide<NP, true>));
-    if (phase == 0) {
-        if (pop) {
-            if (exact) k_rows_wide<NP, true, false><<<grid, RW * 32, 0, st>>>(count, L, mu, mss, sc, sss, endp, ers, nullptr, bits, q, nullptr, coarse, fix, kp);
-            else k_rows_wide<NP, true, true><<<grid, RW * 32, 0, st>>>(count, L, mu, mss, sc, sss, endp, ers, nullptr, bits, q, nullptr, coarse, fix, kp);
-        } else {
-            if (exact) k_rows_wide<NP, false, false><<<grid, RW * 32, 0, st>>>(count, L, mu, mss, sc, sss, endp, ers, sym, bits, q, pairs, nullptr, nullptr, kp);
-            else k_rows_wide<NP, false, true><<<grid, RW * 32, 0, st>>>(count, L, mu, mss, sc, sss, endp, ers, sym, bits, q, pairs, nullptr, nullptr, kp);
-        }
-    } else {
-        if (!pop) return launch_push_pairs(s, first, count, pairs, L, bits, ext, st);
-        if (ext) k_pop_coarse_wide<NP, true><<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, coarse, fix, sym, L, bits, q, ext);
-        else k_pop_coarse_wide<NP, false><<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, coarse, fix, sym, L, bits, q, nullptr);
+        if (!pop) return launch_push_pairs(s, first, count, scr.pairs, L, bits, ext, st);
+        if (ext) k_pop_coarse<NB, true><<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, scr.bases, scr.fix, sym, L, bits, q, ext);
+        else k_pop_coarse<NB, false><<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, scr.bases, scr.fix, sym, L, bits, q, nullptr);
     }
     BSW_LAUNCH_CHECK();
     return BSW_OK;
@@ -806,24 +597,16 @@ int bsw_prior_coarse(const uint32_t *C, int64_t L, int S, uint32_t *coarse, uint
 int bsw_pop_shared_table(bsw_streams *s, int first, int count, const uint32_t *P, const uint32_t *coarse, const uint2 *fix,
                          int16_t *sym, int64_t L, int S, int bits, cudaStream_t st) {
     BSW_REQUIRE(s && first >= 0 && count > 0 && first + count <= s->B, "stream range out of bounds");
-    switch (S) {
-        case 128:  return launch_pop_full<4>(s, first, count, P, coarse, fix, sym, L, bits, 1, st);
-        case 256:  return launch_pop_full<8>(s, first, count, P, coarse, fix, sym, L, bits, 1, st);
-        case 512:  return launch_pop_full<16>(s, first, count, P, coarse, fix, sym, L, bits, 1, st);
-        case 1024: return launch_pop_full<32>(s, first, count, P, coarse, fix, sym, L, bits, 1, st);
-    }
-    return BSW_E_INVALID;
+    return with_support<4, 32>(S, "shared-table pop: support must be one of 128,256,512,1024", [&](auto nb) {
+        k_pop_full<decltype(nb)::value><<<(count + BW - 1) / BW, BW * 32, 0, st>>>(*s, first, count, P, coarse, fix, sym, L, bits, 1);
+        BSW_LAUNCH_CHECK();
+        return BSW_OK;
+    });
 }
 
-// ans_rows6.cu
-int bsw_rows6_build_meta(const double *endp, int64_t ers, int64_t L, int S, void *meta_dev, int *n_affine_host, cudaStream_t st);
-int bsw_rows6_launch(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
-                     int64_t sss, const double *endp, int64_t ers, const void *meta, int16_t *sym, int64_t L, int S, int bits,
-                     int q, void *scratch, size_t scratch_bytes, const int16_t *ext, cudaStream_t st);
-
-// Scratch bytes of the two-phase coder for `count` streams of L rows: per row 16 B (push: P, C, reciprocal) or
-// 136 B (pop: 32 chunk bases + argmax/remnant), whichever kernel family runs and for every support up to 4096.
-size_t bsw_rows_scratch_bytes(int count, int64_t L) { return (size_t)count * L * 136; }
+// Scratch bytes of the two-phase coder for `count` streams of L rows: enough for a pop, which needs more than a push, for
+// either kernel family and every support up to 4096.
+size_t bsw_rows_scratch_bytes(int count, int64_t L) { return RowsScratch::bytes(true, count, L); }
 
 // Two-phase variants of bsw_logistic_push / bsw_logistic_pop (same arguments + caller-provided scratch).
 // phase 0 = the parallel row-table kernel, phase 1 = the serial coder; call both, in order, on one stream, with the
@@ -835,25 +618,17 @@ int bsw_logistic_2p(int phase, bool pop, bsw_streams *s, int first, int count, c
                     int q, void *scratch, size_t scratch_bytes, const int16_t *ext, cudaStream_t st) {
     BSW_REQUIRE(s && first >= 0 && count > 0 && first + count <= s->B, "stream range out of bounds");
     BSW_REQUIRE(mu && sc && endp && sym && scratch && L > 0 && L < 65536 * 32, "two-phase coder: bad arguments");
+    BSW_REQUIRE(bits >= 1 && bits <= 31 && q >= 0 && q < bits, "two-phase coder: bits/quantbits out of range");
     BSW_REQUIRE(ers == 0 || ers >= S, "two-phase coder: endpoint rows must hold S doubles (+1e300 padded)");
-    BSW_REQUIRE(scratch_bytes >= (pop ? bsw_rows_scratch_bytes(count, L) : (size_t)count * L * 16), "two-phase coder: scratch too small");
+    BSW_REQUIRE(scratch_bytes >= RowsScratch::bytes(pop, count, L), "two-phase coder: scratch too small");
     BSW_REQUIRE((((uintptr_t)scratch) & 15) == 0, "two-phase coder: scratch must be 16-byte aligned");
     if (meta) {
         if (phase == 1 && !pop) return launch_push_pairs(s, first, count, scratch, L, bits, ext, st);
         return bsw_rows6_launch(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, meta, sym, L, S, bits, q, scratch, scratch_bytes, ext, st);
     }
-    switch (S) {
-        case 32:   return launch_rows<1>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
-        case 64:   return launch_rows<2>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
-        case 128:  return launch_rows<4>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
-        case 256:  return launch_rows<8>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
-        case 512:  return launch_rows<16>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
-        case 1024: return launch_rows<32>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
-        case 2048: return launch_rows_wide<2>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
-        case 4096: return launch_rows_wide<4>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
-    }
-    bsw_set_error("two-phase coder: support must be one of 32,64,...,4096 (got %d)", S);
-    return BSW_E_INVALID;
+    return with_support<1, 128>(S, "two-phase coder: support must be one of 32,64,...,4096", [&](auto nb) {
+        return launch_rows<decltype(nb)::value>(phase, pop, s, first, count, mu, mss, sc, sss, endp, ers, sym, L, bits, q, scratch, ext, st);
+    });
 }
 
 // ---- FP64 peak microbenchmark (roofline denominator of the row-table kernel; MEASURED_PEAKS.json has no FP64 figure) ----

@@ -19,10 +19,8 @@
 // HBM traffic per (stream,row): 10 B in (mu, sigma, symbol) + 16 B (push) or 136 B (pop) of scratch written and read once.
 #include <stdlib.h>
 #include <type_traits>
-#include "bsw_common.cuh"
+#include "coder.cuh"
 #include "rows6_core.cuh"
-
-#define FULL 0xffffffffu
 
 namespace {
 
@@ -309,36 +307,6 @@ __global__ void __launch_bounds__(512, 2) k_rows6(int count, int64_t L, int S, c
 }
 
 // ---- phase B: pop -----------------------------------------------------------------------------------------------------------
-struct WarpStream6 {          // same state handling as ans_kernels.cu's WarpStream (pop side only)
-    uint32_t *words;
-    uint64_t x;
-    int len, wbase, err;
-    uint32_t wbuf;
-    __device__ __forceinline__ void open(const bsw_streams &sv, int b) {
-        words = sv.words + (int64_t)b * sv.cap; x = sv.heads[b]; len = sv.nwords[b];
-        err = sv.flags[b]; wbase = -1; wbuf = 0;
-    }
-    __device__ __forceinline__ void close(const bsw_streams &sv, int b, int lane) {
-        if (lane == 0) { sv.heads[b] = x; sv.nwords[b] = len; sv.flags[b] = err; if (len < sv.minwords[b]) sv.minwords[b] = len; }
-    }
-    __device__ __forceinline__ uint32_t pop_word(int lane) {
-        int idx = len - 1;
-        if (wbase < 0 || idx < wbase) { wbase = idx & ~31; wbuf = words[wbase + lane]; }
-        len = idx;
-        return __shfl_sync(FULL, wbuf, idx - wbase);
-    }
-    __device__ __forceinline__ void decode(uint32_t p, uint32_t c, uint32_t m, int bits, int lane) {   // cifar_compress.py:63-65
-        x = (uint64_t)p * (x >> bits) + m - c;
-        if (x < ((uint64_t)1 << 32)) {
-            if (len <= 0) { err = BSW_E_UNDERFLOW; return; }
-            x = (x << 32) | pop_word(lane);
-        }
-    }
-};
-__device__ __forceinline__ double shfl_d(double v, int src) {
-    return __hiloint2double(__shfl_sync(FULL, __double2hiint(v), src), __shfl_sync(FULL, __double2loint(v), src));
-}
-
 // MASK: pixel level with block extents -- rows outside the extent keep the block loads and the prefetch going but skip the
 // search and the decode (bsw_x_live, warp-uniform); their symbols are written later by the codec's pad kernel.
 // WIDE: S = 2048 or 4096 -- the wide fix layout and chunks of up to 128 bins (see the branch below).
@@ -351,7 +319,7 @@ __global__ void __launch_bounds__(PW6 * 32) k_pop6(bsw_streams sv, int first, in
     const int si = blockIdx.x * PW6 + (threadIdx.x >> 5);
     if (si >= count) return;
     const int b = first + si;
-    WarpStream6 ws;
+    WarpStream ws;
     ws.open(sv, b);
     if (ws.err) return;
     int vh = 32, vw = 32;
@@ -513,22 +481,16 @@ int bsw_rows6_build_meta(const double *endp, int64_t ers, int64_t L, int S, void
     return BSW_OK;
 }
 
-size_t bsw_rows6_scratch_bytes(int count, int64_t L) {
-    return (size_t)count * L * (32 * 4 + 8);              // pop: 32 chunk bases + fix; push needs 16 B per row
-}
-
 namespace {
 template <bool WIDE>
 int rows6_launch(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
                  int64_t sss, const double *endp, int64_t ers, const void *meta, int16_t *sym, int64_t L, int S, int bits,
                  int q, void *scratch, size_t scratch_bytes, const int16_t *ext, cudaStream_t st) {
     BSW_REQUIRE(bits >= 8 && bits <= 31 && q >= 0 && q < bits, "affine coder: bits/quantbits out of range");
-    BSW_REQUIRE(scratch_bytes >= (pop ? bsw_rows6_scratch_bytes(count, L) : (size_t)count * L * 16), "affine coder: scratch too small");
+    BSW_REQUIRE(scratch_bytes >= RowsScratch::bytes(pop, count, L), "affine coder: scratch too small");
     const R6RowMeta *mt = (const R6RowMeta *)meta;
     const int64_t mrs = ers == 0 ? 0 : 1;
-    uint4 *pairs = (uint4 *)scratch;
-    uint32_t *bases = (uint32_t *)scratch;
-    uint2 *fix = (uint2 *)((uint8_t *)scratch + (size_t)count * L * 128);
+    const RowsScratch scr(scratch, count, L);
     if (phase == 0) {
         // BSW_R6_LPR = lanes per row (32, 8, 4 or 2; default 4 = eight rows per warp): same integers, different mapping (A/B runs)
         static const int env_lpr0 = getenv("BSW_R6_LPR") ? atoi(getenv("BSW_R6_LPR")) : 4;
@@ -537,8 +499,8 @@ int rows6_launch(int phase, bool pop, bsw_streams *s, int first, int count, cons
 #define R6_LAUNCH(POP_, VER_, LPR_)                                                                                             \
     BSW_MAX_SHARED_ONCE((k_rows6<POP_, VER_, LPR_, WIDE>));                                                                       \
     k_rows6<POP_, VER_, LPR_, WIDE><<<dim3((unsigned)((L + 32 / LPR_ - 1) / (32 / LPR_)), (count + 15) / 16), 512, 0, st>>>(            \
-        count, L, S, mu, mss, sc, sss, endp, ers, mt, mrs, POP_ ? nullptr : sym, bits, q, POP_ ? nullptr : pairs,                 \
-        POP_ ? bases : nullptr, POP_ ? fix : nullptr, VER_ ? g_vstat : nullptr, 0,                                                \
+        count, L, S, mu, mss, sc, sss, endp, ers, mt, mrs, POP_ ? nullptr : sym, bits, q, POP_ ? nullptr : scr.pairs,                 \
+        POP_ ? scr.bases : nullptr, POP_ ? scr.fix : nullptr, VER_ ? g_vstat : nullptr, 0,                                                \
         (double)(((int64_t)1 << bits) - ((int64_t)1 << q)) * 1048576.0,                                                           \
         1.0 / ((double)(((int64_t)1 << bits) - ((int64_t)1 << q)) * 1048576.0),                                                     \
         (double)(((int64_t)1 << bits) - ((int64_t)1 << q)) * 1048576.0 + R6_MAGIC0)
@@ -553,8 +515,8 @@ int rows6_launch(int phase, bool pop, bsw_streams *s, int first, int count, cons
     } else {
         BSW_REQUIRE(pop, "affine coder: phase B of a push is k_push_pairs");
         BSW_MAX_SHARED_ONCE((k_pop6<false, WIDE>)); BSW_MAX_SHARED_ONCE((k_pop6<true, WIDE>));
-        if (ext) k_pop6<true, WIDE><<<(count + PW6 - 1) / PW6, PW6 * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, mt, mrs, bases, fix, sym, L, S, bits, q, ext);
-        else k_pop6<false, WIDE><<<(count + PW6 - 1) / PW6, PW6 * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, mt, mrs, bases, fix, sym, L, S, bits, q, nullptr);
+        if (ext) k_pop6<true, WIDE><<<(count + PW6 - 1) / PW6, PW6 * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, mt, mrs, scr.bases, scr.fix, sym, L, S, bits, q, ext);
+        else k_pop6<false, WIDE><<<(count + PW6 - 1) / PW6, PW6 * 32, 0, st>>>(*s, first, count, mu, mss, sc, sss, endp, ers, mt, mrs, scr.bases, scr.fix, sym, L, S, bits, q, nullptr);
     }
     BSW_LAUNCH_CHECK();
     return BSW_OK;

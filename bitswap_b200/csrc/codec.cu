@@ -8,7 +8,7 @@
 // reference's 2*nz GPU<->CPU round trips per image (cifar_compress.py:42-43,66) do not exist here.
 #include <stdlib.h>
 #include <vector>
-#include "bsw_common.cuh"
+#include "coder.cuh"
 #include "nets.cuh"
 
 struct bsw_codec {
@@ -38,25 +38,6 @@ struct bsw_codec {
     int ev_next = 0;
     int dual_stream = 0;
 };
-
-// internal int16-symbol variants of the table-driven coder (ans_kernels.cu)
-int bsw_ans_push_i16(bsw_streams *s, int first, int count, const uint32_t *P, const uint32_t *C, int64_t pss, int64_t css,
-                     const int16_t *sym, int64_t L, int S, int bits, cudaStream_t st);
-int bsw_ans_pop_i16(bsw_streams *s, int first, int count, const uint32_t *P, const uint32_t *C, int64_t pss, int64_t css,
-                    int16_t *sym, int64_t L, int S, int bits, cudaStream_t st);
-
-size_t bsw_rows_scratch_bytes(int count, int64_t L);
-int bsw_streams_mark_rest(bsw_streams *s, int first, int count, cudaStream_t st);
-int bsw_rows_mode();
-int bsw_prior_coarse(const uint32_t *C, int64_t L, int S, uint32_t *coarse, uint2 *fix, cudaStream_t st);
-int bsw_pop_shared_table(bsw_streams *s, int first, int count, const uint32_t *P, const uint32_t *coarse, const uint2 *fix,
-                         int16_t *sym, int64_t L, int S, int bits, cudaStream_t st);
-int bsw_logistic_2p(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
-                    int64_t sss, const double *endp, int64_t ers, const void *meta, int16_t *sym, int64_t L, int S, int bits, int q,
-                    void *scratch, size_t scratch_bytes, const int16_t *ext, cudaStream_t st);
-int bsw_logistic_fused_ext(bool push, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
-                           int64_t sss, const double *endp, int64_t ers, int16_t *sym, int64_t L, int S, int bits, int q,
-                           const int16_t *ext, cudaStream_t st);
 
 __global__ void k_u8_to_i16(const uint8_t *__restrict__ in, int16_t *__restrict__ out, int64_t n) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;

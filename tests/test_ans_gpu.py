@@ -422,6 +422,40 @@ def test_two_phase_abi_extreme_tables_vs_fused_and_oracle(S, q, mode):
         assert res["2p"][2][b] == a.encode(st, sym[b].astype(np.int64)).to_list()
 
 
+@pytest.mark.parametrize("mode", [0, -1, 1])
+@pytest.mark.parametrize("bits,q", [(32, 10), (31, 31), (10, 12)])
+def test_two_phase_abi_refuses_bits_out_of_range(bits, q, mode):
+    """The two-phase coder codes 1 <= bits <= 31 and 0 <= quantbits < bits, like the fused one: anything else is
+    BSW_E_INVALID before any coder kernel runs, for every kernel family, and the streams are left as they were."""
+    check(lib().bsw_set_rows_mode(mode))
+    B, L, S = 3, 40, 1024
+    rs = np.random.RandomState(7)
+    ends = np.linspace(-6, 6, S + 1)[1:-1]
+    e_pad = torch.from_numpy(_pad_big(np.tile(ends, (L, 1)))).to(dev)
+    dmu = torch.from_numpy(rs.normal(0, 1, (B, L)).astype(np.float32)).to(dev)
+    dsc = torch.from_numpy(rs.uniform(0.1, 1.0, (B, L)).astype(np.float32)).to(dev)
+    sym = torch.from_numpy(rs.randint(0, S, size=(B, L)).astype(np.int16)).to(dev)
+    nbytes = int(lib().bsw_logistic_scratch_bytes(B, L, S, 0))
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    states = []
+    for b in range(B):
+        w, head = synthetic.initial_words(500 + b, seed=40 + b)
+        states.append([int(v) for v in w] + [head])
+    ss = StreamSet(B, 1 << 12)
+    ss.import_lists(states)
+    try:
+        for fn, s_ in ((lib().bsw_logistic_push_2p, sym), (lib().bsw_logistic_pop_2p, sym.clone())):
+            rc = fn(ss.handle, 0, B, dmu.data_ptr(), L, dsc.data_ptr(), L, e_pad.data_ptr(), S, s_.data_ptr(), L, S, bits, q,
+                    scratch.data_ptr(), nbytes, cuda_stream_ptr())
+            assert rc == 4, (fn, rc)
+            assert b"out of range" in lib().bsw_last_error()
+        torch.cuda.synchronize()
+    finally:
+        check(lib().bsw_set_rows_mode(-1))
+    assert ss.export_lists() == states
+    assert not ss.sizes()[2].any()
+
+
 def test_screening_cdf_error_is_far_inside_the_window():
     """k_rows trusts bsw_cdf_apx only when the scaled pmf is >= 64 units (2^-51 each) away from a truncation boundary;
     the pmf error is at most twice the cdf error, so the cdf error must stay below 32 units.  Measured worst case over

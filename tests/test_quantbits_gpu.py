@@ -126,8 +126,8 @@ def _check_vs_oracle(res, tabs, states, sym, check_streams):
 @pytest.mark.parametrize("family", ["generic", "affine", "forced_affine"])
 def test_two_phase_wide_support_vs_oracle(S, q, family):
     """pop then push of one level through bsw_logistic_pop_2p / push_2p, against our exported pmfs -> oracle ANS.__init__ ->
-    oracle coder, at every power of two from 32 to 4096 bins.  generic = k_rows<S/32> / k_pop_coarse<S/32> (k_rows_wide /
-    k_pop_coarse_wide above 1024), affine = k_rows6 / k_pop6 on uniform grids, forced_affine =
+    oracle coder, at every power of two from 32 to 4096 bins.  generic = k_rows<S/32> / k_pop_coarse<S/32> (k_rows_wide<S/1024>
+    above 1024), affine = k_rows6 / k_pop6 on uniform grids, forced_affine =
     the affine kernels on the equal-mass top-level rows (every bin takes the exact path).  B = 64 streams, L = 99 rows (not
     a multiple of the 8 rows per warp); ordinary, needle-sharp, all-bins-live and off-grid rows."""
     B, L = 64, 99
