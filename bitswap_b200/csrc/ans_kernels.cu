@@ -811,8 +811,10 @@ extern "C" int bsw_bins_create(bsw_bins **out, int nz, int zdim, int q, int xdim
     bsw_bins *b = new bsw_bins();
     b->nz = nz; b->zdim = zdim; b->q = q; b->S = 1 << q; b->xdim = xdim;
     const int S = b->S;
-    // pad value of every endpoint row: any finite value this large gives cdf == 1.0 exactly in every kernel
-    // (a literal +inf would turn the reciprocal-division shortcut into inf - inf)
+    // pad value of every endpoint row.  The exact evaluations never read it (every kernel takes cdf = 1 for the last bin:
+    // with a tiny sigma the corrected division of bsw_cdf_fast turns (1e300 - mu) / sigma into inf - inf), and the
+    // screening evaluations that do read it clamp t and get 1.0 exactly (a literal +inf would turn the
+    // reciprocal-division shortcut into inf - inf for every sigma)
     const double inf = 1e300;
     size_t rows = (size_t)nz * zdim;
     std::vector<double> pad(rows * S);

@@ -40,11 +40,13 @@ struct RowTile {
 
 __device__ __forceinline__ uint32_t smem_u32r(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// exact integer pmf (before the +1) of bin j of this lane's block: the rare path of the screened kernel
+// exact integer pmf (before the +1) of bin j of this lane's block: the rare path of the screened kernel.  The row's last
+// bin (lane 31, j = NB - 1) has upper cdf 1 exactly (:184), as in every other kernel: its tile entry is the +1e300 pad,
+// and for sigma below ~5.6e-9 the corrected division of bsw_cdf_fast turns (1e300 - mu) / sigma into inf - inf = NaN.
 template <int NB, int STRIDE>
 __device__ __noinline__ uint32_t rows_exact_pm(const double *tile, int lane, int j0, int t, double m, double s, double rs, double mult) {
     const int j = j0 + t;                                 // (added here so that the hot loop does not carry j0+1..j0+3)
-    const double c = bsw_cdf_fast(tile[lane * STRIDE + j], m, s, rs);
+    const double c = (lane == 31 && j == NB - 1) ? 1.0 : bsw_cdf_fast(tile[lane * STRIDE + j], m, s, rs);
     double p = 0.0;                                       // lower edge of bin 0 is cdf = 0 (cifar_compress.py:184)
     if (j > 0) p = bsw_cdf_fast(tile[lane * STRIDE + j - 1], m, s, rs);
     else if (lane > 0) p = bsw_cdf_fast(tile[(lane - 1) * STRIDE + NB - 1], m, s, rs);

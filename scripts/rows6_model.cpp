@@ -3,9 +3,16 @@
 // against the exact function on random uniform-grid rows, and checks
 //   (1) every emitted integer pmf == the exact function's, (2) dead bins really have P == 1, (3) the worst screening error
 //   of a trusted bin is far inside the window, (4) the chunk-base / pop search reproduces a search of the full table.
-// Build: g++ -O2 -std=c++17 -o rows6_model scripts/rows6_model.cpp -lm ; run: ./rows6_model [rows] [seed] [S]
+// Build: g++ -O2 -std=c++17 -o rows6_model scripts/rows6_model.cpp -lm ; run: ./rows6_model [rows] [seed] [S] [family]
 // S = 0 (default): the mix of S = 1024 / 256 / 64 rows; S = 2048 or 4096: every row at that support (quantbits 11 / 12),
 // with needle-sharp, wide (every bin live), off-grid-mean and out-of-range rows among them.
+// family = 0 (default): every row spans about -6.5 .. 6.5.  1-6: the grids discretize() can build, np.linspace between the
+// extrema of one latent dimension, with mu and sigma drawn relative to each grid (see grid_row):
+//   1 off-centre (centre within +-1000, span 1-21)   2 float16 extrema at or near +-65504, possibly asymmetric
+//   3 far from zero and narrow (30000-60000, span <= 1)   4 tiny spans 2^-20 .. 2^-24 at 0 and at 1000
+//   5 coarse: dt = d / sigma just under and just over 64 (where the plan falls back)
+//   6 rows perturbed off the affine line by up to the classification tolerance (windows up to the 262144 cap and past it)
+// Rows that fail k_row_meta's rule get dev = +inf, as in the kernel (the plan then distrusts every bin).
 #include <stdio.h>
 #include <stdlib.h>
 #include <vector>
@@ -33,14 +40,67 @@ static double urand() { rng ^= rng << 13; rng ^= rng >> 7; rng ^= rng << 17; ret
 
 constexpr int LPR = 4, CPL = 32 / LPR;      // the kernel's default mapping: 4 lanes per row, 8 chunks per lane
 
+static double urange(double lo, double hi) { return lo + (hi - lo) * urand(); }
+static double sgn() { return urand() < 0.5 ? -1.0 : 1.0; }
+// round to the nearest float16 value (the samples discretize() takes the extrema of are float16), saturating at +-65504
+static double half(double x) {
+    if (x == 0.0) return 0.0;
+    int ex; frexp(fabs(x), &ex);
+    const int qe = std::max(ex - 11, -24);
+    return fmax(-65504.0, fmin(65504.0, ldexp(nearbyint(ldexp(x, -qe)), qe)));
+}
+
+// One endpoint row of grid family fam (1-6) at support S as k_uniform_edges builds it (y_k = lo + k (hi - lo) / S, the
+// multiply-add contracted), and mu / sigma drawn relative to the grid's centre c, half-width h and bin width d: a few bins
+// live, many live, mass just beyond the grid, or anything in between.
+static void grid_row(int fam, int S, std::vector<double> &e, float &muf, float &scf) {
+    double lo, hi;
+    switch (fam) {
+        case 1: { const double c = urange(-1000, 1000), w = urange(1, 21); lo = half(c - w * urange(0.2, 0.8)); hi = half(lo + w); break; }
+        case 2: { const int k = (int)(urand() * 4);
+                  lo = k == 0 ? -65504.0 : half(-urange(30000, 65504));
+                  hi = k == 1 ? 65504.0 : (k == 2 ? half(urange(-1000, 60000)) : half(urange(30000, 65504)));
+                  if (k == 3) { lo = -65504.0; hi = 65504.0; }
+                  break; }
+        case 3: { const double c = sgn() * urange(30000, 60000), w = urange(1e-3, 1); lo = c - w * urange(0.2, 0.8); hi = lo + w; break; }
+        case 4: { const double c = urand() < 0.5 ? 0.0 : 1000.0, w = ldexp(1.0, -20 - (int)(urand() * 5)); lo = c - w * urange(0.2, 0.8); hi = lo + w; break; }
+        case 5: { lo = half(urange(-10, 5)); hi = half(lo + urange(0.5, 20)); break; }
+        default: { lo = urange(-300, 300); hi = lo + exp(urange(log(0.5), log(100.0))); break; }
+    }
+    const double step = (hi - lo) / S;
+    for (int k = 0; k < S - 1; ++k) e[k] = fma((double)(k + 1), step, lo);
+    const double c = 0.5 * (lo + hi), h = 0.5 * (hi - lo), d = step;
+    double mu, sc;
+    if (fam == 5) {                                       // dt = d / sigma in 64 * [0.97, 1.03]
+        sc = d / (64.0 * urange(0.97, 1.03)); mu = c + h * urange(-1, 1);
+    } else {
+        switch ((int)(urand() * 4)) {
+            case 0: sc = d * pow(10.0, urange(-1.5, 0.5)); mu = c + h * urange(-1, 1); break;                  // a few bins live
+            case 1: sc = h * urange(0.05, 0.6); mu = c + h * urange(-1, 1); break;                             // many live
+            case 2: sc = d * pow(10.0, urange(-1, 1.5)); mu = c + sgn() * (h + sc * urange(0, 12)); break;     // just beyond the grid
+            default: sc = d * pow(10.0, urange(0, log10(fmax(1.0, h / d)))); mu = c + h * urange(-1.2, 1.2); break;
+        }
+    }
+    if (fam == 6) {                                       // deviation up to 1e-13 max(1, emax), the classification tolerance
+        const double emax = fmax(fabs(lo), fabs(hi));
+        const double dv = 1e-13 * fmax(1.0, emax) * pow(10.0, urange(-6, 0));
+        for (int k = 1; k < S - 2; ++k) e[k] += dv * urange(-1, 1);
+        e[1 + (int)(urand() * (S - 3))] += sgn() * dv;
+    }
+    muf = (float)mu; scf = (float)sc;
+    if (!(scf > 0.0f)) scf = 1e-38f;
+}
+
 int main(int argc, char **argv) {
     long nrows = argc > 1 ? atol(argv[1]) : 20000;
     if (argc > 2) rng ^= (uint64_t)atol(argv[2]) * 0x9E3779B97F4A7C15ull;
     const int Sw = argc > 3 ? atoi(argv[3]) : 0;
     if (Sw != 0 && Sw != 2048 && Sw != 4096) { printf("S must be 0, 2048 or 4096\n"); return 1; }
+    const int fam = argc > 4 ? atoi(argv[4]) : 0;
+    if (fam < 0 || fam > 6) { printf("family must be 0 .. 6\n"); return 1; }
     const int bits = 31;
     long fixbad = 0, maxsteps = 0;
-    long mism = 0, deadbad = 0, popbad = 0, doubted = 0, bins = 0, evaluated = 0, notok = 0;
+    long mism = 0, deadbad = 0, popbad = 0, doubted = 0, bins = 0, evaluated = 0, notok = 0, nonaffine = 0;
     double worst = 0;  // window units
     double worst_frac = 0, worst64 = 0;
     for (long it = 0; it < nrows; ++it) {
@@ -50,17 +110,21 @@ int main(int argc, char **argv) {
         const bool wide_s = S > 1024;
         std::vector<double> e(S);
         double lo, hi;
-        if (S == 256 && !Sw) { for (int k = 1; k <= 255; ++k) e[k - 1] = (((double)k - 127.5) / 127.5) - 1. / 255.; }
+        float muf, scf;
+        if (fam) grid_row(fam, S, e, muf, scf);
+        else if (S == 256 && !Sw) { for (int k = 1; k <= 255; ++k) e[k - 1] = (((double)k - 127.5) / 127.5) - 1. / 255.; }
         else { lo = -6 - urand(); hi = 6 + urand(); double step = (hi - lo) / S; for (int k = 0; k < S - 1; ++k) e[k] = lo + (k + 1) * step; }
         e[S - 1] = 1e300;
-        // meta as k_row_meta computes it
+        // meta as k_row_meta computes it, classification included
         R6RowMeta M; int n = S - 1;
         M.a = e[0]; M.d = (e[n - 1] - e[0]) / (double)(n - 1);
         double dev = 0, emax = 0;
         for (int k = 0; k < n; ++k) { dev = fmax(dev, fabs(e[k] - fma((double)k, M.d, M.a))); emax = fmax(emax, fabs(e[k])); }
-        dev += emax * 2.3e-16; M.dev = dev; M.rsv = 0;
-        float muf, scf;
-        switch (mode) {
+        dev += emax * 2.3e-16;
+        const bool affine = (M.d > 0.0) && (dev <= 1e-13 * fmax(1.0, emax)) && (emax < 1e6);
+        M.dev = affine ? dev : HUGE_VAL; M.rsv = 0;
+        if (!affine) ++nonaffine;
+        if (!fam) switch (mode) {
             case 0: case 1: muf = (float)((urand() - 0.5) * 10); scf = (float)(0.1 + 0.9 * urand()); break;
             case 2: muf = (float)((urand() - 0.5) * 14); scf = 0.1f + (float)(0.01 * urand()); break;             // sharp
             case 3: muf = (float)((urand() < 0.5 ? -1 : 1) * (7 + 20 * urand()));                                     // mass outside the grid,
@@ -148,5 +212,6 @@ int main(int argc, char **argv) {
     printf("worst trusted err among rows with the minimum window (64 units): %.2f units\n", worst64);
     printf("support %s: longest chain since its last exp %ld steps of 4 bins; wide fix-word mismatches %ld\n", Sw ? (Sw == 2048 ? "2048" : "4096") : "mixed", maxsteps, fixbad);
     printf("mismatches %ld (in dead zones %ld)  pop-search mismatches %ld  worst trusted err %.2f units (%.3f of its window)\n", mism, deadbad, popbad, worst, worst_frac);
+    if (argc > 4) printf("family %d: rows not affine %ld\n", fam, nonaffine);
     return (mism || popbad || fixbad) ? 2 : 0;
 }
