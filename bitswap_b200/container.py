@@ -30,6 +30,17 @@ Regions: a chain is a stack, so decoding pops its blocks last to first; to reach
 pops n - j blocks and no further, and a chain none of whose blocks is wanted is not imported at all.  decompress_regions
 decodes only that (plan_regions says how much), and decompress_images is the same path with one whole-image region per
 container.
+
+Archives: a set of images as one array whose chains run across images.  Each chain borrows its first latent samples from
+the initial words and keeps them, so one chain per small image pays them per image; compress_archive tiles every image as
+edges="code" does, lays their row-major blocks end to end in the order given and cuts that one sequence into
+chain_sizes(total blocks, chain_blocks) runs, each a chain from the seeded initial state.  Layout:
+    [ words_0 ... words_{K-1} | (nwords_k, head_lo_k, head_hi_k, nblocks_k) for k < K | (h_i, w_i) for i < N
+    | K, N, excess_state_len, seed, scheme, ARCHIVE_MARK ]
+Read as a reference tail its width is ARCHIVE_MARK >= 2^31 and as a multi-chain container its last word is not CHAIN_MARK,
+so unpack_container refuses it.  Decoding an image pops, in each chain holding its blocks, from the chain's end down to its
+first block there; a chain popped to its first block must come back to the seeded initial state (cifar_compress.py:356).
+Containers and archives share one encode loop (_encode) and one decode loop (_decode_regions) over a block sequence.
 """
 import collections
 import numbers
@@ -37,12 +48,15 @@ import numbers
 import numpy as np
 import torch
 
-from .codec import BITSWAP
+from .codec import BBANS, BITSWAP
 from .streams import StreamSet
 from .synthetic import initial_words
 
 CHAIN_MARK = 0x8043484E                  # bit 31 | "CHN": last word of a multi-chain container
 MAX_BLOCKS = 1 << 20                     # blocks per image a container may declare
+ARCHIVE_MARK = 0x80415243                # bit 31 | "ARC": last word of an archive
+MAX_ARCHIVE_BLOCKS = 1 << 24             # blocks an archive may declare in all
+MAX_INITIAL_WORDS = 1 << 24              # largest excess_state_len an archive may declare
 
 
 def extract_blocks(arr, block_size=(32, 32)):
@@ -155,13 +169,29 @@ def compress_images(codec, images, excess_state_len=10000, seed=100, scheme=BITS
         tiled = [extract_edge_blocks(im) for im in images]
     else:
         tiled = [(b, None, h, w) for b, h, w in (extract_blocks(im) for im in images)]
-    # chains (image, first block, blocks) in image and block order; streams hold them largest first
-    chains = []
-    for i, t in enumerate(tiled):
+    # one block sequence of every image in turn; each image's chains are runs inside its own blocks
+    chains, off = [], 0
+    for t in tiled:
         sizes = chain_sizes(t[0].shape[0], chain_blocks)
-        chains += [(i, s, nb) for s, nb in zip(np.cumsum([0] + sizes[:-1]).tolist(), sizes)]
-    order = sorted(range(len(chains)), key=lambda c: (-chains[c][2], c))
-    nblk = [chains[c][2] for c in order]
+        chains += [(off + s, nb) for s, nb in zip(np.cumsum([0] + sizes[:-1]).tolist(), sizes)]
+        off += t[0].shape[0]
+    blocks = np.concatenate([_blocks_to_model(t[0], hwc_quirk) for t in tiled])
+    extents = None if edges == "crop" else np.concatenate([t[1] for t in tiled])
+    coded = _encode(codec, blocks, extents, chains, scheme, excess_state_len, seed, words_per_block)
+    out, k = [], 0
+    for t in tiled:
+        K = len(chain_sizes(t[0].shape[0], chain_blocks))
+        out.append(pack_container(coded[k:k + K], t[2], t[3]))
+        k += K
+    return out
+
+
+def _encode(codec, blocks, extents, chains, scheme, excess_state_len, seed, words_per_block):
+    """Codes a block sequence (blocks [n, C, 32, 32] in model layout, extents int16 [n, 2] or None) as the chains (start,
+    nblocks) given, each a run of it, from the seeded initial state.  Returns [(words above the lowest depth, head,
+    nblocks)] in chain order.  Streams hold the chains largest first, so the active streams at each step are a prefix."""
+    order = sorted(range(len(chains)), key=lambda c: (-chains[c][1], c))
+    nblk = [chains[c][1] for c in order]
     w, head = initial_words(excess_state_len, seed=seed)
     # capacity: `words_per_block` words per 32x32 block of the longest chain (1400 = 14.6 bits/dim; 8 bits/dim of raw pixels
     # is 768).  A chain that still overflows is retried with twice the room instead of failing after it was coded.
@@ -169,25 +199,23 @@ def compress_images(codec, images, excess_state_len=10000, seed=100, scheme=BITS
         ss = StreamSet(len(chains), excess_state_len + (words_per_block << attempt) * max(nblk) + 64, device=codec.device)
         ss.fill(w, head)
         try:
-            return _compress_chains(codec, ss, tiled, chains, order, nblk, scheme, hwc_quirk)
+            return _compress_chains(codec, ss, blocks, extents, chains, order, nblk, scheme)
         except OverflowError:
             if attempt == 3:
                 raise
     raise AssertionError("unreachable")
 
 
-def _compress_chains(codec, ss, tiled, chains, order, nblk, scheme, hwc_quirk):
+def _compress_chains(codec, ss, blocks, extents, chains, order, nblk, scheme):
     n = len(order)
     # all blocks to the device once: [step t, stream j] = block t of the j-th largest chain (CHW, demo_compress.py:120)
-    C = tiled[chains[order[0]][0]][0].shape[-1]
-    host = np.zeros((max(nblk), n, C, 32, 32), dtype=np.uint8)
-    model = [_blocks_to_model(t[0], hwc_quirk) for t in tiled]
+    host = np.zeros((max(nblk), n) + blocks.shape[1:], dtype=np.uint8)
     for j, c in enumerate(order):
-        i, s, nb = chains[c]
-        host[:nb, j] = model[i][s:s + nb]
+        s, nb = chains[c]
+        host[:nb, j] = blocks[s:s + nb]
     dev = torch.from_numpy(host).to(torch.device("cuda", codec.device))
-    ext = _extents_to_device(codec, [None if tiled[i][1] is None else tiled[i][1][s:s + nb] for i, s, nb in
-                                     (chains[c] for c in order)], nblk)
+    ext = _extents_to_device(codec, [None if extents is None else extents[s:s + nb] for s, nb in (chains[c] for c in order)],
+                             nblk)
     active = _active(nblk)
     for t in range(max(nblk)):
         for b, cnt in _sub_ranges(int(active[t]), codec.max_batch):
@@ -196,13 +224,9 @@ def _compress_chains(codec, ss, tiled, chains, order, nblk, scheme, hwc_quirk):
     ss.raise_on_error()
     words, offs, heads, _ = ss.export()
     lo = ss.min_words()                                       # never-borrowed initial words (demo_compress.py:137,160)
-    mine = [[] for _ in tiled]                                # each image's streams, in block order
     stream = np.empty(n, dtype=np.int64)
     stream[order] = np.arange(n)
-    for c, (i, _, _) in enumerate(chains):
-        mine[i].append(int(stream[c]))
-    return [pack_container([(words[offs[j] + lo[j]:offs[j + 1]], int(heads[j]), nblk[j]) for j in js], h, wd)
-            for js, (_, _, h, wd) in zip(mine, tiled)]
+    return [(words[offs[j] + lo[j]:offs[j + 1]], int(heads[j]), nb) for j, (_, nb) in zip(stream.tolist(), chains)]
 
 
 def _extents_to_device(codec, extents, nblk):
@@ -272,8 +296,24 @@ earliest block the regions need counted from the chain's first block (the chain'
 and the blocks to pop to reach it, nblocks - first (0: the chain is skipped).  needed: bool [nblocks], the row-major
 blocks the regions cover."""
 
+# A decode job: a block sequence of images, each image's row-major blocks in turn (image i owns blocks ioff[i] to
+# ioff[i + 1]), and the chains that code it, contiguous runs in sequence order (chain k: pieces[k] and heads[k], blocks
+# cstart[k] to cstart[k] + cnb[k]).  A container is one image whose chains stay inside it; an archive lets them run across.
+_Job = collections.namedtuple("_Job", "pieces heads cstart cnb shapes ioff")
 
-def _check_region(r, parsed):
+
+def _containers_job(parsed):
+    """The decode job of unpack_container results: the containers' images in turn, each with its own chains."""
+    nb = [int(p[3].sum()) for p in parsed]
+    ioff = np.zeros(len(parsed) + 1, dtype=np.int64)
+    np.cumsum(nb, out=ioff[1:])
+    cnb = np.concatenate([p[3] for p in parsed]) if parsed else np.zeros(0, np.int64)
+    return _Job([p[0][p[1][k]:p[1][k + 1]] for p in parsed for k in range(len(p[3]))],
+                np.concatenate([p[2] for p in parsed]) if parsed else np.zeros(0, np.uint64),
+                np.cumsum(cnb) - cnb, cnb, [(p[4], p[5]) for p in parsed], ioff)
+
+
+def _check_region(r, shapes):
     try:
         fields = tuple(r)
     except TypeError:
@@ -281,40 +321,37 @@ def _check_region(r, parsed):
     if len(fields) != 5 or not all(isinstance(v, numbers.Integral) and not isinstance(v, bool) for v in fields):
         raise ValueError(f"a region is five ints (i, y, x, h, w), got {r!r}")
     i, y, x, h, w = (int(v) for v in fields)
-    if not 0 <= i < len(parsed):
-        raise ValueError(f"region {r!r}: no container {i} among {len(parsed)}")
-    H, W = parsed[i][4], parsed[i][5]
+    if not 0 <= i < len(shapes):
+        raise ValueError(f"region {r!r}: no image {i} among {len(shapes)}")
+    H, W = shapes[i]
     if h < 1 or w < 1 or y < 0 or x < 0 or y + h > H or x + w > W:
-        raise ValueError(f"region {r!r} is empty or leaves the {H} x {W} image of container {i}")
+        raise ValueError(f"region {r!r} is empty or leaves the {H} x {W} image {i}")
     return i, y, x, h, w
 
 
-def _plan(parsed, regions):
-    """(regions as int tuples, one RegionPlan per container) for unpack_container results.  Every region is checked here."""
-    regions = [_check_region(r, parsed) for r in regions]
-    boxes = collections.defaultdict(list)
+def _plan(job, regions):
+    """(regions as int tuples, RegionPlan over the job's chains and block sequence).  Every region is checked here."""
+    regions = [_check_region(r, job.shapes) for r in regions]
+    needed = np.zeros(int(job.ioff[-1]), dtype=bool)
     for i, y, x, h, w in regions:
-        boxes[i].append((y, x, h, w))
-    plans = []
-    for i, (_, _, _, nblocks, H, W) in enumerate(parsed):
-        gw = block_grid(H, W)[1]
-        needed = np.zeros(int(nblocks.sum()), dtype=bool)
-        grid = needed.reshape(-1, gw)
-        for y, x, h, w in boxes[i]:
-            grid[y // 32:(y + h - 1) // 32 + 1, x // 32:(x + w - 1) // 32 + 1] = True
-        starts = np.cumsum(nblocks) - nblocks
-        earliest = np.minimum.reduceat(np.where(needed, np.arange(needed.size), needed.size), starts)
-        first = np.minimum(earliest - starts, nblocks)
-        plans.append(RegionPlan(first, nblocks - first, needed))
-    return regions, plans
+        grid = needed[job.ioff[i]:job.ioff[i + 1]].reshape(-1, block_grid(*job.shapes[i])[1])
+        grid[y // 32:(y + h - 1) // 32 + 1, x // 32:(x + w - 1) // 32 + 1] = True
+    if not len(job.cnb):
+        return regions, RegionPlan(job.cnb.copy(), job.cnb.copy(), needed)
+    earliest = np.minimum.reduceat(np.where(needed, np.arange(needed.size), needed.size), job.cstart)
+    first = np.minimum(earliest - job.cstart, job.cnb)
+    return regions, RegionPlan(first, job.cnb - first, needed)
 
 
 def plan_regions(containers, regions, hwc_quirk=False):
     """The decode plan of decompress_regions, computed on the host alone: one RegionPlan per container.  regions: list of
     (i, y, x, h, w) in pixels of container i's decoded image (the cropped size for a crop-mode container).  A malformed
     container, or a region that is empty, leaves the image, has a non-int field or names no container, is a ValueError."""
-    parsed = [unpack_container(c, hwc_quirk) for c in containers]
-    return _plan(parsed, regions)[1]
+    job = _containers_job([unpack_container(c, hwc_quirk) for c in containers])
+    plan = _plan(job, regions)[1]
+    k = np.searchsorted(job.cstart, job.ioff)                     # container i's chains: k[i] to k[i + 1]
+    return [RegionPlan(plan.first[k[i]:k[i + 1]], plan.depth[k[i]:k[i + 1]], plan.needed[job.ioff[i]:job.ioff[i + 1]])
+            for i in range(len(job.shapes))]
 
 
 def decompress_regions(codec, containers, regions, channels=3, scheme=BITSWAP, hwc_quirk=False, headroom_words=None):
@@ -322,32 +359,31 @@ def decompress_regions(codec, containers, regions, channels=3, scheme=BITSWAP, h
     Only the chains holding a wanted block are imported, and each is popped only down to the earliest block any region on
     its container wants (plan_regions): a chain of n blocks whose earliest wanted block is j costs n - j block decodes.
     Blocks are row-major, so a window near an image's bottom is cheapest, and a single-chain container gains only there."""
-    parsed = [unpack_container(c, hwc_quirk) for c in containers]
-    return _decode_regions(codec, parsed, regions, channels, scheme, hwc_quirk, headroom_words)
+    job = _containers_job([unpack_container(c, hwc_quirk) for c in containers])
+    return _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_words)
 
 
 def decompress_images(codec, containers, channels=3, scheme=BITSWAP, hwc_quirk=False, headroom_words=None):
     """Inverse of compress_images: list of container arrays -> list of HWC uint8 images (the cropped size for a crop-mode
     container, the full size for an edge-coded one: a header whose h or w is not a multiple of 32).  Single- and
     multi-chain containers can be mixed in one call."""
-    parsed = [unpack_container(c, hwc_quirk) for c in containers]
-    return _decode_regions(codec, parsed, [(i, 0, 0, p[4], p[5]) for i, p in enumerate(parsed)], channels, scheme,
+    job = _containers_job([unpack_container(c, hwc_quirk) for c in containers])
+    return _decode_regions(codec, job, [(i, 0, 0, h, w) for i, (h, w) in enumerate(job.shapes)], channels, scheme,
                            hwc_quirk, headroom_words)
 
 
-def _decode_regions(codec, parsed, regions, channels, scheme, hwc_quirk, headroom_words):
-    regions, plans = _plan(parsed, regions)
+def _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_words, initial=None):
+    """Decodes the job's regions.  channels None: the codec's.  initial (words, head): the seeded initial state every chain
+    started from; each chain popped down to its first block must then hold its top words and head, or ValueError."""
+    regions, plan = _plan(job, regions)
     if not regions:
         return []
-    # chains in image and block order: image, index within the image, first block, blocks, blocks to pop
-    cimg = np.concatenate([np.full(len(p[3]), i) for i, p in enumerate(parsed)])
-    ck = np.concatenate([np.arange(len(p[3])) for p in parsed])
-    cstart = np.concatenate([np.cumsum(p[3]) - p[3] for p in parsed])
-    cnb = np.concatenate([p[3] for p in parsed])
-    cdepth = np.concatenate([pl.depth for pl in plans])
-    order = np.argsort(-cdepth, kind="stable")[:np.count_nonzero(cdepth)]   # streams: deepest chain first, skipped ones out
-    pieces = [parsed[i][0][parsed[i][1][k]:parsed[i][1][k + 1]] for i, k in zip(cimg[order], ck[order])]
-    depth = cdepth[order].tolist()
+    if channels is None:
+        channels = codec.cfg.xs[0]
+    cstart, cnb = job.cstart, job.cnb
+    order = np.argsort(-plan.depth, kind="stable")[:np.count_nonzero(plan.depth)]  # streams: deepest first, skipped ones out
+    pieces = [job.pieces[c] for c in order]
+    depth = plan.depth[order].tolist()
     n = len(depth)
     # The receiver pushes too (it returns the borrowed bits, cifar_compress.py:306-313): one block's worth of latents,
     # nz * zdim symbols at <= 31 bits each, can sit on the stack above the chain's own length.
@@ -356,14 +392,13 @@ def _decode_regions(codec, parsed, regions, channels, scheme, hwc_quirk, headroo
     ss = StreamSet(n, max(len(p) for p in pieces) + headroom_words, device=codec.device)
     offs = np.zeros(n + 1, dtype=np.int64)
     np.cumsum([len(p) for p in pieces], out=offs[1:])
-    ss.import_packed(np.concatenate(pieces), offs, np.array([parsed[i][2][k] for i, k in zip(cimg[order], ck[order])],
-                                                              dtype=np.uint64))
+    ss.import_packed(np.concatenate(pieces), offs, job.heads[order])
     # Steps are aligned at the chains' ends: step s pops block n - 1 - s of every stream deeper than s, so the active
     # streams stay a prefix and [s, stream] holds that block, in the output and in the extents alike.
     dev = torch.empty((max(depth), n, channels, 32, 32), dtype=torch.uint8, device=torch.device("cuda", codec.device))
-    extents = [block_extents(p[4], p[5]) for p in parsed]
-    ext = _extents_to_device(codec, [extents[i][s + nb - d:s + nb][::-1] for i, s, nb, d in
-                                     zip(cimg[order], cstart[order], cnb[order], depth)], depth)
+    extents = np.concatenate([block_extents(h, w) for h, w in job.shapes])
+    ext = _extents_to_device(codec, [extents[s + nb - d:s + nb][::-1] for s, nb, d in zip(cstart[order], cnb[order], depth)],
+                             depth)
     active = _active(depth)
     for s in range(max(depth)):
         for b, cnt in _sub_ranges(int(active[s]), codec.max_batch):
@@ -371,25 +406,142 @@ def _decode_regions(codec, parsed, regions, channels, scheme, hwc_quirk, headroo
                          extent=None if ext is None else ext[s, b:b + cnt])
     if hasattr(codec, "join"):                                             # (free-running multi-lane codec: lanes -> current stream)
         codec.join()
-    # the needed blocks of every image, gathered on the device into one transfer; pos[i][b]: block b's row in it
+    # the needed blocks, gathered on the device into one transfer; pos[b]: block b's row in it
     stream = np.full(len(cnb), -1, dtype=np.int64)
     stream[order] = np.arange(n)
-    first_chain = np.cumsum([0] + [len(p[3]) for p in parsed])
-    rows, pos, m = [], [], 0
-    for i, (p, pl) in enumerate(zip(parsed, plans)):
-        b = np.flatnonzero(pl.needed)
-        c = first_chain[i] + np.searchsorted(np.cumsum(p[3]), b, side="right")
-        rows.append((cstart[c] + cnb[c] - 1 - b) * n + stream[c])
-        pos.append(np.full(pl.needed.size, -1, dtype=np.int64))
-        pos[i][b] = m + np.arange(b.size)
-        m += b.size
-    idx = torch.from_numpy(np.concatenate(rows)).to(dev.device)
+    b = np.flatnonzero(plan.needed)
+    c = np.searchsorted(cstart + cnb, b, side="right")
+    pos = np.full(plan.needed.size, -1, dtype=np.int64)
+    pos[b] = np.arange(b.size)
+    idx = torch.from_numpy((cstart[c] + cnb[c] - 1 - b) * n + stream[c]).to(dev.device)
     host = _model_to_blocks(dev.view(-1, channels, 32, 32).index_select(0, idx).cpu().numpy(), hwc_quirk)
     ss.raise_on_error()
+    if initial is not None:
+        _check_initial_state(ss, order, plan.first[order] == 0, *initial)
     out = []
     for i, y, x, h, w in regions:
-        gw = block_grid(parsed[i][4], parsed[i][5])[1]
+        gw = block_grid(*job.shapes[i])[1]
         by, bx = np.arange(y // 32, (y + h - 1) // 32 + 1), np.arange(x // 32, (x + w - 1) // 32 + 1)
-        tile = unextract_blocks(host[pos[i][by[:, None] * gw + bx[None, :]].reshape(-1)], 32 * by.size, 32 * bx.size)
+        tile = unextract_blocks(host[pos[job.ioff[i] + by[:, None] * gw + bx[None, :]].reshape(-1)], 32 * by.size, 32 * bx.size)
         out.append(np.ascontiguousarray(tile[y - 32 * by[0]:y - 32 * by[0] + h, x - 32 * bx[0]:x - 32 * bx[0] + w]))
     return out
+
+
+def _check_initial_state(ss, order, done, words, head):
+    """A chain popped down to its first block holds what it started from: the top words of the seeded initial stack and
+    its head (cifar_compress.py:356).  done: bool per stream, the streams popped that far; order: each stream's chain."""
+    got, offs, heads, _ = ss.export()
+    for j in np.flatnonzero(done).tolist():
+        m = int(offs[j + 1] - offs[j])
+        if not (m <= words.size and int(heads[j]) == head and np.array_equal(got[offs[j]:offs[j + 1]], words[words.size - m:])):
+            raise ValueError(f"chain {int(order[j])} decoded to a state other than the initial one it was coded from: a "
+                             f"different model, bins or conv path than the encoder's, or a corrupt archive")
+
+
+def pack_archive(chains, shapes, excess_state_len, seed, scheme):
+    """An archive from its chains in block-sequence order, [(words uint32 [m], head int, nblocks)], and its images' (h, w):
+    [ words_0 ... words_{K-1} | (nwords_k, head_lo_k, head_hi_k, nblocks_k) for k < K | (h_i, w_i) for i < N
+    | K, N, excess_state_len, seed, scheme, ARCHIVE_MARK ]."""
+    table = np.array([(len(ws), hd & 0xffffffff, hd >> 32, nb) for ws, hd, nb in chains], dtype=np.uint32).reshape(-1)
+    return np.concatenate([np.asarray(ws, dtype=np.uint32) for ws, _, _ in chains]
+                          + [table, np.asarray(shapes, dtype=np.uint32).reshape(-1),
+                             np.array([len(chains), len(shapes), excess_state_len, seed, scheme, ARCHIVE_MARK], dtype=np.uint32)])
+
+
+def unpack_archive(a):
+    """Inverse of pack_archive: (words uint32, offsets int64 [K+1], heads uint64 [K], nblocks int64 [K], shapes int64 [N, 2],
+    excess_state_len, seed, scheme), chain k's words being words[offsets[k]:offsets[k+1]].  Every field is checked here,
+    before anything is sized from it: a truncated or inconsistent archive is a ValueError."""
+    a = np.asarray(a, dtype=np.uint32)
+    if a.ndim != 1 or a.size < 6 or int(a[-1]) != ARCHIVE_MARK:
+        raise ValueError("not an archive: it must be a 1-D uint32 array ending in ARCHIVE_MARK")
+    k, n, n_init, seed, scheme = (int(v) for v in a[-6:-1])
+    if k < 1 or n < 1 or a.size < 6 + 4 * k + 2 * n:
+        raise ValueError(f"archive of {a.size} words cannot hold the tables of its {k} chains and {n} images")
+    body = a.size - 6 - 4 * k - 2 * n
+    table = a[body:body + 4 * k].reshape(k, 4).astype(np.int64)
+    shapes = a[body + 4 * k:-6].reshape(n, 2).astype(np.int64)
+    if (shapes < 1).any():
+        raise ValueError("archive: an image with no pixels")
+    blocks = -(-shapes[:, 0] // 32) * -(-shapes[:, 1] // 32)
+    if (blocks > MAX_BLOCKS).any():
+        raise ValueError(f"archive: an image of more than {MAX_BLOCKS} blocks")
+    nwords, nblocks = table[:, 0], table[:, 3]
+    if (nblocks < 1).any():
+        raise ValueError("archive: a chain with no blocks")
+    if int(nblocks.sum()) != int(blocks.sum()) or int(blocks.sum()) > MAX_ARCHIVE_BLOCKS:
+        raise ValueError(f"archive: the chains hold {int(nblocks.sum())} blocks, the images {int(blocks.sum())} "
+                         f"(at most {MAX_ARCHIVE_BLOCKS})")
+    if int(nwords.sum()) != body:
+        raise ValueError(f"archive: the chains claim {int(nwords.sum())} words, the archive holds {body}")
+    if not 2 <= n_init <= MAX_INITIAL_WORDS:
+        raise ValueError(f"archive: excess_state_len {n_init} outside [2, {MAX_INITIAL_WORDS}]")
+    if scheme not in (BITSWAP, BBANS):
+        raise ValueError(f"archive: unknown scheme {scheme}")
+    offsets = np.zeros(k + 1, dtype=np.int64)
+    np.cumsum(nwords, out=offsets[1:])
+    heads = (table[:, 2].astype(np.uint64) << np.uint64(32)) | table[:, 1].astype(np.uint64)
+    return a[:body], offsets, heads, nblocks, shapes, n_init, seed, scheme
+
+
+def _archive_job(a):
+    words, offsets, heads, nblocks, shapes, n_init, seed, scheme = unpack_archive(a)
+    ioff = np.zeros(len(shapes) + 1, dtype=np.int64)
+    np.cumsum(-(-shapes[:, 0] // 32) * -(-shapes[:, 1] // 32), out=ioff[1:])
+    job = _Job([words[offsets[k]:offsets[k + 1]] for k in range(len(heads))], heads, np.cumsum(nblocks) - nblocks, nblocks,
+               [(int(h), int(w)) for h, w in shapes], ioff)
+    return job, n_init, seed, scheme
+
+
+def compress_archive(codec, images, chain_blocks=64, scheme=BITSWAP, excess_state_len=10000, seed=100, words_per_block=1400):
+    """images: a sequence of HWC uint8 arrays of any sizes (H, W >= 1, C = the model's) -> one np.uint32 archive.
+    Each image is tiled as compress_images(edges="code") tiles it; the row-major blocks of all images, in the order given,
+    form one sequence, cut into chain_sizes(total blocks, chain_blocks) contiguous runs, each coded as a chain from the seeded
+    initial state.  A chain may start or end inside an image, so the initial words are paid once per chain, not once per
+    image.  chain_blocks None: one chain over everything (the reference's experiment layout, cifar_compress.py)."""
+    chain_blocks = _check_chain_blocks(chain_blocks)
+    images = [np.asarray(im) for im in images]
+    if not images:
+        raise ValueError("an archive holds at least one image")
+    if scheme not in (BITSWAP, BBANS):
+        raise ValueError(f"scheme must be BITSWAP or BBANS, got {scheme!r}")
+    for name, v, lo, hi in (("excess_state_len", excess_state_len, 2, MAX_INITIAL_WORDS), ("seed", seed, 0, (1 << 32) - 1)):
+        if isinstance(v, bool) or not isinstance(v, numbers.Integral) or not lo <= v <= hi:
+            raise ValueError(f"{name} must be an int in [{lo}, {hi}], got {v!r}")
+    C = codec.cfg.xs[0]
+    for i, im in enumerate(images):
+        if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != C or im.shape[0] < 1 or im.shape[1] < 1:
+            raise ValueError(f"image {i}: expected an H x W x {C} uint8 array with H, W >= 1, got {im.dtype} {im.shape}")
+        if np.prod(block_grid(*im.shape[:2])) > MAX_BLOCKS:
+            raise ValueError(f"image {i} of {im.shape[0]} x {im.shape[1]} has more than {MAX_BLOCKS} blocks")
+    tiled = [extract_edge_blocks(im) for im in images]
+    total = sum(t[0].shape[0] for t in tiled)
+    if total > MAX_ARCHIVE_BLOCKS:
+        raise ValueError(f"the images hold {total} blocks, an archive at most {MAX_ARCHIVE_BLOCKS}")
+    sizes = chain_sizes(total, chain_blocks)
+    chains = list(zip(np.cumsum([0] + sizes[:-1]).tolist(), sizes))
+    blocks = np.concatenate([_blocks_to_model(t[0], False) for t in tiled])
+    coded = _encode(codec, blocks, np.concatenate([t[1] for t in tiled]), chains, scheme, int(excess_state_len), int(seed),
+                    words_per_block)
+    return pack_archive(coded, [(t[2], t[3]) for t in tiled], int(excess_state_len), int(seed), scheme)
+
+
+def plan_archive(archive, regions=None):
+    """The decode plan of decompress_archive, on the host alone: one RegionPlan over the archive's chains and its block
+    sequence (every image's row-major blocks in turn).  regions None: every image whole."""
+    job = _archive_job(archive)[0]
+    return _plan(job, _all_images(job) if regions is None else regions)[1]
+
+
+def decompress_archive(codec, archive, regions=None):
+    """regions None -> every image of the archive, exactly as given; else a list of (i, y, x, h, w) over image i -> one HWC
+    uint8 array per region, byte-identical to the crop of the full decode.  Each chain holding a wanted block is popped
+    from its end down to the earliest wanted block in it (plan_archive).  Every chain popped down to its first block must
+    come back to the seeded initial state it was coded from; otherwise ValueError naming the chain."""
+    job, n_init, seed, scheme = _archive_job(archive)
+    regions = _all_images(job) if regions is None else regions
+    return _decode_regions(codec, job, regions, None, scheme, False, None, initial=initial_words(n_init, seed=seed))
+
+
+def _all_images(job):
+    return [(i, 0, 0, h, w) for i, (h, w) in enumerate(job.shapes)]
