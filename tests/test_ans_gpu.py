@@ -18,6 +18,8 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
+from coder_harness import (check_vs_oracle, coder_paths, initial_states, level_case, oracle_tables, pad_big,   # noqa: E402
+                           ref_pmfs_cuda, run_2p, run_fused)
 from oracle import oracle as O                      # noqa: E402  (checker only)
 from bitswap_b200 import synthetic                   # noqa: E402
 from bitswap_b200._lib import lib, check, cuda_stream_ptr   # noqa: E402
@@ -106,8 +108,7 @@ def test_out_of_range_symbols_raise_index_error_like_the_reference():
         mu = np.zeros((B, L), dtype=np.float32); sc = np.full((B, L), 0.5, dtype=np.float32)
         s16 = np.tile((sym % 64).astype(np.int16), (B, 1)); s16[2, 5] = 64
         with pytest.raises(IndexError):
-            _run_2p(ends, mu, sc, 64, 6, [st] * B, s16, mode)
-        check(lib().bsw_set_rows_mode(-1))
+            run_2p(ends, mu, sc, 64, 6, [st] * B, s16, mode, cap=1 << 14)
 
 
 def test_bad_arguments_are_rejected():
@@ -142,10 +143,7 @@ def test_p0_batched_coder_vs_oracle(B, L, S, shared):
     P = torch.from_numpy(np.stack([t[0] for t in tabs]).astype(np.uint32).view(np.int32)).to(dev)
     C = torch.from_numpy(np.stack([t[1] for t in tabs]).astype(np.uint32).view(np.int32)).to(dev)
     sym = rs.randint(0, S, size=(B, L)).astype(np.int32)
-    states = []
-    for b in range(B):
-        w, head = synthetic.initial_words(400 + 13 * b, seed=100 + b)
-        states.append([int(v) for v in w] + [head])
+    states = initial_states(B, seed=100, n=400, step=13)
     ss = StreamSet(B, 4096)
     ss.import_lists(states)
     pss, css = (0, 0) if shared else (L * S, L * (S + 1))
@@ -180,14 +178,6 @@ def test_p0_batched_coder_vs_oracle(B, L, S, shared):
             assert got[b] == states[b]
 
 
-def _ref_pmfs_cuda(ends, mu, sc):
-    """The reference's tensor expression (cifar_compress.py:182-184) evaluated by torch ON THE GPU, as the
-    reference itself runs it (device = cuda, cifar_compress.py:77)."""
-    cdfs = torch.sigmoid((ends.t() - mu) / sc).t()
-    pmfs = cdfs[:, 1:] - cdfs[:, :-1]
-    return torch.cat((cdfs[:, 0].unsqueeze(1), pmfs, 1. - cdfs[:, -1].unsqueeze(1)), dim=1)
-
-
 def test_p2_logistic_pmfs():
     g = np.load(os.path.join(GOLDEN, "pmfs_small.npz"))
     for ends, mu, sc, want in ((g["ends"], g["mu"], g["sc"], g["pm"]), (g["xe"], g["xmu"], g["xsc"], g["xpm"]),
@@ -198,7 +188,7 @@ def test_p2_logistic_pmfs():
         check(lib().bsw_logistic_pmfs(e.data_ptr(), S - 1, m.data_ptr(), s.data_ptr(), 1 if m.numel() > 1 else 0, L, S,
                                       out.data_ptr(), cuda_stream_ptr()))
         assert np.abs(out.cpu().numpy() - want).max() <= 4e-16          # vs torch-CPU (reference classes) golden
-        assert torch.equal(out, _ref_pmfs_cuda(e, m, s))                  # vs the reference expression on this GPU
+        assert torch.equal(out, ref_pmfs_cuda(e, m, s))                  # vs the reference expression on this GPU
     # a full-size level: 2048 x 1024, bit-exact against torch-CUDA
     rs = np.random.RandomState(1)
     L, S = 2048, 1024
@@ -208,7 +198,7 @@ def test_p2_logistic_pmfs():
     s = torch.from_numpy(rs.uniform(0.1, 1.0, L).astype(np.float32)).double().to(dev)
     out = torch.empty((L, S), dtype=torch.float64, device=dev)
     check(lib().bsw_logistic_pmfs(e.data_ptr(), S - 1, m.data_ptr(), s.data_ptr(), 1, L, S, out.data_ptr(), cuda_stream_ptr()))
-    ref = _ref_pmfs_cuda(e, m, s)
+    ref = ref_pmfs_cuda(e, m, s)
     assert torch.equal(out, ref), f"{(out != ref).sum().item()} of {out.numel()} pmfs differ from torch-CUDA"
 
 
@@ -243,21 +233,10 @@ def test_p2_fused_logistic_coder_vs_oracle_on_our_pmfs(B, L, S, q, kind):
     e_raw = torch.from_numpy(np.ascontiguousarray(ends_rows)).to(dev)
     dmu, dsc = torch.from_numpy(mu).to(dev), torch.from_numpy(sc).to(dev)
     dsc_arg = dsc[:1].contiguous() if kind == "x" else dsc
-    states = []
-    for b in range(B):
-        w, head = synthetic.initial_words(1500 + 7 * b, seed=100 + b)
-        states.append([int(v) for v in w] + [head])
+    states = initial_states(B, seed=100, n=1500)
     ss = StreamSet(B, 1 << 14)
     ss.import_lists(states)
-    # oracle side, on OUR pmfs
-    tabs = []
-    for b in range(B):
-        pm = torch.empty((L, S), dtype=torch.float64, device=dev)
-        mu64, sc64 = dmu[b].double().contiguous(), dsc[b].double().contiguous()     # keep alive across the call
-        check(lib().bsw_logistic_pmfs(e_raw.data_ptr(), S - 1, mu64.data_ptr(), sc64.data_ptr(), 1, L, S,
-                                      pm.data_ptr(), cuda_stream_ptr()))
-        torch.cuda.synchronize()
-        tabs.append(O.tables_c(pm.cpu().numpy(), 31, q))
+    tabs = oracle_tables(ends_rows, mu, sc, S, q)                   # oracle side, on OUR pmfs
     # pop first (bits-back), then push other symbols
     out = torch.zeros((B, L), dtype=torch.int16, device=dev)
     check(lib().bsw_logistic_pop(ss.handle, 0, B, dmu.data_ptr(), L, dsc_arg.data_ptr(), sss, e_pad.data_ptr(), ers,
@@ -346,13 +325,6 @@ def test_packed_export_import_roundtrip():
     assert np.array_equal(sub_o, o[5:15] - o[5]) and np.array_equal(sub_w, w[o[5]:o[14]])
 
 
-def _pad_big(ends):
-    L, Sm1 = ends.shape
-    out = np.full((L, Sm1 + 1), 1e300)
-    out[:, :Sm1] = ends
-    return out
-
-
 @pytest.mark.parametrize("S,q,mode", [(1024, 10, 0), (1024, 10, -1), (1024, 10, 1), (256, 8, 0), (256, 8, -1), (128, 7, -1), (128, 7, 0),
                                       (64, 6, 0), (64, 6, -1), (32, 5, 0), (32, 5, -1), (512, 9, 0), (512, 9, -1), (512, 9, 1),
                                       (16, 4, -1), (16, 4, 1), (8, 3, -1), (8, 3, 1)])
@@ -362,9 +334,7 @@ def test_two_phase_abi_extreme_tables_vs_fused_and_oracle(S, q, mode):
     outside the bin range, symbols in the dead tails, plus ordinary rows.  mode 0 = generic kernels (k_rows/k_pop_coarse),
     -1 = classify the rows (uniform grids here -> the affine-row kernels k_rows6/k_pop6), 1 = affine kernels forced.
     S = 8 and 16 exist for the affine kernels only (the generic and fused ones own S/32 bins per lane): oracle alone."""
-    check(lib().bsw_set_rows_mode(mode))
-    full = 0
-    rs = np.random.RandomState(S + full)
+    rs = np.random.RandomState(S)
     B, L = 9, 96
     lo, hi = -6 - rs.uniform(0, 1, L), 6 + rs.uniform(0, 1, L)
     ends = np.linspace(lo, hi, S + 1, axis=1)[:, 1:-1].copy()
@@ -372,54 +342,15 @@ def test_two_phase_abi_extreme_tables_vs_fused_and_oracle(S, q, mode):
     sc = rs.uniform(0.1, 1.0, (B, L)).astype(np.float32)
     sc[:, 0::4] = np.float32((2. / 255.) / 8.)                 # needle-sharp rows
     mu[:, 1::8] = rs.choice([-25.0, 25.0, -7.5, 7.5], size=mu[:, 1::8].shape).astype(np.float32)    # mass outside the bins
-    e_pad = torch.from_numpy(_pad_big(ends)).to(dev)
-    e_raw = torch.from_numpy(ends).to(dev)
-    dmu, dsc = torch.from_numpy(mu).to(dev), torch.from_numpy(sc).to(dev)
-    nbytes = int(lib().bsw_logistic_scratch_bytes(B, L, S, full))
-    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    states = []
-    for b in range(B):
-        w, head = synthetic.initial_words(3000 + b, seed=500 + b)
-        states.append([int(v) for v in w] + [head])
-    tabs = []
-    for b in range(B):
-        pm = torch.empty((L, S), dtype=torch.float64, device=dev)
-        m64, s64 = dmu[b].double().contiguous(), dsc[b].double().contiguous()
-        check(lib().bsw_logistic_pmfs(e_raw.data_ptr(), S - 1, m64.data_ptr(), s64.data_ptr(), 1, L, S, pm.data_ptr(), cuda_stream_ptr()))
-        torch.cuda.synchronize()
-        tabs.append(O.tables_c(pm.cpu().numpy(), 31, q))
+    states = initial_states(B, seed=500, n=3000, step=1)
+    tabs = oracle_tables(ends, mu, sc, S, q)
     sym = rs.randint(0, S, size=(B, L)).astype(np.int16)
     sym[:, :6] = [0, S - 1, 1, S - 2, S // 2, 0]
-    dsym = torch.from_numpy(sym).to(dev)
-    res = {}
-    for name in ("2p", "fused") if S >= 32 else ("2p",):
-        ss = StreamSet(B, 1 << 14)
-        ss.import_lists(states)
-        out = torch.zeros((B, L), dtype=torch.int16, device=dev)
-        if name == "2p":
-            check(lib().bsw_logistic_pop_2p(ss.handle, 0, B, dmu.data_ptr(), L, dsc.data_ptr(), L, e_pad.data_ptr(), S, out.data_ptr(),
-                                            L, S, 31, q, scratch.data_ptr(), nbytes, cuda_stream_ptr()))
-        else:
-            check(lib().bsw_logistic_pop(ss.handle, 0, B, dmu.data_ptr(), L, dsc.data_ptr(), L, e_pad.data_ptr(), S, out.data_ptr(),
-                                         L, S, 31, q, cuda_stream_ptr()))
-        ss.raise_on_error()
-        after_pop, popped = ss.export_lists(), out.cpu().numpy().copy()
-        if name == "2p":
-            check(lib().bsw_logistic_push_2p(ss.handle, 0, B, dmu.data_ptr(), L, dsc.data_ptr(), L, e_pad.data_ptr(), S, dsym.data_ptr(),
-                                             L, S, 31, q, scratch.data_ptr(), nbytes, cuda_stream_ptr()))
-        else:
-            check(lib().bsw_logistic_push(ss.handle, 0, B, dmu.data_ptr(), L, dsc.data_ptr(), L, e_pad.data_ptr(), S, dsym.data_ptr(),
-                                          L, S, 31, q, cuda_stream_ptr()))
-        ss.raise_on_error()
-        res[name] = (after_pop, popped, ss.export_lists())
-    check(lib().bsw_set_rows_mode(-1))
+    res = run_2p(ends, mu, sc, S, q, states, sym, mode, cap=1 << 14)
     if S >= 32:
-        assert res["2p"][0] == res["fused"][0] and np.array_equal(res["2p"][1], res["fused"][1]) and res["2p"][2] == res["fused"][2]
-    for b in range(B):
-        a = O.AnsC(tables=tabs[b])
-        st, s_ = a.decode(O.CState.from_list(states[b]))
-        assert np.array_equal(res["2p"][1][b], s_) and res["2p"][0][b] == st.to_list()
-        assert res["2p"][2][b] == a.encode(st, sym[b].astype(np.int64)).to_list()
+        fused = run_fused(ends, mu, sc, S, q, states, sym, cap=1 << 14)
+        assert res[0] == fused[0] and np.array_equal(res[1], fused[1]) and res[2] == fused[2]
+    check_vs_oracle(res, tabs, states, sym, range(B))
 
 
 @pytest.mark.parametrize("mode", [0, -1, 1])
@@ -427,31 +358,25 @@ def test_two_phase_abi_extreme_tables_vs_fused_and_oracle(S, q, mode):
 def test_two_phase_abi_refuses_bits_out_of_range(bits, q, mode):
     """The two-phase coder codes 1 <= bits <= 31 and 0 <= quantbits < bits, like the fused one: anything else is
     BSW_E_INVALID before any coder kernel runs, for every kernel family, and the streams are left as they were."""
-    check(lib().bsw_set_rows_mode(mode))
     B, L, S = 3, 40, 1024
     rs = np.random.RandomState(7)
     ends = np.linspace(-6, 6, S + 1)[1:-1]
-    e_pad = torch.from_numpy(_pad_big(np.tile(ends, (L, 1)))).to(dev)
+    e_pad = torch.from_numpy(pad_big(np.tile(ends, (L, 1)))).to(dev)
     dmu = torch.from_numpy(rs.normal(0, 1, (B, L)).astype(np.float32)).to(dev)
     dsc = torch.from_numpy(rs.uniform(0.1, 1.0, (B, L)).astype(np.float32)).to(dev)
     sym = torch.from_numpy(rs.randint(0, S, size=(B, L)).astype(np.int16)).to(dev)
     nbytes = int(lib().bsw_logistic_scratch_bytes(B, L, S, 0))
     scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    states = []
-    for b in range(B):
-        w, head = synthetic.initial_words(500 + b, seed=40 + b)
-        states.append([int(v) for v in w] + [head])
+    states = initial_states(B, seed=40, n=500, step=1)
     ss = StreamSet(B, 1 << 12)
     ss.import_lists(states)
-    try:
+    with coder_paths(rows_mode=mode):
         for fn, s_ in ((lib().bsw_logistic_push_2p, sym), (lib().bsw_logistic_pop_2p, sym.clone())):
             rc = fn(ss.handle, 0, B, dmu.data_ptr(), L, dsc.data_ptr(), L, e_pad.data_ptr(), S, s_.data_ptr(), L, S, bits, q,
                     scratch.data_ptr(), nbytes, cuda_stream_ptr())
             assert rc == 4, (fn, rc)
             assert b"out of range" in lib().bsw_last_error()
         torch.cuda.synchronize()
-    finally:
-        check(lib().bsw_set_rows_mode(-1))
     assert ss.export_lists() == states
     assert not ss.sizes()[2].any()
 
@@ -466,41 +391,6 @@ def test_screening_cdf_error_is_far_inside_the_window():
     assert worst.value < 8.0
 
 
-def _level_case(L, S, q, B, seed, affine=True, sc_lo=0.1):
-    rs = np.random.RandomState(seed)
-    if affine:
-        lo, hi = -6 - rs.uniform(0, 1, L), 6 + rs.uniform(0, 1, L)
-        ends = np.linspace(lo, hi, S + 1, axis=1)[:, 1:-1].copy()
-    else:                                                   # the top level: equal-mass logistic bins, float32 (discretization.py:25-27)
-        from bitswap_b200.rand import Bins
-        ends = Bins(torch.zeros((1, 1, L)), torch.ones((1, 1, L)), q).endpoints().numpy().reshape(L, S - 1).astype(np.float64)
-    mu = rs.normal(0, 1.5, (B, L)).astype(np.float32)
-    sc = rs.uniform(sc_lo, 1.0, (B, L)).astype(np.float32)
-    return ends, mu, sc
-
-
-def _run_2p(ends, mu, sc, S, q, states, sym, mode):
-    """pop then push of one level through the two-phase ABI; returns (states after pop, popped symbols, states after push)."""
-    B, L = mu.shape
-    check(lib().bsw_set_rows_mode(mode))
-    e_pad = torch.from_numpy(_pad_big(ends)).to(dev)
-    dmu, dsc, dsym = torch.from_numpy(mu).to(dev), torch.from_numpy(sc).to(dev), torch.from_numpy(sym).to(dev)
-    nbytes = int(lib().bsw_logistic_scratch_bytes(B, L, S, 0))
-    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    ss = StreamSet(B, 1 << 14)
-    ss.import_lists(states)
-    out = torch.zeros((B, L), dtype=torch.int16, device=dev)
-    check(lib().bsw_logistic_pop_2p(ss.handle, 0, B, dmu.data_ptr(), L, dsc.data_ptr(), L, e_pad.data_ptr(), S, out.data_ptr(),
-                                    L, S, 31, q, scratch.data_ptr(), nbytes, cuda_stream_ptr()))
-    ss.raise_on_error()
-    a, popped = ss.export_lists(), out.cpu().numpy().copy()
-    check(lib().bsw_logistic_push_2p(ss.handle, 0, B, dmu.data_ptr(), L, dsc.data_ptr(), L, e_pad.data_ptr(), S, dsym.data_ptr(),
-                                     L, S, 31, q, scratch.data_ptr(), nbytes, cuda_stream_ptr()))
-    ss.raise_on_error()
-    check(lib().bsw_set_rows_mode(-1))
-    return a, popped, ss.export_lists()
-
-
 def test_affine_rows_full_size_level_every_bin_verified_against_the_exact_function():
     """VERDICT r1 weak #3: the screened table kernels are sound only if every integer they emit is the exact function's.
     A full-size latent level (2048 rows x 1024 bins, q = 10, sigma down to the 0.1 floor) is run through k_rows6 in
@@ -508,28 +398,22 @@ def test_affine_rows_full_size_level_every_bin_verified_against_the_exact_functi
     screened value: 0 disagreements, the worst screening error of a trusted bin below a quarter of its window, and the
     streams equal what the generic kernels leave."""
     L, S, q, B = 2048, 1024, 10, 16
-    ends, mu, sc = _level_case(L, S, q, B, seed=3)
+    ends, mu, sc = level_case(L, S, q, B, seed=3)
     sc[:, ::7] = np.float32(0.1)
     mu[:, ::11] *= 3
     rs = np.random.RandomState(5)
     sym = rs.randint(0, S, size=(B, L)).astype(np.int16)
-    states = []
-    for b in range(B):
-        w, head = synthetic.initial_words(6000 + b, seed=700 + b)
-        states.append([int(v) for v in w] + [head])
-    check(lib().bsw_rows6_set_verify(1))
+    states = initial_states(B, seed=700, n=6000, step=1)
     stats = np.zeros(4, dtype=np.uint64)
-    try:
-        got = _run_2p(ends, mu, sc, S, q, states, sym, mode=-1)
+    with coder_paths(verify=1):
+        got = run_2p(ends, mu, sc, S, q, states, sym, mode=-1, cap=1 << 14)
         check(lib().bsw_rows6_verify_read(stats.ctypes.data))
-    finally:
-        check(lib().bsw_rows6_set_verify(0))
     mism, worst, checked, exact_path = (int(v) for v in stats)
     print(f"verify: {checked} bins evaluated of {2 * B * L * S}, {exact_path} took the exact path, worst trusted error "
           f"{worst / 10:.1f} % of the window, {mism} mismatches")
     assert checked > 0.25 * 2 * B * L * S and mism == 0
     assert worst <= 250, worst                            # a trusted bin's error must stay below a quarter of its window
-    ref = _run_2p(ends, mu, sc, S, q, states, sym, mode=0)
+    ref = run_2p(ends, mu, sc, S, q, states, sym, mode=0, cap=1 << 14)
     assert got[0] == ref[0] and np.array_equal(got[1], ref[1]) and got[2] == ref[2]
 
 
@@ -537,15 +421,12 @@ def test_affine_kernels_forced_on_non_uniform_rows_fall_back_to_the_exact_functi
     """mode 1 pushes the equal-mass top-level rows (not a uniform grid) through k_rows6/k_pop6: the plan refuses to
     vouch for them (mask = 0) and every bin takes the exact path -- same streams as the generic kernels."""
     L, S, q, B = 96, 1024, 10, 5
-    ends, mu, sc = _level_case(L, S, q, B, seed=9, affine=False)
+    ends, mu, sc = level_case(L, S, q, B, seed=9, affine=False)
     sym = np.random.RandomState(1).randint(0, S, size=(B, L)).astype(np.int16)
-    states = []
-    for b in range(B):
-        w, head = synthetic.initial_words(3000 + b, seed=800 + b)
-        states.append([int(v) for v in w] + [head])
-    a = _run_2p(ends, mu, sc, S, q, states, sym, mode=1)
-    b = _run_2p(ends, mu, sc, S, q, states, sym, mode=0)
-    c = _run_2p(ends, mu, sc, S, q, states, sym, mode=-1)       # classification -> generic
+    states = initial_states(B, seed=800, n=3000, step=1)
+    a = run_2p(ends, mu, sc, S, q, states, sym, mode=1, cap=1 << 14)
+    b = run_2p(ends, mu, sc, S, q, states, sym, mode=0, cap=1 << 14)
+    c = run_2p(ends, mu, sc, S, q, states, sym, mode=-1, cap=1 << 14)       # classification -> generic
     assert a[0] == b[0] == c[0] and np.array_equal(a[1], b[1]) and a[2] == b[2] == c[2]
 
 
@@ -558,37 +439,21 @@ def test_affine_rows_mapping_does_not_change_the_integers(L, S, q):
     tails (needle-sharp rows) and symbols in them.  The reference is the generic kernels' run; at S = 8 and 16, which only
     the affine kernels code, it is the oracle coder on our exported pmfs."""
     B = 5
-    ends, mu, sc = _level_case(L, S, q, B, seed=17)
+    ends, mu, sc = level_case(L, S, q, B, seed=17)
     sc[:, ::5] = np.float32((2. / 255.) / 8.)
     mu[:, 1::9] *= 4
     rs = np.random.RandomState(23)
     sym = rs.randint(0, S, size=(B, L)).astype(np.int16)
     sym[:, :4] = [0, S - 1, 1, S // 2]
-    states = []
-    for b in range(B):
-        w, head = synthetic.initial_words(7000 + b, seed=900 + b)
-        states.append([int(v) for v in w] + [head])
+    states = initial_states(B, seed=900, n=7000, step=1)
     res = {}
-    try:
-        for lpr in (32, 8, 4, 2):
-            check(lib().bsw_rows6_set_lanes_per_row(lpr))
-            res[lpr] = _run_2p(ends, mu, sc, S, q, states, sym, mode=1)
-    finally:
-        check(lib().bsw_rows6_set_lanes_per_row(0))
+    for lpr in (32, 8, 4, 2):
+        with coder_paths(lanes_per_row=lpr):
+            res[lpr] = run_2p(ends, mu, sc, S, q, states, sym, mode=1, cap=1 << 14)
     if S >= 32:
-        ref = _run_2p(ends, mu, sc, S, q, states, sym, mode=0)
+        ref = run_2p(ends, mu, sc, S, q, states, sym, mode=0, cap=1 << 14)
     else:
         ref = res[32]
-        e_raw = torch.from_numpy(np.ascontiguousarray(ends)).to(dev)
-        for b in range(B):
-            pm = torch.empty((L, S), dtype=torch.float64, device=dev)
-            m64, s64 = torch.from_numpy(mu[b]).double().to(dev), torch.from_numpy(sc[b]).double().to(dev)
-            check(lib().bsw_logistic_pmfs(e_raw.data_ptr(), S - 1, m64.data_ptr(), s64.data_ptr(), 1, L, S, pm.data_ptr(),
-                                          cuda_stream_ptr()))
-            torch.cuda.synchronize()
-            a = O.AnsC(tables=O.tables_c(pm.cpu().numpy(), 31, q))
-            st, s_ = a.decode(O.CState.from_list(states[b]))
-            assert np.array_equal(ref[1][b], s_) and ref[0][b] == st.to_list(), f"stream {b}: pop differs from the oracle"
-            assert ref[2][b] == a.encode(st, sym[b].astype(np.int64)).to_list(), f"stream {b}: push differs from the oracle"
+        check_vs_oracle(ref, oracle_tables(ends, mu, sc, S, q), states, sym, range(B))
     for lpr, got in res.items():
         assert got[0] == ref[0] and np.array_equal(got[1], ref[1]) and got[2] == ref[2], f"lanes per row = {lpr}"

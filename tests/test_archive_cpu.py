@@ -5,18 +5,12 @@ import types
 import numpy as np
 import pytest
 
+from codec_harness import NoDevice
 from bitswap_b200 import container
 from bitswap_b200.codec import BBANS, BITSWAP
 from bitswap_b200.container import (ARCHIVE_MARK, CHAIN_MARK, MAX_BLOCKS, block_grid, chain_sizes, compress_archive,
                                     decompress_archive, extract_edge_blocks, pack_archive, plan_archive, unpack_archive,
                                     unpack_container)
-
-
-class NoDevice:
-    """A codec stand-in that fails the test if anything on it is touched."""
-
-    def __getattr__(self, name):
-        raise AssertionError(f"codec.{name} touched")
 
 
 def _blocks(h, w):

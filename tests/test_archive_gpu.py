@@ -11,7 +11,7 @@ pytestmark = pytest.mark.gpu
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from test_chains_gpu import _gpu_oracle, _lone_chain, _oracle_chain, _setup   # noqa: E402
+from codec_harness import Counting, chains_of, gpu_oracle, lone_chain, oracle_chain, random_images, setup   # noqa: E402
 from bitswap_b200 import container, synthetic                              # noqa: E402
 from bitswap_b200.config import preset                                     # noqa: E402
 from bitswap_b200.model import Model                                       # noqa: E402
@@ -23,36 +23,10 @@ N_INIT = 3000
 SIZES = [(1, 1), (100, 70), (28, 28), (33, 65), (5, 40), (64, 31)]          # 1 + 12 + 1 + 6 + 2 + 2 = 24 blocks
 
 
-def _images(C, sizes, seed):
-    rs = np.random.RandomState(seed)
-    return [rs.randint(0, 256, (h, w, C)).astype(np.uint8) for h, w in sizes]
-
-
 def _sequence(images):
     """(blocks [n, 32, 32, C], extents [n, 2]) of the archive's global block sequence."""
     tiles = [extract_edge_blocks(im) for im in images]
     return np.concatenate([t[0] for t in tiles]), np.concatenate([t[1] for t in tiles])
-
-
-def _chains_of(a):
-    """[(words, head, nblocks)] of an archive, in sequence order."""
-    words, offs, heads, nblocks = unpack_archive(a)[:4]
-    return [(words[offs[k]:offs[k + 1]], int(heads[k]), int(nblocks[k])) for k in range(len(heads))]
-
-
-class Counting:
-    """Codec proxy counting decode calls and the blocks they pop."""
-
-    def __init__(self, codec):
-        self.codec, self.calls, self.blocks = codec, 0, 0
-
-    def __getattr__(self, name):
-        return getattr(self.codec, name)
-
-    def decode(self, ss, count, **kw):
-        self.calls += 1
-        self.blocks += count
-        return self.codec.decode(ss, count, **kw)
 
 
 def _planned_calls(plan, max_batch):
@@ -61,42 +35,38 @@ def _planned_calls(plan, max_batch):
 
 @pytest.mark.parametrize("name,scheme", [("tiny", BITSWAP), ("tiny", BBANS), ("tiny3", BITSWAP), ("tiny3", BBANS)])
 def test_round_trips_and_every_chain_equals_the_oracle(name, scheme):
-    cfg, m, sd, zend, zcen, bins = _setup(name, 16)
-    codec = BitSwapCodec(cfg, m, bins, 16)
-    images = _images(cfg.xs[0], SIZES, seed=71)
+    cfg, m, sd, zend, zcen, bins, codec = setup(name, 16)
+    images = random_images(cfg.xs[0], SIZES, seed=71)
     blocks, ext = _sequence(images)
-    orc = _gpu_oracle(cfg, m, sd, zend, zcen)
+    orc = gpu_oracle(cfg, m, sd, zend, zcen)
     for L in (None, 1, 3, 7):
         a = compress_archive(codec, images, chain_blocks=L, scheme=scheme, excess_state_len=N_INIT)
         back = decompress_archive(codec, a)
         assert len(back) == len(images)
         assert all(b.shape == im.shape and np.array_equal(b, im) for b, im in zip(back, images)), L
-        chains = _chains_of(a)
+        chains = chains_of(unpack_archive(a))
         assert [nb for _, _, nb in chains] == chain_sizes(len(blocks), L)
         s = 0
         for k, (ws, hd, nb) in enumerate(chains):
-            ow, oh = _oracle_chain(orc, blocks[s:s + nb], ext[s:s + nb], scheme)
+            ow, oh = oracle_chain(orc, blocks[s:s + nb], ext[s:s + nb], scheme)
             assert np.array_equal(ws, ow) and hd == oh, (L, k)
             s += nb
 
 
 @pytest.mark.parametrize("L", [None, 1, 4, 5])
 def test_an_archive_of_one_image_holds_the_containers_chains(L):
-    cfg, m, sd, zend, zcen, bins = _setup("tiny3", 8)
-    codec = BitSwapCodec(cfg, m, bins, 8)
-    img = _images(3, [(100, 130)], seed=73)                                     # 4 x 5 blocks
+    cfg, m, sd, zend, zcen, bins, codec = setup("tiny3", 8)
+    img = random_images(3, [(100, 130)], seed=73)                                     # 4 x 5 blocks
     a = compress_archive(codec, img, chain_blocks=L, excess_state_len=N_INIT)
     (c,) = compress_images(codec, img, excess_state_len=N_INIT, edges="code", chain_blocks=L)
-    words, offs, heads, nblocks, _, _ = unpack_container(c)
-    want = [(words[offs[k]:offs[k + 1]], int(heads[k]), int(nblocks[k])) for k in range(len(heads))]
-    got = _chains_of(a)
+    want = chains_of(unpack_container(c))
+    got = chains_of(unpack_archive(a))
     assert len(got) == len(want) and all(np.array_equal(g[0], w[0]) and g[1:] == w[1:] for g, w in zip(got, want))
 
 
 def test_regions_equal_crops_of_the_full_decode_with_the_planned_pops():
-    cfg, m, sd, zend, zcen, bins = _setup("tiny", 8)
-    codec = BitSwapCodec(cfg, m, bins, 8)
-    images = _images(1, SIZES + [(90, 40), (1, 100)], seed=75)
+    cfg, m, sd, zend, zcen, bins, codec = setup("tiny", 8)
+    images = random_images(1, SIZES + [(90, 40), (1, 100)], seed=75)
     rs = np.random.RandomState(76)
     for L in (None, 3, 5):
         a = compress_archive(codec, images, chain_blocks=L, scheme=BBANS, excess_state_len=N_INIT)
@@ -126,11 +96,11 @@ def test_regions_equal_crops_of_the_full_decode_with_the_planned_pops():
 def test_more_chains_than_max_batch_and_a_free_running_pipelined_codec(scheme):
     """25 chains through max_batch 24 (two calls per step), max_batch 8 (four) and a free-running 2-lane PipelinedCodec of
     max_batch 8 write the same archive and decode it exactly."""
-    cfg, m, sd, zend, zcen, bins = _setup("tiny3", 24)
-    images = _images(3, [(150, 390), (33, 65), (1, 1), (28, 28)], seed=77)       # 65 + 6 + 1 + 1 = 73 blocks
+    cfg, m, sd, zend, zcen, bins, codec = setup("tiny3", 24)
+    images = random_images(3, [(150, 390), (33, 65), (1, 1), (28, 28)], seed=77)       # 65 + 6 + 1 + 1 = 73 blocks
     kw = dict(chain_blocks=3, scheme=scheme, excess_state_len=N_INIT)
-    want = compress_archive(BitSwapCodec(cfg, m, bins, 24), images, **kw)
-    assert len(_chains_of(want)) == 25
+    want = compress_archive(codec, images, **kw)
+    assert len(chains_of(unpack_archive(want))) == 25
     pc = PipelinedCodec(cfg, sd, bins, 8, lanes=2, use_tensor_cores=False, free_running=True)
     for codec in (BitSwapCodec(cfg, m, bins, 8), pc):
         got = compress_archive(codec, images, **kw)
@@ -150,16 +120,16 @@ def test_imagenetcrop4_tensor_cores_each_chain_equals_a_lone_chain():
     pc = PipelinedCodec(cfg, sd, bins, 8, lanes=2, use_tensor_cores=True, free_running=True)
     rs = np.random.RandomState(79)
     sizes = [(int(rs.randint(1, 70)), int(rs.randint(1, 70))) for _ in range(30)]
-    images = _images(3, sizes, seed=80)
+    images = random_images(3, sizes, seed=80)
     blocks, ext = _sequence(images)
     a = compress_archive(pc, images, chain_blocks=8, excess_state_len=4000)
     back = decompress_archive(pc, a)
     assert all(np.array_equal(b, im) for b, im in zip(back, images))
-    chains = _chains_of(a)
+    chains = chains_of(unpack_archive(a))
     assert [nb for _, _, nb in chains] == chain_sizes(len(blocks), 8) and len(chains) >= 4
     s = 0
     for k, (ws, hd, nb) in enumerate(chains):
-        lw, lh = _lone_chain(pc, blocks[s:s + nb], ext[s:s + nb], BITSWAP)
+        lw, lh = lone_chain(pc, blocks[s:s + nb], ext[s:s + nb], BITSWAP)
         assert np.array_equal(ws, lw) and hd == lh, k
         s += nb
 
@@ -173,11 +143,10 @@ def _flip_head_lo(a, k):
 
 
 def test_the_initial_state_check():
-    cfg, m, sd, zend, zcen, bins = _setup("tiny3", 8)
-    codec = BitSwapCodec(cfg, m, bins, 8)
-    images = _images(3, SIZES, seed=81)
+    cfg, m, sd, zend, zcen, bins, codec = setup("tiny3", 8)
+    images = random_images(3, SIZES, seed=81)
     a = compress_archive(codec, images, chain_blocks=5, excess_state_len=N_INIT)     # 24 blocks: chains of 5, 5, 5, 5, 4
-    assert [nb for _, _, nb in _chains_of(a)] == [5, 5, 5, 5, 4]
+    assert [nb for _, _, nb in chains_of(unpack_archive(a))] == [5, 5, 5, 5, 4]
     # a codec built from other weights decodes other symbols: a chain does not come back to its initial state (or, checked
     # first, the stream flags report a pop past its stack or a symbol outside its table)
     sd51 = synthetic.synthetic_state_dict(cfg, seed=51, varied=True)

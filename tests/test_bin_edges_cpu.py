@@ -3,224 +3,15 @@ pinned here without a GPU.
 
 A pop reads mm = x & (2^31 - 1) and picks the bin with searchsorted(C[:-1], mm, 'right') - 1; a head drawn at random sits on a
 given bin edge with probability 2^-31, so random states say nothing about the comparisons that decide edges (`<=` against
-`<`) or the renormalisation thresholds (x < 2^32 after a pop, x >= 2^33 P[s] before a push).  The head builder below puts a
-head exactly on those values, and the vectorised coder below is the reference's ANS.encode / ANS.decode (cifar_compress.py
-:48-67) for N streams at once, checked here against the literal port (AnsPort) and the C oracle (AnsC)."""
-import os
-import sys
-
+`<`) or the renormalisation thresholds (x < 2^32 after a pop, x >= 2^33 P[s] before a push).  The head builder of
+coder_harness.py puts a head exactly on those values, and its vectorised coder is the reference's ANS.encode / ANS.decode
+(cifar_compress.py:48-67) for N streams at once, checked here against the literal port (AnsPort) and the C oracle (AnsC)."""
 import numpy as np
 import pytest
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from oracle import oracle as O                                                      # noqa: E402
-
-BITS = 31
-U64 = np.uint64
-TWO32 = 1 << 32
-POP_KINDS = ("lower", "upper", "renorm 2^32-1", "renorm 2^32", "random")
-PUSH_KINDS = ("lim-1", "lim", "kmax*p-1", "kmax*p", "kmin*p-1", "kmin*p", "kmid*p", "random")
-
-
-# ---- the vectorised coder ---------------------------------------------------------------------------------------------------
-class RowTables:
-    """Integer tables of R rows, P [R, S] and C [R, S + 1] (int64, as O.tables_np returns them), and the key searchsorted runs
-    on: row r's C[r, :-1] offset by r * 2^32, so one call searches every stream in its own row."""
-
-    def __init__(self, P, C):
-        self.P, self.C = np.ascontiguousarray(P, dtype=np.int64), np.ascontiguousarray(C, dtype=np.int64)
-        self.R, self.S = self.P.shape
-        self.key = ((np.arange(self.R, dtype=np.int64)[:, None] << 32) + self.C[:, :-1]).ravel()
-
-    def search(self, rows, mm, side="right"):
-        """searchsorted(C[rows[j], :-1], mm[j], side) - 1 for every stream j (the reference's ANS.decode with 'right')."""
-        q = (rows << 32) + mm.astype(np.int64)
-        return np.searchsorted(self.key, q, side) - 1 - rows * self.S
-
-
-class Stacks:
-    """N reference states: words [N, cap] uint32 bottom-first with n [N] of them in use, and the heads x [N] uint64."""
-
-    def __init__(self, words, n, x):
-        self.w, self.n, self.x = words, np.asarray(n, dtype=np.int64).copy(), np.asarray(x, dtype=U64).copy()
-
-    @classmethod
-    def from_packed(cls, words, offsets, heads, cap):
-        offsets = np.asarray(offsets, dtype=np.int64)
-        n = np.diff(offsets)
-        w = np.zeros((len(n), cap), dtype=np.uint32)
-        w[np.arange(cap)[None, :] < n[:, None]] = words
-        return cls(w, n, heads)
-
-    @classmethod
-    def from_lists(cls, states, cap):
-        n = np.array([len(s) - 1 for s in states], dtype=np.int64)
-        w = np.zeros((len(states), cap), dtype=np.uint32)
-        for j, s in enumerate(states):
-            w[j, :n[j]] = np.array(s[:-1], dtype=np.uint64).astype(np.uint32)
-        return cls(w, n, np.array([s[-1] for s in states], dtype=U64))
-
-    def packed(self):
-        """(words uint32 [sum n], offsets int64 [N + 1], heads uint64 [N]), the layout of StreamSet.export."""
-        offs = np.zeros(self.n.size + 1, dtype=np.int64)
-        np.cumsum(self.n, out=offs[1:])
-        return self.w[np.arange(self.w.shape[1])[None, :] < self.n[:, None]], offs, self.x.copy()
-
-    def to_lists(self):
-        return [[int(v) for v in self.w[j, :self.n[j]]] + [int(self.x[j])] for j in range(self.n.size)]
-
-
-def _rows_for(rows, N):
-    rows = np.asarray(rows, dtype=np.int64)
-    return np.broadcast_to(rows, (N, rows.shape[-1]))
-
-
-def pop(tab, rows, st, side="right", bits=BITS):
-    """ANS.decode of len(rows) rows for every stream in `st` (in place), rows descending; rows [L] (shared) or [N, L].
-    Returns the symbols [N, L].  side='left' is a deliberately wrong search the harness must catch."""
-    N = st.x.size
-    rows = _rows_for(rows, N)
-    sym = np.empty(rows.shape, dtype=np.int64)
-    mask = U64((1 << bits) - 1)
-    for i in range(rows.shape[1] - 1, -1, -1):
-        r = rows[:, i]
-        mm = st.x & mask                                                            # :60
-        s = tab.search(r, mm, side)                                                 # :61
-        p, c = tab.P[r, s].astype(U64), tab.C[r, s].astype(U64)
-        x = p * (st.x >> U64(bits)) + mm - c                                        # :63
-        need = np.flatnonzero(x < U64(TWO32))                                       # :64
-        if (st.n[need] <= 0).any():
-            raise IndexError("pop from empty ANS stack")
-        st.n[need] -= 1
-        x[need] = (x[need] << U64(32)) | st.w[need, st.n[need]].astype(U64)         # :65
-        st.x = x
-        sym[:, i] = s
-    return sym
-
-
-def push(tab, rows, st, sym, bits=BITS):
-    """ANS.encode of len(rows) rows for every stream in `st` (in place), rows ascending; sym [N, L]."""
-    N = st.x.size
-    rows = _rows_for(rows, N)
-    sym = np.asarray(sym, dtype=np.int64)
-    for i in range(rows.shape[1]):
-        r, s = rows[:, i], sym[:, i]
-        p, c = tab.P[r, s].astype(U64), tab.C[r, s].astype(U64)
-        lim = U64(((TWO32 >> bits) << 32)) * p                                      # :51
-        big = np.flatnonzero(st.x >= lim)
-        if (st.n[big] >= st.w.shape[1]).any():
-            raise OverflowError("stack capacity")
-        st.w[big, st.n[big]] = (st.x[big] & U64(0xffffffff)).astype(np.uint32)     # :52-53
-        st.n[big] += 1
-        st.x[big] >>= U64(32)
-        st.x = ((st.x // p) << U64(bits)) + st.x % p + c                           # :54
-    return st
-
-
-def assert_same(label, got_sym, got_packed, want_sym, want, top=None):
-    """Popped symbols (optional), then heads, word counts and word stacks, all as packed numpy arrays.  top: index of the
-    view's top row, whose symbol is checked (and reported) first."""
-    words, offs, heads = got_packed[:3]
-    w_words, w_offs, w_heads = want.packed()
-    if want_sym is not None:
-        got_sym = np.asarray(got_sym).astype(np.int64)
-        if top is not None:
-            bad = np.flatnonzero(got_sym[:, top] != want_sym[:, top])
-            assert bad.size == 0, f"{label}: top-row symbol of {bad.size} streams, first {bad[:6].tolist()}: " \
-                                  f"got {got_sym[bad[:6], top].tolist()}, want {want_sym[bad[:6], top].tolist()}"
-        bad = np.flatnonzero((got_sym != want_sym).any(axis=1))
-        assert bad.size == 0, f"{label}: symbols of {bad.size} streams differ, first {bad[:6].tolist()}"
-    bad = np.flatnonzero(np.asarray(heads, dtype=U64) != w_heads)
-    assert bad.size == 0, f"{label}: heads of {bad.size} streams differ, first {bad[:6].tolist()}"
-    bad = np.flatnonzero(np.diff(offs) != np.diff(w_offs))
-    assert bad.size == 0, f"{label}: word counts of {bad.size} streams differ, first {bad[:6].tolist()}"
-    assert np.array_equal(np.asarray(words, dtype=np.uint32), w_words), f"{label}: word stacks differ"
-
-
-# ---- the head builder -------------------------------------------------------------------------------------------------------
-def pop_heads(p, c, kind, rs, bits=BITS):
-    """Heads x in [2^32, 2^64) for a pop of bins with integer pmf p and cdf c (int64 arrays, one entry per head): mm = x & mask
-    on the bin's lower edge C[s] or upper edge C[s + 1] - 1, or such that the decoded value p (x >> 31) + mm - c is exactly
-    2^32 - 1 (a word is read) or 2^32 (none is), or mm anywhere in the bin under a random upper part.  Returns (x uint64, ok):
-    ok is False where no mm inside the bin gives the kind (the renormalisation targets need x >> 31 >= 2)."""
-    p, c = np.asarray(p, dtype=np.int64), np.asarray(c, dtype=np.int64)
-    n = p.size
-    hi = rs.randint(2, 1 << (64 - bits), n, dtype=np.int64)
-    ok = np.ones(n, dtype=bool)
-    if kind == "lower":
-        mm = c
-    elif kind == "upper":
-        mm = c + p - 1
-    elif kind in ("renorm 2^32-1", "renorm 2^32"):
-        T = TWO32 - (1 if kind == "renorm 2^32-1" else 0)
-        hi, d = T // p, T % p
-        ok = hi >= 2
-        hi = np.where(ok, hi, 2)
-        mm = c + np.where(ok, d, 0)
-    elif kind == "random":
-        hi = rs.randint(1 << (63 - bits), 1 << (64 - bits), n, dtype=np.int64)
-        mm = c + (rs.random_sample(n) * p).astype(np.int64)
-    else:
-        raise ValueError(kind)
-    return (hi.astype(U64) << U64(bits)) | mm.astype(U64), ok
-
-
-def push_heads(p, kind, rs, bits=BITS):
-    """Heads x in [2^32, 2^64) for a push of bins with integer pmf p: x = lim - 1 and lim with lim = 2^33 p (the
-    renormalisation threshold), x = k p - 1 and k p for the largest k with k p < lim, the smallest with k p - 1 >= 2^32 and one
-    in between (the quotient steps of the division the kernels replace with a reciprocal), or any x.  Returns (x, ok)."""
-    p = np.asarray(p, dtype=np.int64)
-    n = p.size
-    lim = p.astype(object) * ((TWO32 >> bits) << 32)
-    kmax = (lim - 1) // p.astype(object)
-    kmin = (TWO32 + 1 + p.astype(object) - 1) // p.astype(object)
-    if kind in ("lim-1", "lim"):
-        x = lim - (1 if kind == "lim-1" else 0)
-    elif kind.startswith("k"):
-        k = {"kmax": kmax, "kmin": kmin}.get(kind[:4])
-        if k is None:
-            k = kmin + (np.array([int(v) for v in (kmax - kmin)], dtype=object) * rs.random_sample(n)).astype(np.int64)
-        x = k * p.astype(object) - (1 if kind.endswith("-1") else 0)
-    elif kind == "random":
-        x = np.array([int(v) for v in rs.randint(1, 1 << 32, n, dtype=np.int64)], dtype=object) << 32
-        x = x | np.array([int(v) for v in rs.randint(0, 1 << 32, n, dtype=np.int64)], dtype=object)
-    else:
-        raise ValueError(kind)
-    x = np.array([int(v) for v in x], dtype=object)
-    ok = (x >= TWO32) & (x < (1 << 64))
-    return np.array([int(v) if o else TWO32 for v, o in zip(x, ok)], dtype=U64), ok.astype(bool)
-
-
-def check_pop_heads(x, rows_tab, r, s, kind, bits=BITS):
-    """Each head lands where it claims: its bin is s, and the kind's edge or decoded value holds."""
-    tab = rows_tab
-    mm = (x & U64((1 << bits) - 1)).astype(np.int64)
-    assert (x >= U64(TWO32)).all()
-    assert np.array_equal(tab.search(r, mm), s), kind
-    if kind == "lower":
-        assert np.array_equal(mm, tab.C[r, s])
-    elif kind == "upper":
-        assert np.array_equal(mm, tab.C[r, s + 1] - 1)
-    elif kind.startswith("renorm"):
-        y = tab.P[r, s].astype(U64) * (x >> U64(bits)) + mm.astype(U64) - tab.C[r, s].astype(U64)
-        assert (y == U64(TWO32 - (1 if kind == "renorm 2^32-1" else 0))).all(), kind
-
-
-def check_push_heads(x, p, kind, bits=BITS):
-    lim = [int(v) * ((TWO32 >> bits) << 32) for v in p]
-    xs = [int(v) for v in x]
-    assert all(TWO32 <= v < (1 << 64) for v in xs)
-    if kind == "lim-1":
-        assert all(v == m - 1 for v, m in zip(xs, lim))
-    elif kind == "lim":
-        assert all(v == m for v, m in zip(xs, lim))
-    elif kind.startswith("k"):
-        d = 1 if kind.endswith("-1") else 0
-        assert all((v + d) % int(q) == 0 and v + d < m for v, q, m in zip(xs, p, lim)), kind
-        if kind.startswith("kmax"):
-            assert all(v + d + int(q) >= m for v, q, m in zip(xs, p, lim))
-        if kind.startswith("kmin"):
-            assert all(v + d - int(q) - 1 < TWO32 for v, q in zip(xs, p))
+from coder_harness import (BITS, POP_KINDS, PUSH_KINDS, U64, RowTables, Stacks, assert_same, check_pop_heads,
+                           check_push_heads, pop, pop_heads, push, push_heads)
+from oracle import oracle as O
 
 
 # ---- tables with the shapes where searches go wrong -------------------------------------------------------------------------

@@ -4,14 +4,14 @@ integer tables.
 A pop is asked, with a chosen head, which bin holds mm at the one value where the answer changes: for a target row t the
 kernels get a view of L' rows ending at t (mu, sigma and endpoints offset by whole rows, stream strides 0, so every stream
 reads the same rows), and stream j's head sits on one edge of bin s_j of row t, or makes the decoded value 2^32 - 1 or 2^32
-(test_bin_edges_cpu.pop_heads).  The view's top row i = L' - 1 is popped first; the rows below pop random words.  L' cycles
+(coder_harness.pop_heads).  The view's top row i = L' - 1 is popped first; the rows below pop random words.  L' cycles
 over 1, 2, 31, 32, 33, 64 and 65, so the target row sits on lane i & 31 = 0, 1, 30 or 31 of the first 32-row block the kernels
 load, alone in its block or with whole blocks below it that are adopted through the one-block-ahead preload (only the random
 heads of the rows below meet that path).  A push codes every (row, symbol) pair once (stream j pushes (j + 7 r) mod S at
 row r) from heads on the push threshold 2^33 P[s] and on the quotient steps of the division the kernels replace with a
 reciprocal.
 
-Everything is compared with the vectorised reference coder of test_bin_edges_cpu.py on tables built from the reference's
+Everything is compared with the vectorised reference coder of coder_harness.py on tables built from the reference's
 own expression evaluated on this GPU (torch.sigmoid, float64) and ANS.__init__: popped symbols (the top row's first), heads,
 word counts and word stacks."""
 import os
@@ -26,16 +26,12 @@ import torch
 pytestmark = pytest.mark.gpu
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from coder_harness import (POP_KINDS, PUSH_KINDS, RowTables, Stacks, assert_same, check_pop_heads,   # noqa: E402
+                           check_push_heads, coder_paths, dev, family_case, linspace_rows, pad_big, pop, pop_heads,
+                           push, push_heads, ref_pmfs_cuda)
 from oracle import oracle as O                                                                  # noqa: E402
 from bitswap_b200.streams import StreamSet                                                      # noqa: E402
 from bitswap_b200._lib import lib, check, cuda_stream_ptr                                       # noqa: E402
-from test_bin_edges_cpu import (RowTables, Stacks, pop, push, assert_same, pop_heads, push_heads,  # noqa: E402
-                                check_pop_heads, check_push_heads, POP_KINDS, PUSH_KINDS)
-from test_grids_gpu import _family_case, _linspace_rows                                         # noqa: E402
-from test_quantbits_gpu import _pad_big                                                         # noqa: E402
-from test_ans_gpu import _ref_pmfs_cuda                                                         # noqa: E402
-
-dev = "cuda"
 VIEWS = (1, 2, 31, 32, 33, 64, 65)
 # two-phase paths: (rows mode, k_rows6 lanes per row); mode -1 classifies the rows (k_rows6 / k_pop6 when every row is a
 # uniform grid), 1 forces the affine kernels (non-uniform rows take the exact path for every bin), 0 is k_rows /
@@ -51,29 +47,18 @@ class Level:
     def __init__(self, ends, mu, sc, S, q, shared_row=False):
         self.S, self.q, self.R = S, q, mu.size
         self.ers = 0 if shared_row else S
-        self.e_pad = torch.from_numpy(_pad_big(ends)).to(dev)
+        self.e_pad = torch.from_numpy(pad_big(ends)).to(dev)
         self.mu = torch.from_numpy(np.ascontiguousarray(mu, dtype=np.float32)).to(dev)
         self.sc = torch.from_numpy(np.ascontiguousarray(sc, dtype=np.float32)).to(dev)
         e = torch.from_numpy(np.ascontiguousarray(ends, dtype=np.float64)).to(dev)
         if shared_row:
             e = e.expand(self.R, -1)
-        pm = torch.cat([_ref_pmfs_cuda(e[r:r + 256], self.mu[r:r + 256].double(), self.sc[r:r + 256].double()).cpu()
+        pm = torch.cat([ref_pmfs_cuda(e[r:r + 256], self.mu[r:r + 256].double(), self.sc[r:r + 256].double()).cpu()
                         for r in range(0, self.R, 256)]).numpy()
         P, C = O.tables_np(pm, 31, q)
         self.tab = RowTables(P, C)
         self.P32 = torch.from_numpy(P.astype(np.uint32).view(np.int32)).to(dev)
         self.C32 = torch.from_numpy(C.astype(np.uint32).view(np.int32)).to(dev)
-
-
-def _set_path(fam):
-    mode, lpr = TWO_PHASE[fam]
-    check(lib().bsw_set_rows_mode(mode))
-    check(lib().bsw_rows6_set_lanes_per_row(lpr))
-
-
-def _reset_path():
-    check(lib().bsw_set_rows_mode(-1))
-    check(lib().bsw_rows6_set_lanes_per_row(0))
 
 
 def _code(fam, push_, lv, ss, N, r0, L, sym=None, mu=None, sc=None):
@@ -101,11 +86,9 @@ def _code(fam, push_, lv, ss, N, r0, L, sym=None, mu=None, sc=None):
     else:
         nbytes = int(lib().bsw_logistic_scratch_bytes(N, L, S, 0))
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        _set_path(fam)
-        try:
+        mode, lpr = TWO_PHASE[fam]
+        with coder_paths(rows_mode=mode, lanes_per_row=lpr):
             check((lib().bsw_logistic_push_2p if push_ else lib().bsw_logistic_pop_2p)(*args, scratch.data_ptr(), nbytes, st))
-        finally:
-            _reset_path()
     return None if push_ else s16.cpu().numpy()
 
 
@@ -190,7 +173,7 @@ def _special_level(S, R, seed, dyadic=True):
     kind = np.arange(R) % (len(SPECIAL) + 3)
     ex = (kind == 4) | (kind == 5)
     lo[ex], hi[ex] = -8.0, 8.0
-    ends = _linspace_rows(lo, hi, S)
+    ends = linspace_rows(lo, hi, S)
     mu = rs.normal(0, 1.5, R)
     sc = rs.uniform(0.1, 1.0, R)
     sc[kind == 0] = 1e-4
@@ -272,7 +255,7 @@ def test_pop_edges_on_hostile_grid_families(family, S):
     q = S.bit_length() - 1
     t0 = time.time()
     R = 130
-    ends, mu, sc = _family_case(family, R, S, 1, seed=4000 + 10 * family + S)
+    ends, mu, sc = family_case(family, R, S, 1, seed=4000 + 10 * family + S)
     lv = Level(ends, mu[0], sc[0], S, q)
     counts = Counter()
     fams = ("affine", "classified", "generic")

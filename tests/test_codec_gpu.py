@@ -1,5 +1,4 @@
 """GPU parity of the nets (P3) and of the device-resident recursion (P4), through the C ABI."""
-import json
 import os
 
 import numpy as np
@@ -8,24 +7,16 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
+from coder_harness import initial_states                           # noqa: E402
+from codec_harness import GOLDEN, TOL, bitswap_golden, gpu_oracle, model, setup, tc_case   # noqa: E402
+from conv_harness import outputs_in_conv_modes      # noqa: E402
 from oracle import oracle as O                      # noqa: E402  (checker only)
 from bitswap_b200 import synthetic                   # noqa: E402
-from bitswap_b200.config import preset               # noqa: E402
+from bitswap_b200.config import CodecConfig, preset  # noqa: E402
 from bitswap_b200.model import Model                 # noqa: E402
 from bitswap_b200.codec import BitSwapCodec, Bins, BITSWAP, BBANS   # noqa: E402
 from bitswap_b200.streams import StreamSet           # noqa: E402
 from bitswap_b200.rand import ImageBins              # noqa: E402
-from bitswap_b200._lib import lib, check           # noqa: E402
-
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-TOL = 1e-4          # north_star: per-latent mu/sigma within 1e-4 of the reference torch model
-
-
-def _model(cfg, max_batch, tc=False):
-    sd = synthetic.synthetic_state_dict(cfg, seed=50, varied=True)
-    m = Model.from_config(cfg, max_batch=max_batch, use_tensor_cores=tc).load_state_dict(sd)
-    m.compress()
-    return m, sd
 
 
 @pytest.mark.parametrize("name", ["tiny", "tiny3"])
@@ -33,7 +24,7 @@ def test_p3_nets_vs_reference_golden(name):
     """mu/scale of every infer(i)/generate(i) against outputs of the REFERENCE Model (golden file)."""
     cfg = preset(name)
     g = np.load(os.path.join(GOLDEN, f"model_{name}.npz"))
-    m, _ = _model(cfg, 4)
+    m, _ = model(cfg, 4)
     _, zcen = synthetic.synthetic_bins(cfg, seed=0)
     xcen = ImageBins(torch.float64, "cpu", cfg.xdim).centres()
     zr = torch.arange(cfg.zdim)
@@ -57,7 +48,7 @@ def test_p3_nets_vs_reference_golden(name):
 def test_p3_nets_vs_oracle_full_width(name, B):
     """Reference-sized nets (W=63 / W=252) against the torch float32 oracle, batched, batch-invariant."""
     cfg = preset(name)
-    m, sd = _model(cfg, B)
+    m, sd = model(cfg, B)
     orc = O.ModelOracle(cfg, sd)
     rs = np.random.RandomState(4)
     _, zcen = synthetic.synthetic_bins(cfg, seed=0)
@@ -80,16 +71,6 @@ def test_p3_nets_vs_oracle_full_width(name, B):
     assert worst < TOL, worst
 
 
-def _setup(name, B, cap, tc=False):
-    cfg = preset(name)
-    m, sd = _model(cfg, B, tc)
-    zend, zcen = synthetic.synthetic_bins(cfg, seed=0)
-    bins = Bins(cfg, zend, zcen)
-    codec = BitSwapCodec(cfg, m, bins, B)
-    ss = StreamSet(B, cap)
-    return cfg, m, sd, zend, zcen, codec, ss
-
-
 @pytest.mark.parametrize("name", ["tiny", "tiny3"])
 def test_p4_bitswap_vs_reference_trace(name):
     """Own nets + own tables on the inputs of the reference-classes golden run.  Bits-back pops SAMPLE the
@@ -98,9 +79,10 @@ def test_p4_bitswap_vs_reference_trace(name):
     made with injected nets in test_p4_vs_oracle_with_injected_nets).  What must hold: the code length agrees
     statistically (bits/dim), identical streams stay identical, and decoding restores pixels and the initial
     state exactly."""
-    g = json.load(open(os.path.join(GOLDEN, f"bitswap_{name}.json")))
+    g = bitswap_golden(name)
     B = 3
-    cfg, m, sd, zend, zcen, codec, ss = _setup(name, B, 8192)
+    cfg, m, sd, zend, zcen, bins, codec = setup(name, B)
+    ss = StreamSet(B, 8192)
     imgs = synthetic.synthetic_images(cfg, g["nimg"], seed=7)
     w, head = synthetic.initial_words(g["nwords"], seed=100)
     ss.fill(w, head)
@@ -126,12 +108,10 @@ def test_p4_vs_oracle_with_injected_nets(name, scheme):
     """Oracle recursion driven with OUR mu/sigma and the reference's float64 table expression evaluated by torch on the
     GPU (where the reference evaluates it): EVERY stream's state list is bit-identical, for distinct images/streams."""
     B, nimg = 4, 2
-    cfg, m, sd, zend, zcen, codec, ss = _setup(name, B, 1 << 14)
+    cfg, m, sd, zend, zcen, bins, codec = setup(name, B)
+    ss = StreamSet(B, 1 << 14)
     imgs = synthetic.synthetic_images(cfg, B * nimg, seed=11).reshape(nimg, B, *cfg.xs)
-    states = []
-    for b in range(B):
-        w, head = synthetic.initial_words(3000 + 11 * b, seed=100 + b)
-        states.append([int(v) for v in w] + [head])
+    states = initial_states(B, seed=100, n=3000, step=11)
     ss.import_lists(states)
     for xi in range(nimg):
         codec.encode(ss, torch.from_numpy(imgs[xi]).cuda(), scheme=scheme)
@@ -139,16 +119,7 @@ def test_p4_vs_oracle_with_injected_nets(name, scheme):
     got = ss.export_lists()
     n_ident = 0
     for b in range(B):
-        def hook(kind, level, mu, sc):
-            f = m.infer(level) if kind == "infer" else m.generate(level)
-            return tuple(t.cpu() for t in f(hook.given.cuda()))
-        orc = O.BitSwapOracle(cfg, O.ModelOracle(cfg, sd), zend, zcen, coder="c", pmf="cuda")
-        # inject our nets: wrap _net so the GPU model sees the same `given`
-        def _net(kind, level, given, _m=m):
-            f = _m.infer(level) if kind == "infer" else _m.generate(level)
-            mu, sc = f(given.cuda())
-            return mu.cpu(), sc.cpu()
-        orc._net = _net
+        orc = gpu_oracle(cfg, m, sd, zend, zcen, cls=O.BitSwapOracle)
         st = O.CState.from_list(states[b])
         for xi in range(nimg):
             st = (orc.encode_image if scheme == BITSWAP else orc.encode_image_bbans)(st, imgs[xi, b])
@@ -167,7 +138,8 @@ def test_p4_vs_oracle_with_injected_nets(name, scheme):
 def test_p4_roundtrip_sub_range_and_chain_independence():
     """Coding streams [2,6) leaves the others untouched; a stream's result does not depend on its neighbours."""
     B = 8
-    cfg, m, sd, zend, zcen, codec, ss = _setup("tiny", B, 8192)
+    cfg, m, sd, zend, zcen, bins, codec = setup("tiny", B)
+    ss = StreamSet(B, 8192)
     w, head = synthetic.initial_words(1200, seed=100)
     ss.fill(w, head)
     init = ss.export_lists()
@@ -186,40 +158,13 @@ def test_p4_roundtrip_sub_range_and_chain_independence():
 # ---------------------------------------------------------------------------------------------------
 # tensor-core path (conv_tc.cu): bf16 hi/lo split, three wgmma per k-step, float32 register accumulation
 # ---------------------------------------------------------------------------------------------------
-from bitswap_b200.config import CodecConfig          # noqa: E402
-
-
-def _tc_case(cfg, B, seed=4, dtype=torch.float32):
-    sd = synthetic.synthetic_state_dict(cfg, seed=50, varied=True)
-    m_tc = Model.from_config(cfg, max_batch=B, use_tensor_cores=True).load_state_dict(sd)
-    m_si = Model.from_config(cfg, max_batch=B, use_tensor_cores=False).load_state_dict(sd)
-    m_tc.compress(); m_si.compress()
-    orc = O.ModelOracle(cfg, sd, dtype=dtype)
-    rs = np.random.RandomState(seed)
-    worst_o = worst_s = 0.0
-    for i in range(cfg.nz):
-        gx = torch.from_numpy((rs.randint(0, 256, (B, cfg.xdim)) - 127.5) / 127.5) if i == 0 else \
-            torch.from_numpy(rs.uniform(-5, 5, (B, cfg.zdim)))
-        gz = torch.from_numpy(rs.uniform(-5, 5, (B, cfg.zdim)))
-        for kind, g in (("infer", gx), ("generate", gz)):
-            f = lambda mm: (mm.infer(i) if kind == "infer" else mm.generate(i))     # noqa: E731
-            mu, sc = f(m_tc)(g.cuda())
-            mu_s, sc_s = f(m_si)(g.cuda())
-            mu_o, sc_o = f(orc)(g)
-            worst_o = max(worst_o, (mu.cpu() - mu_o).abs().max().item(), (sc.cpu() - sc_o).abs().max().item())
-            worst_s = max(worst_s, (mu - mu_s).abs().max().item(), (sc - sc_s).abs().max().item())
-            mu1, sc1 = f(m_tc)(g[B - 1:].cuda())           # batch invariance: last row alone, bit-identical
-            assert torch.equal(mu1[0], mu[B - 1]) and torch.equal(sc1[0], sc[B - 1])
-    return worst_o, worst_s
-
-
 @pytest.mark.parametrize("label,cfg", [
     ("one 3x3 layer", CodecConfig(xs=(3, 32, 32), nz=1, zchannels=8, nprocessing=0, resdepth=1, reswidth=252)),
     ("one 5x5 layer", CodecConfig(xs=(3, 32, 32), nz=1, zchannels=8, nprocessing=1, resdepth=0, reswidth=252)),
     ("width 256 crop", CodecConfig(xs=(3, 32, 32), nz=2, zchannels=8, nprocessing=1, resdepth=2, reswidth=256, cond_xscale=True)),
 ])
 def test_p3_tc_single_layers(label, cfg):
-    worst_o, worst_s = _tc_case(cfg, 3)
+    worst_o, worst_s = tc_case(cfg, 3)
     print(f"tensor cores {label}: max |err| vs torch-f32 oracle {worst_o:.2e}, vs SIMT f32 path {worst_s:.2e}")
     assert worst_o < TOL and worst_s < TOL
 
@@ -236,7 +181,7 @@ def test_p3_tc_single_layers(label, cfg):
 ])
 def test_p3_tc_dispatch_seams_vs_f64_oracle(label, cfg):
     """Whole nets at the dispatch seams of run_net on a tensor-core model, against the float64 oracle."""
-    worst_o, worst_s = _tc_case(cfg, 3, dtype=torch.float64)
+    worst_o, worst_s = tc_case(cfg, 3, dtype=torch.float64)
     print(f"tensor cores {label}: max |err| vs torch-f64 oracle {worst_o:.2e}, vs SIMT f32 path {worst_s:.2e}")
     assert worst_o < TOL and worst_s < TOL
 
@@ -247,28 +192,8 @@ def test_p3_tc_persistent_kernel_equals_per_tile_kernels():
     same epilogue arithmetic -> bit-identical mu and sigma.  B = 170 gives 680 half-image tiles per conv, i.e. up to
     six tiles per CTA on 132 SMs: accumulators and stages are reused across tiles; every conv shape on the path
     (in-convs with 1 and 25 taps, dense 3x3, 5x5, heads)."""
-    B = 170
     cfg = CodecConfig(xs=(3, 32, 32), nz=2, zchannels=8, nprocessing=1, resdepth=1, reswidth=252)
-    sd = synthetic.synthetic_state_dict(cfg, seed=61, varied=True)
-    m = Model.from_config(cfg, max_batch=B, use_tensor_cores=True).load_state_dict(sd)
-    m.compress()
-    rs = np.random.RandomState(4)
-    gx = torch.from_numpy((rs.randint(0, 256, (B, cfg.xdim)) - 127.5) / 127.5).cuda()
-    gz = torch.from_numpy(rs.uniform(-5, 5, (B, cfg.zdim))).cuda()
-    out = {}
-    try:
-        for mode in (0, 7):                                # per-tile grid | persistent grid
-            check(lib().bsw_set_conv_mode(mode))
-            res = []
-            for i in range(cfg.nz):
-                mu, sc = m.infer(i)(gx if i == 0 else gz)
-                res += [mu.clone(), sc.clone()]
-                mu, sc = m.generate(i)(gz)
-                res += [mu.clone(), sc.clone()]
-            torch.cuda.synchronize()
-            out[mode] = res
-    finally:
-        check(lib().bsw_set_conv_mode(-1))
+    out = outputs_in_conv_modes(cfg, 170, (0, 7))
     for a, b in zip(out[0], out[7]):
         assert torch.equal(a, b), "conv mode 7"
     assert all(torch.isfinite(t).all() for t in out[7])
@@ -276,7 +201,7 @@ def test_p3_tc_persistent_kernel_equals_per_tile_kernels():
 
 def test_p3_tc_cifar8_full():
     cfg = preset("cifar8")
-    worst_o, worst_s = _tc_case(cfg, 2)
+    worst_o, worst_s = tc_case(cfg, 2)
     print(f"tensor cores cifar8: max |err| vs torch-f32 oracle {worst_o:.2e}, vs SIMT f32 path {worst_s:.2e}")
     assert worst_o < TOL and worst_s < TOL
 
@@ -285,7 +210,8 @@ def test_p4_tc_roundtrip_cifar8():
     """Encoder and decoder regenerate bit-identical tables from the tensor-core nets: exact round trip, with a
     different batch split on the decode side (H3: results do not depend on batch size or position)."""
     B = 6
-    cfg, m, sd, zend, zcen, codec, ss = _setup("cifar8", B, 8192, tc=True)
+    cfg, m, sd, zend, zcen, bins, codec = setup("cifar8", B, tc=True)
+    ss = StreamSet(B, 8192)
     w, head = synthetic.initial_words(4096, seed=100)
     ss.fill(w, head)
     init = ss.export_lists()
@@ -306,12 +232,10 @@ def test_two_phase_coder_equals_fused_coder(name, scheme):
     """ans_rows.cu (parallel row tables + serial coder) and the fused one-warp-per-stream kernels must leave
     bit-identical streams and symbols."""
     B = 5
-    cfg, m, sd, zend, zcen, codec, ss = _setup(name, B, 1 << 14)
+    cfg, m, sd, zend, zcen, bins, codec = setup(name, B)
+    ss = StreamSet(B, 1 << 14)
     imgs = synthetic.synthetic_images(cfg, B, seed=31)
-    states = []
-    for b in range(B):
-        w, head = synthetic.initial_words(5000 + 3 * b, seed=200 + b)
-        states.append([int(v) for v in w] + [head])
+    states = initial_states(B, seed=200, n=5000, step=3)
     res = []
     for two_phase in (True, False):
         codec.set_two_phase(two_phase)
@@ -338,7 +262,7 @@ def test_config0_mnist_b1_state_identical_at_every_level():
     import ctypes
     from bitswap_b200._lib import lib, check, cuda_stream_ptr
     cfg = preset("mnist2")
-    m, sd = _model(cfg, 1)
+    m, sd = model(cfg, 1)
     zend, zcen = synthetic.synthetic_bins(cfg, seed=0)
     bins = Bins(cfg, zend, zcen)
     S, q = cfg.zsupport, cfg.quantbits
@@ -350,13 +274,8 @@ def test_config0_mnist_b1_state_identical_at_every_level():
 
     # oracle trace with the GPU nets injected
     trace = []
-    orc = O.BitSwapOracle(cfg, O.ModelOracle(cfg, sd), zend, zcen, coder="c", pmf="cuda", trace=trace)
-
-    def gpu_net(kind, level, given):
-        f = m.infer(level) if kind == "infer" else m.generate(level)
-        mu, sc = f(given.cuda())
-        return mu.cpu(), sc.cpu()
-    orc._net = gpu_net
+    orc = gpu_oracle(cfg, m, sd, zend, zcen, cls=O.BitSwapOracle)
+    orc.trace = trace
     imgs = np.zeros((2, 1, 32, 32), dtype=np.uint8)
     imgs[:, :, 2:30, 2:30] = synthetic.synthetic_images(cfg, 2, seed=13)[:, :, 2:30, 2:30]     # Pad(2), mnist_compress.py:129
     w, head = synthetic.initial_words(1500, seed=100)
@@ -416,13 +335,11 @@ def test_pipelined_codec_equals_single_codec():
     """PipelinedCodec (sub-batches on separate CUDA streams) leaves exactly the streams a single codec leaves."""
     from bitswap_b200.codec import PipelinedCodec
     B = 7
-    cfg, m, sd, zend, zcen, codec, ss = _setup("tiny3", B, 1 << 14)
+    cfg, m, sd, zend, zcen, bins, codec = setup("tiny3", B)
+    ss = StreamSet(B, 1 << 14)
     pc = PipelinedCodec(cfg, sd, Bins(cfg, zend, zcen), B, lanes=3, use_tensor_cores=False)
     imgs = synthetic.synthetic_images(cfg, 2 * B, seed=41).reshape(2, B, *cfg.xs)
-    states = []
-    for b in range(B):
-        w, head = synthetic.initial_words(4000 + b, seed=300 + b)
-        states.append([int(v) for v in w] + [head])
+    states = initial_states(B, seed=300, n=4000, step=1)
     res = []
     for c in (codec, pc):
         ss.import_lists(states)
@@ -453,10 +370,7 @@ def test_overlap_mode_equals_program_order(name, tc, scheme, lanes):
     pc = PipelinedCodec(cfg, sd, Bins(cfg, zend, zcen), B, lanes=lanes, use_tensor_cores=tc)
     ss = StreamSet(B, 1 << 15)
     imgs = synthetic.synthetic_images(cfg, 3 * B, seed=43).reshape(3, B, *cfg.xs)
-    states = []
-    for b in range(B):
-        w, head = synthetic.initial_words(5000 + b, seed=400 + b)
-        states.append([int(v) for v in w] + [head])
+    states = initial_states(B, seed=400, n=5000, step=1)
     res = []
     for mode in (0, 1):
         pc.set_dual_stream(mode)
@@ -483,16 +397,10 @@ def test_container_variable_size_images_vs_oracle_demo_procedure():
     sizes = [(64, 96), (32, 32), (100, 70), (40, 129)]
     rs = np.random.RandomState(5)
     images = [rs.randint(0, 256, (h, w, 3)).astype(np.uint8) for h, w in sizes]
-    cfg_, m, sd, zend, zcen, codec, _ = _setup("tiny3", len(images), 64)
+    _, m, sd, zend, zcen, _, codec = setup("tiny3", len(images))
     conts = compress_images(codec, images, excess_state_len=3000)
     # oracle: the reference demo loop, one image at a time
-    orc = O.BitSwapOracle(cfg, O.ModelOracle(cfg, sd), zend, zcen, coder="c", pmf="cuda")
-
-    def gpu_net(kind, level, given):
-        f = m.infer(level) if kind == "infer" else m.generate(level)
-        mu, sc = f(given.cuda())
-        return mu.cpu(), sc.cpu()
-    orc._net = gpu_net
+    orc = gpu_oracle(cfg, m, sd, zend, zcen, cls=O.BitSwapOracle)
     for img, cont in zip(images, conts):
         blocks, h, w = extract_blocks(img)
         wds, head = synthetic.initial_words(3000, seed=100)
@@ -619,7 +527,7 @@ def test_elbo_on_gpu_nets_matches_oracle_nets():
     from bitswap_b200.elbo import elbo
     cfg = preset("tiny3")
     B = 4
-    m, sd = _model(cfg, B)
+    m, sd = model(cfg, B)
     orc = O.ModelOracle(cfg, sd)
     x = torch.from_numpy(synthetic.synthetic_images(cfg, B, seed=19, kind="smooth"))
     gen = torch.Generator().manual_seed(7)
@@ -661,14 +569,7 @@ def test_p4_full_size_configs_vs_oracle_and_batch_roundtrip(name, B, lanes, nsam
     got = ss.export_lists()
     assert got[0] == got[1] and got[0] != got[2]
     sample = sorted(set(int(v) for v in np.linspace(0, B - 1, nsample).round()))
-    m = pc.models[0]
-    orc = O.BitSwapOracle(cfg, O.ModelOracle(cfg, sd), zend, zcen, coder="c", pmf="cuda")
-
-    def gpu_net(kind, level, given):
-        f = m.infer(level) if kind == "infer" else m.generate(level)
-        mu, sc = f(given.cuda())
-        return mu.cpu(), sc.cpu()
-    orc._net = gpu_net
+    orc = gpu_oracle(cfg, pc.models[0], sd, zend, zcen, cls=O.BitSwapOracle)
     for b in sample:
         want = orc.encode_image(O.CState(w, head), imgs[b]).to_list()
         assert got[b] == want, f"{name}: stream {b} differs from the oracle"

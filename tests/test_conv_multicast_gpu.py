@@ -7,10 +7,10 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
+from conv_harness import conv_mode, outputs_in_conv_modes   # noqa: E402
 from bitswap_b200 import synthetic                   # noqa: E402
 from bitswap_b200.config import CodecConfig          # noqa: E402
 from bitswap_b200.model import Model                 # noqa: E402
-from bitswap_b200._lib import lib, check             # noqa: E402
 
 NO_MULTICAST = 8
 
@@ -21,27 +21,7 @@ def test_multicast_clusters_equal_single_cta_convs(B):
     path: in-convs with 1 and 25 taps, dense 3x3, 5x5 and the heads.  B = 170 leaves some clusters of the persistent grid
     one image more than others; B = 1 is a single cluster."""
     cfg = CodecConfig(xs=(3, 32, 32), nz=2, zchannels=8, nprocessing=1, resdepth=1, reswidth=252)
-    sd = synthetic.synthetic_state_dict(cfg, seed=61, varied=True)
-    m = Model.from_config(cfg, max_batch=B, use_tensor_cores=True).load_state_dict(sd)
-    m.compress()
-    rs = np.random.RandomState(5)
-    gx = torch.from_numpy((rs.randint(0, 256, (B, cfg.xdim)) - 127.5) / 127.5).cuda()
-    gz = torch.from_numpy(rs.uniform(-5, 5, (B, cfg.zdim))).cuda()
-    out = {}
-    try:
-        for grid in (0, 7):
-            for mode in (grid, grid | NO_MULTICAST):
-                check(lib().bsw_set_conv_mode(mode))
-                res = []
-                for i in range(cfg.nz):
-                    mu, sc = m.infer(i)(gx if i == 0 else gz)
-                    res += [mu.clone(), sc.clone()]
-                    mu, sc = m.generate(i)(gz)
-                    res += [mu.clone(), sc.clone()]
-                torch.cuda.synchronize()
-                out[mode] = res
-    finally:
-        check(lib().bsw_set_conv_mode(-1))
+    out = outputs_in_conv_modes(cfg, B, (0, NO_MULTICAST, 7, 7 | NO_MULTICAST), seed=5)
     for grid in (0, 7):
         for a, b in zip(out[grid], out[grid | NO_MULTICAST]):
             assert torch.equal(a, b), f"conv mode {grid} with and without multicast"
@@ -62,15 +42,12 @@ def test_default_multicast_grid_vs_float64_oracle():
     gx = torch.from_numpy((rs.randint(0, 256, (B, cfg.xdim)) - 127.5) / 127.5).cuda()
     gz = torch.from_numpy(rs.uniform(-5, 5, (B, cfg.zdim))).cuda()
     worst = 0.0
-    try:
-        check(lib().bsw_set_conv_mode(7))
+    with conv_mode(7):
         for i in range(cfg.nz):
             for kind, g in (("infer", gx if i == 0 else gz), ("generate", gz)):
                 mu, sc = (m.infer(i) if kind == "infer" else m.generate(i))(g)
                 mu_o, sc_o = (orc.infer(i) if kind == "infer" else orc.generate(i))(g)
                 worst = max(worst, (mu - mu_o).abs().max().item(), (sc - sc_o).abs().max().item())
-    finally:
-        check(lib().bsw_set_conv_mode(-1))
     print(f"mode 7, B = {B}: max |err| vs torch-f64 oracle {worst:.2e}")
     assert worst < 1e-4, worst
 

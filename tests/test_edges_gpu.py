@@ -11,49 +11,20 @@ pytestmark = pytest.mark.gpu
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from edge_oracle import EdgeOracle, pad_block                        # noqa: E402
+from coder_harness import coder_paths, initial_states                 # noqa: E402
+from codec_harness import demo_oracle_container, gpu_oracle, setup     # noqa: E402
+from edge_oracle import pad_block                                      # noqa: E402
 from oracle import oracle as O                                         # noqa: E402
 from bitswap_b200 import synthetic                                     # noqa: E402
 from bitswap_b200.config import preset                                 # noqa: E402
-from bitswap_b200.model import Model                                   # noqa: E402
-from bitswap_b200.codec import BitSwapCodec, Bins, PipelinedCodec, BITSWAP, BBANS   # noqa: E402
+from bitswap_b200.codec import Bins, PipelinedCodec, BITSWAP, BBANS    # noqa: E402
 from bitswap_b200.streams import StreamSet                             # noqa: E402
-from bitswap_b200._lib import lib, check                               # noqa: E402
 
 MIXED = [(1, 1), (1, 32), (32, 1), (17, 29), (32, 32), (5, 7)]
 
 
-def _setup(name, B, tc=False):
-    cfg = preset(name)
-    sd = synthetic.synthetic_state_dict(cfg, seed=50, varied=True)
-    m = Model.from_config(cfg, max_batch=B, use_tensor_cores=tc).load_state_dict(sd)
-    m.compress()
-    zend, zcen = synthetic.synthetic_bins(cfg, seed=0)
-    bins = Bins(cfg, zend, zcen)
-    return cfg, m, sd, zend, zcen, bins, BitSwapCodec(cfg, m, bins, B)
-
-
-def _states(B, seed, n=3000):
-    out = []
-    for b in range(B):
-        w, head = synthetic.initial_words(n + 7 * b, seed=seed + b)
-        out.append([int(v) for v in w] + [head])
-    return out
-
-
 def _ext(extents):
     return torch.tensor(extents, dtype=torch.int16, device="cuda")
-
-
-def _gpu_oracle(cfg, m, sd, zend, zcen):
-    orc = EdgeOracle(cfg, O.ModelOracle(cfg, sd), zend, zcen, coder="c", pmf="cuda")
-
-    def gpu_net(kind, level, given):
-        f = m.infer(level) if kind == "infer" else m.generate(level)
-        mu, sc = f(given.cuda())
-        return mu.cpu(), sc.cpu()
-    orc._net = gpu_net
-    return orc
 
 
 def _code(codec, ss, states, imgs, exts, scheme):
@@ -78,11 +49,11 @@ def test_ext_vs_oracle_with_injected_nets(name, scheme):
     """Mixed extents in one batch, on a sub-range of the stream set: every stream's state list equals the oracle's after
     encode; decode restores the valid pixels (edge-padded) and the initial states; the streams outside the range stay put."""
     B, first = len(MIXED), 2
-    cfg, m, sd, zend, zcen, bins, codec = _setup(name, B)
+    cfg, m, sd, zend, zcen, bins, codec = setup(name, B)
     imgs = synthetic.synthetic_images(cfg, 2 * B, seed=11).reshape(2, B, *cfg.xs)
     exts = [MIXED, MIXED[::-1]]
     ss = StreamSet(B + first + 1, 1 << 14)
-    states = _states(B + first + 1, 500)
+    states = initial_states(B + first + 1, 500)
     ss.import_lists(states)
     for x, e in zip(imgs, exts):
         codec.encode(ss, torch.from_numpy(x).cuda(), first=first, scheme=scheme, extent=_ext(e))
@@ -90,7 +61,7 @@ def test_ext_vs_oracle_with_injected_nets(name, scheme):
     ss.raise_on_error()
     got = ss.export_lists()
     assert got[:first] == states[:first] and got[first + B:] == states[first + B:]
-    orc = _gpu_oracle(cfg, m, sd, zend, zcen)
+    orc = gpu_oracle(cfg, m, sd, zend, zcen)
     enc = orc.encode_image if scheme == BITSWAP else orc.encode_image_bbans
     for b in range(B):
         st = O.CState.from_list(states[first + b])
@@ -108,10 +79,10 @@ def test_ext_vs_oracle_with_injected_nets(name, scheme):
 @pytest.mark.parametrize("scheme", [BITSWAP, BBANS])
 def test_full_extents_equal_the_plain_calls(scheme):
     B = 5
-    cfg, m, sd, zend, zcen, bins, codec = _setup("tiny3", B)
+    cfg, m, sd, zend, zcen, bins, codec = setup("tiny3", B)
     imgs = list(synthetic.synthetic_images(cfg, 2 * B, seed=13).reshape(2, B, *cfg.xs))
     ss = StreamSet(B, 1 << 14)
-    states = _states(B, 600)
+    states = initial_states(B, 600)
     a = _code(codec, ss, states, imgs, [None, None], scheme)
     b = _code(codec, ss, states, imgs, [[(32, 32)] * B] * 2, scheme)
     assert a[0] == b[0]
@@ -124,26 +95,22 @@ def test_masked_calls_agree_across_coder_variants(scheme):
     """Two-phase on/off, generic (rows mode 0) and affine (rows mode 1) pixel kernels, overlap mode on/off and a
     PipelinedCodec with 1 and 3 lanes leave identical streams and decode identical blocks."""
     B = len(MIXED)
-    cfg, m, sd, zend, zcen, bins, codec = _setup("tiny3", B)
+    cfg, m, sd, zend, zcen, bins, codec = setup("tiny3", B)
     imgs = list(synthetic.synthetic_images(cfg, 2 * B, seed=17).reshape(2, B, *cfg.xs))
     exts = [MIXED, MIXED[::-1]]
     ss = StreamSet(B, 1 << 14)
-    states = _states(B, 700)
+    states = initial_states(B, 700)
     want = _code(codec, ss, states, imgs, exts, scheme)
     variants = []
-    try:
-        codec.set_two_phase(False)
-        variants.append(("fused", _code(codec, ss, states, imgs, exts, scheme)))
-        codec.set_two_phase(True)
-        for mode in (0, 1):
-            check(lib().bsw_set_rows_mode(mode))
+    codec.set_two_phase(False)
+    variants.append(("fused", _code(codec, ss, states, imgs, exts, scheme)))
+    codec.set_two_phase(True)
+    for mode in (0, 1):
+        with coder_paths(rows_mode=mode):
             variants.append((f"rows mode {mode}", _code(codec, ss, states, imgs, exts, scheme)))
-        check(lib().bsw_set_rows_mode(-1))
-        codec.set_dual_stream(True)
-        variants.append(("overlap", _code(codec, ss, states, imgs, exts, scheme)))
-        codec.set_dual_stream(False)
-    finally:
-        check(lib().bsw_set_rows_mode(-1))
+    codec.set_dual_stream(True)
+    variants.append(("overlap", _code(codec, ss, states, imgs, exts, scheme)))
+    codec.set_dual_stream(False)
     for lanes in (1, 3):
         pc = PipelinedCodec(cfg, sd, bins, B, lanes=lanes, use_tensor_cores=False)
         variants.append((f"{lanes} lanes", _code(pc, ss, states, imgs, exts, scheme)))
@@ -154,7 +121,7 @@ def test_masked_calls_agree_across_coder_variants(scheme):
 
 def test_pad_area_does_not_change_the_bitstream():
     B = len(MIXED)
-    cfg, m, sd, zend, zcen, bins, codec = _setup("tiny3", B)
+    cfg, m, sd, zend, zcen, bins, codec = setup("tiny3", B)
     x = synthetic.synthetic_images(cfg, B, seed=19)
     y = x.copy()
     rs = np.random.RandomState(3)
@@ -164,7 +131,7 @@ def test_pad_area_does_not_change_the_bitstream():
         keep[:, :vh, :vw] = True
         y[b] = np.where(keep, y[b], noise)
     ss = StreamSet(B, 1 << 14)
-    states = _states(B, 800)
+    states = initial_states(B, 800)
     a = _code(codec, ss, states, [x], [MIXED], BITSWAP)
     b = _code(codec, ss, states, [y], [MIXED], BITSWAP)
     assert a[0] == b[0] and np.array_equal(a[1][0], b[1][0])
@@ -172,9 +139,9 @@ def test_pad_area_does_not_change_the_bitstream():
 
 def test_invalid_extent_flags_only_that_stream():
     B = 4
-    cfg, m, sd, zend, zcen, bins, codec = _setup("tiny3", B)
+    cfg, m, sd, zend, zcen, bins, codec = setup("tiny3", B)
     x = synthetic.synthetic_images(cfg, B, seed=23)
-    states = _states(B, 900)
+    states = initial_states(B, 900)
     ss = StreamSet(B, 1 << 14)
     ss.import_lists(states)
     codec.encode(ss, torch.from_numpy(x).cuda(), extent=_ext([(32, 32), (0, 5), (33, 1), (7, 7)]))
@@ -198,38 +165,21 @@ def test_invalid_extent_flags_only_that_stream():
     assert np.array_equal(out[3].reshape(-1), pad_block(x[3].reshape(-1), (7, 7)).astype(np.uint8))
 
 
-def _demo_oracle_container(orc, img, n_init):
-    """The reference demo procedure (demo_compress.py:113-162,268-284) run by the oracle on one image, with extents."""
-    from bitswap_b200.container import extract_edge_blocks
-    blocks, extents, h, w = extract_edge_blocks(img)
-    wds, head = synthetic.initial_words(n_init, seed=100)
-    st = O.CState(wds, head)
-    low = st.n
-    pops = []
-    orc.trace = pops
-    for b, e in zip(blocks, extents):
-        st = orc.encode_image(st, b.transpose(2, 0, 1), extent=(int(e[0]), int(e[1])))
-    orc.trace = None
-    low = min([ln - 1 for tag, ln, _ in pops if tag.startswith("pop")] + [low])
-    return np.concatenate([st.words[low:st.n], np.array([st.head & 0xffffffff, st.head >> 32, len(blocks), h, w],
-                                                         dtype=np.uint64)]).astype(np.uint32)
-
-
 def test_container_edges_code_vs_oracle_demo_procedure():
     from bitswap_b200.container import compress_images, decompress_images
     sizes = [(100, 70), (20, 20), (33, 1), (64, 96), (225, 224)]
     rs = np.random.RandomState(5)
     images = [rs.randint(0, 256, (h, w, 3)).astype(np.uint8) for h, w in sizes]
-    cfg, m, sd, zend, zcen, bins, codec = _setup("tiny3", len(images))
+    cfg, m, sd, zend, zcen, bins, codec = setup("tiny3", len(images))
     conts = compress_images(codec, images, excess_state_len=3000, edges="code")
     back = decompress_images(codec, conts)
     for img, rec in zip(images, back):
         assert rec.shape == img.shape and np.array_equal(rec, img)
     crop = compress_images(codec, [images[3]], excess_state_len=3000)
     assert np.array_equal(crop[0], conts[3])                  # whole blocks: byte-identical to the crop mode
-    orc = _gpu_oracle(cfg, m, sd, zend, zcen)
+    orc = gpu_oracle(cfg, m, sd, zend, zcen)
     for img, cont in zip(images, conts):
-        assert np.array_equal(cont, _demo_oracle_container(orc, img, 3000)), img.shape
+        assert np.array_equal(cont, demo_oracle_container(orc, img, 3000)), img.shape
     pc = PipelinedCodec(cfg, sd, bins, len(images), lanes=3, use_tensor_cores=False, free_running=True)
     conts_pc = compress_images(pc, images, excess_state_len=3000, edges="code")
     assert all(np.array_equal(a, b) for a, b in zip(conts, conts_pc))
@@ -252,5 +202,5 @@ def test_imagenetcrop4_tensor_cores_partial_blocks():
     conts = compress_images(pc, images, excess_state_len=4000, edges="code")
     back = decompress_images(pc, conts)
     assert all(np.array_equal(a, b) for a, b in zip(images, back))
-    orc = _gpu_oracle(cfg, pc.models[0], sd, zend, zcen)
-    assert np.array_equal(conts[2], _demo_oracle_container(orc, images[2], 4000))
+    orc = gpu_oracle(cfg, pc.models[0], sd, zend, zcen)
+    assert np.array_equal(conts[2], demo_oracle_container(orc, images[2], 4000))

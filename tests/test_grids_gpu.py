@@ -17,6 +17,9 @@ import torch
 pytestmark = pytest.mark.gpu
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from coder_harness import (check_vs_oracle, coder_paths, dev, draw, family_case, half, initial_states,   # noqa: E402
+                           linspace_rows, oracle_tables, push_pop, ref_pmfs_cuda, run_2p, run_fused)
+from codec_harness import gpu_oracle                                                # noqa: E402
 from oracle import oracle as O                                                      # noqa: E402
 from bitswap_b200 import synthetic                                                  # noqa: E402
 from bitswap_b200.config import CodecConfig, preset, with_                          # noqa: E402
@@ -24,83 +27,8 @@ from bitswap_b200.model import Model                                            
 from bitswap_b200.codec import BitSwapCodec, Bins, BITSWAP, BBANS                  # noqa: E402
 from bitswap_b200.streams import StreamSet                                          # noqa: E402
 from bitswap_b200._lib import lib, check, cuda_stream_ptr                           # noqa: E402
-from test_quantbits_gpu import _run_2p, _oracle_tables, _check_vs_oracle, _states, _oracle_with, _pad_big   # noqa: E402
-from test_ans_gpu import _ref_pmfs_cuda                                             # noqa: E402
 
-dev = "cuda"
 FAMILIES = {1: "off-centre", 2: "float16 extrema", 3: "far and narrow", 4: "tiny span", 5: "dt near 64", 6: "perturbed"}
-
-
-def _half(x):
-    """Nearest float16 value, saturating at +-65504 (discretize() takes the extrema of float16 samples)."""
-    return np.clip(np.asarray(x, dtype=np.float64), -65504.0, 65504.0).astype(np.float16).astype(np.float64)
-
-
-def _linspace_rows(lo, hi, S):
-    """Rows of np.linspace(lo, hi, S + 1) without their two ends: the S - 1 endpoints of an S-bin uniform grid."""
-    return np.linspace(lo, hi, S + 1, axis=1)[:, 1:-1].copy()
-
-
-def _family_extrema(family, L, rs):
-    u = lambda a, b: rs.uniform(a, b, L)                                       # noqa: E731
-    sgn = rs.choice([-1.0, 1.0], L)
-    if family == 1:                                           # off-centre: centre within +-1000, span 1 .. 21
-        c, w = u(-1000, 1000), u(1, 21)
-        lo = _half(c - w * u(0.2, 0.8))
-        return lo, _half(lo + w)
-    if family == 2:                                           # float16 extrema at or near +-65504, possibly asymmetric
-        k = rs.randint(0, 4, L)
-        lo = np.where(k == 0, -65504.0, _half(-u(30000, 65504)))
-        hi = np.where(k == 1, 65504.0, np.where(k == 2, _half(u(-1000, 60000)), _half(u(30000, 65504))))
-        lo[k == 3], hi[k == 3] = -65504.0, 65504.0
-        return lo, hi
-    if family == 3:                                           # far from zero and narrow: |centre| in 30000 .. 60000, span <= 1
-        c, w = sgn * u(30000, 60000), u(1e-3, 1)
-        lo = c - w * u(0.2, 0.8)
-        return lo, lo + w
-    if family == 4:                                           # tiny spans 2^-20 .. 2^-24, at 0 and at 1000
-        c, w = rs.choice([0.0, 1000.0], L), np.ldexp(1.0, -rs.randint(20, 25, L))
-        lo = c - w * u(0.2, 0.8)
-        return lo, lo + w
-    if family == 5:                                           # ordinary spans; sigma puts dt at the plan's limit of 64
-        lo = _half(u(-10, 5))
-        return lo, _half(lo + u(0.5, 20))
-    lo = u(-300, 300)                                         # 6: perturbed off the affine line (below)
-    return lo, lo + np.exp(u(np.log(0.5), np.log(100.0)))
-
-
-def _draw(lo, hi, S, B, rs, family=0):
-    """mu, sigma [B, L] (float32) relative to each row's centre c, half-width h and bin width d: a few bins live, many live,
-    mass just beyond the grid, or anything in between.  Constant rows (d = 0) get sigma in [0.1, 1] around their value."""
-    L = lo.shape[0]
-    c, h = 0.5 * (lo + hi), 0.5 * (hi - lo)
-    d = (hi - lo) / S
-    u = lambda a, b: rs.uniform(a, b, (B, L))                                  # noqa: E731
-    kind = rs.randint(0, 4, (B, L))
-    sc = np.select([kind == 0, kind == 1, kind == 2],
-                   [d * 10 ** u(-1.5, 0.5), h * u(0.05, 0.6), d * 10 ** u(-1, 1.5)],
-                   d * 10 ** (u(0, 1) * np.log10(np.maximum(1.0, h / np.where(d > 0, d, 1.0)))))
-    mu = np.where(kind == 2, c + rs.choice([-1.0, 1.0], (B, L)) * (h + sc * u(0, 12)), c + h * u(-1.2, 1.2))
-    if family == 5:
-        sc = d / (64.0 * u(0.97, 1.03))
-        mu = c + h * u(-1, 1)
-    flat = np.broadcast_to(d <= 0, (B, L))
-    sc = np.where(flat, u(0.1, 1.0), sc)
-    mu = np.where(flat, c + u(-1, 1), mu)
-    return mu.astype(np.float32), np.maximum(sc.astype(np.float32), np.float32(1e-38))
-
-
-def _family_case(family, L, S, B, seed):
-    rs = np.random.RandomState(seed)
-    lo, hi = _family_extrema(family, L, rs)
-    ends = _linspace_rows(lo, hi, S)
-    mu, sc = _draw(lo, hi, S, B, rs, family)
-    if family == 6:                     # every interior endpoint off the line by up to dv, one of them by exactly dv:
-        emax = np.maximum(np.abs(lo), np.abs(hi))              # dv up to the classification tolerance 1e-13 max(1, emax)
-        dv = 1e-13 * np.maximum(1.0, emax) * 10 ** rs.uniform(-6, 0, L)
-        ends[:, 1:-1] += dv[:, None] * rs.uniform(-1, 1, (L, S - 3))
-        ends[np.arange(L), rs.randint(1, S - 2, L)] += rs.choice([-1.0, 1.0], L) * dv
-    return ends, mu, sc
 
 
 def _affine_rule(ends):
@@ -125,7 +53,7 @@ def _symbols(B, L, S, rs):
 def _special_rows(S):
     """One row per level, each a grid discretize() can build or a row just either side of the rule."""
     def lin(lo, hi):
-        return _linspace_rows(np.array([lo]), np.array([hi]), S)[0]
+        return linspace_rows(np.array([lo]), np.array([hi]), S)[0]
 
     def perturbed(f):
         e = lin(-300.0, 200.0)
@@ -133,7 +61,7 @@ def _special_rows(S):
         return e
     return {
         "float16 +-65504": lin(-65504.0, 65504.0),
-        "float16 -65504 .. 1234": lin(-65504.0, float(_half(1234.3))),
+        "float16 -65504 .. 1234": lin(-65504.0, float(half(1234.3))),
         "one float16 ulp at 1000": lin(1000.0, 1000.5),
         "one float16 ulp at -2": lin(-2.0, -2.0 + 2.0 ** -10),
         "one float16 ulp at 0 (subnormal)": lin(0.0, 2.0 ** -24),
@@ -155,7 +83,7 @@ def test_row_classification_matches_the_rule_and_every_level_codes_exactly(q):
     L = cfg.zdim
     rs = np.random.RandomState(q)
     lo, hi = -6 - rs.uniform(0, 1, (cfg.nz, L)), 6 + rs.uniform(0, 1, (cfg.nz, L))
-    zend = np.stack([_linspace_rows(lo[i], hi[i], S) for i in range(cfg.nz)])
+    zend = np.stack([linspace_rows(lo[i], hi[i], S) for i in range(cfg.nz)])
     at = [(37 * i + 5) % L for i in range(cfg.nz)]
     for i, row in enumerate(special.values()):
         zend[i, at[i]] = row
@@ -171,13 +99,13 @@ def test_row_classification_matches_the_rule_and_every_level_codes_exactly(q):
     for i, name in enumerate(names):
         ends = zend[i]
         elo, ehi = ends[:, 0] - (ends[:, -1] - ends[:, 0]) / (S - 2), ends[:, -1] + (ends[:, -1] - ends[:, 0]) / (S - 2)
-        mu, sc = _draw(elo, ehi, S, B, rs)
+        mu, sc = draw(elo, ehi, S, B, rs)
         sym = _symbols(B, L, S, rs)
-        states = _states(B, seed=40 + i, n=1500)
-        res = _run_2p(ends, mu, sc, S, q, states, sym, mode=-1)
-        gen = _run_2p(ends, mu, sc, S, q, states, sym, mode=0)
+        states = initial_states(B, seed=40 + i, n=1500)
+        res = run_2p(ends, mu, sc, S, q, states, sym, mode=-1)
+        gen = run_2p(ends, mu, sc, S, q, states, sym, mode=0)
         assert gen[0] == res[0] and np.array_equal(gen[1], res[1]) and gen[2] == res[2], name
-        _check_vs_oracle(res, _oracle_tables(ends, mu, sc, S, q), states, sym, range(B))
+        check_vs_oracle(res, oracle_tables(ends, mu, sc, S, q), states, sym, range(B))
 
 
 # ---- full-size levels of every grid family in verify mode ------------------------------------------------------------------
@@ -192,16 +120,13 @@ def test_affine_rows_verified_on_every_grid_family(family, S):
     so that a level with some rows outside the rule still runs them (those rows take the exact path for every bin)."""
     q = S.bit_length() - 1
     L, B = 2048, 4
-    ends, mu, sc = _family_case(family, L, S, B, seed=1000 * family + S)
+    ends, mu, sc = family_case(family, L, S, B, seed=1000 * family + S)
     sym = _symbols(B, L, S, np.random.RandomState(S + family))
-    states = _states(B, seed=70 * family, n=6000)
-    check(lib().bsw_rows6_set_verify(1))
+    states = initial_states(B, seed=70 * family, n=6000)
     stats = np.zeros(4, dtype=np.uint64)
-    try:
-        got = _run_2p(ends, mu, sc, S, q, states, sym, mode=1)
+    with coder_paths(verify=1):
+        got = run_2p(ends, mu, sc, S, q, states, sym, mode=1)
         check(lib().bsw_rows6_verify_read(stats.ctypes.data))
-    finally:
-        check(lib().bsw_rows6_set_verify(0))
     mism, worst, checked, exact_path = (int(v) for v in stats)
     n_aff = int(_affine_rule(ends).sum())
     print(f"{FAMILIES[family]} S={S}: {n_aff} of {L} rows affine, {checked} bins evaluated of {2 * B * L * S}, exact path "
@@ -210,7 +135,7 @@ def test_affine_rows_verified_on_every_grid_family(family, S):
     assert checked > 0 and mism == 0
     assert worst <= 250, worst
     if n_aff == L:                                        # the classification picks these kernels by itself
-        cls = _run_2p(ends, mu, sc, S, q, states, sym, mode=-1)
+        cls = run_2p(ends, mu, sc, S, q, states, sym, mode=-1)
         assert got[0] == cls[0] and np.array_equal(got[1], cls[1]) and got[2] == cls[2]
     _check_picked_vs_oracle(got, ends, mu, sc, S, q, states, sym)
 
@@ -218,7 +143,7 @@ def test_affine_rows_verified_on_every_grid_family(family, S):
 def _check_picked_vs_oracle(res, ends, mu, sc, S, q, states, sym, picks=(0, 3)):
     picks = list(picks)
     sub = ([res[0][b] for b in picks], res[1][picks], [res[2][b] for b in picks])
-    _check_vs_oracle(sub, _oracle_tables(ends, mu[picks], sc[picks], S, q), [states[b] for b in picks], sym[picks],
+    check_vs_oracle(sub, oracle_tables(ends, mu[picks], sc[picks], S, q), [states[b] for b in picks], sym[picks],
                      range(len(picks)))
 
 
@@ -228,10 +153,10 @@ def test_generic_kernels_on_every_grid_family(family, S):
     the affine rule): streams and symbols equal to the oracle's."""
     q = S.bit_length() - 1
     L, B = 2048, 4
-    ends, mu, sc = _family_case(family, L, S, B, seed=1000 * family + S)
+    ends, mu, sc = family_case(family, L, S, B, seed=1000 * family + S)
     sym = _symbols(B, L, S, np.random.RandomState(S + family))
-    states = _states(B, seed=70 * family, n=6000)
-    _check_picked_vs_oracle(_run_2p(ends, mu, sc, S, q, states, sym, mode=0), ends, mu, sc, S, q, states, sym)
+    states = initial_states(B, seed=70 * family, n=6000)
+    _check_picked_vs_oracle(run_2p(ends, mu, sc, S, q, states, sym, mode=0), ends, mu, sc, S, q, states, sym)
 
 
 # ---- degenerate rows on the generic and fused coders -----------------------------------------------------------------------
@@ -245,28 +170,11 @@ def _degenerate_case(L, S, B, seed):
     lo[kind == 2] = rs.choice([0.0, 1000.0], (kind == 2).sum())
     hi[kind == 2] = lo[kind == 2] + np.ldexp(1.0, -rs.randint(20, 25, (kind == 2).sum()))
     lo[kind == 3], hi[kind == 3] = 1.0, 1.0 + 2.0 ** -10                # one float16 ulp: S - 1 endpoints in [1, 1 + 2^-10]
-    ends = _linspace_rows(lo, hi, S)
-    ends[kind == 1] = _half(ends[kind == 1])
+    ends = linspace_rows(lo, hi, S)
+    ends[kind == 1] = half(ends[kind == 1])
     ends[kind == 4] = np.repeat(ends[kind == 4][:, ::8], 8, axis=1)[:, :S - 1]    # equal in runs of 8
-    mu, sc = _draw(lo, hi, S, B, rs)
+    mu, sc = draw(lo, hi, S, B, rs)
     return ends, mu, sc
-
-
-def _run_fused(ends, mu, sc, S, q, states, sym):
-    B, L = mu.shape
-    e_pad = torch.from_numpy(_pad_big(ends)).to(dev)
-    dmu, dsc, dsym = torch.from_numpy(mu).to(dev), torch.from_numpy(sc).to(dev), torch.from_numpy(sym).to(dev)
-    ss = StreamSet(B, 1 << 15)
-    ss.import_lists(states)
-    out = torch.zeros((B, L), dtype=torch.int16, device=dev)
-    check(lib().bsw_logistic_pop(ss.handle, 0, B, dmu.data_ptr(), L, dsc.data_ptr(), L, e_pad.data_ptr(), S, out.data_ptr(), L, S,
-                                 31, q, cuda_stream_ptr()))
-    ss.raise_on_error()
-    a, popped = ss.export_lists(), out.cpu().numpy().copy()
-    check(lib().bsw_logistic_push(ss.handle, 0, B, dmu.data_ptr(), L, dsc.data_ptr(), L, e_pad.data_ptr(), S, dsym.data_ptr(), L,
-                                  S, 31, q, cuda_stream_ptr()))
-    ss.raise_on_error()
-    return a, popped, ss.export_lists()
 
 
 @pytest.mark.parametrize("coder", ["generic", "classified", "affine", "fused"])
@@ -282,44 +190,13 @@ def test_degenerate_rows_on_the_generic_and_fused_coders(S, coder):
     ends, mu, sc = _degenerate_case(L, S, B, seed=S)
     assert (np.diff(ends, axis=1) == 0).any(axis=1).sum() >= L // 3
     sym = _symbols(B, L, S, np.random.RandomState(S + 1))
-    states = _states(B, seed=S, n=2000)
-    tabs = _oracle_tables(ends, mu, sc, S, q)
+    states = initial_states(B, seed=S, n=2000)
+    tabs = oracle_tables(ends, mu, sc, S, q)
     if coder == "fused":
-        res = _run_fused(ends, mu, sc, S, q, states, sym)
+        res = run_fused(ends, mu, sc, S, q, states, sym)
     else:
-        res = _run_2p(ends, mu, sc, S, q, states, sym, {"generic": 0, "classified": -1, "affine": 1}[coder])
-    _check_vs_oracle(res, tabs, states, sym, range(B))
-
-
-def _push_pop(ends, mu, sc, S, q, states, sym, coder):
-    """push `sym`, then pop them again; returns (states after push, popped symbols, states after pop)."""
-    B, L = mu.shape
-    e_pad = torch.from_numpy(_pad_big(ends)).to(dev)
-    dmu, dsc, dsym = torch.from_numpy(mu).to(dev), torch.from_numpy(sc).to(dev), torch.from_numpy(sym).to(dev)
-    nbytes = int(lib().bsw_logistic_scratch_bytes(B, L, S, 0))
-    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    ss = StreamSet(B, 1 << 15)
-    ss.import_lists(states)
-    out = torch.zeros((B, L), dtype=torch.int16, device=dev)
-    args = (dmu.data_ptr(), L, dsc.data_ptr(), L, e_pad.data_ptr(), S)
-    check(lib().bsw_set_rows_mode({"generic": 0, "classified": -1, "affine": 1, "fused": -1}[coder]))
-    try:
-        if coder == "fused":
-            check(lib().bsw_logistic_push(ss.handle, 0, B, *args, dsym.data_ptr(), L, S, 31, q, cuda_stream_ptr()))
-            ss.raise_on_error()
-            pushed = ss.export_lists()
-            check(lib().bsw_logistic_pop(ss.handle, 0, B, *args, out.data_ptr(), L, S, 31, q, cuda_stream_ptr()))
-        else:
-            check(lib().bsw_logistic_push_2p(ss.handle, 0, B, *args, dsym.data_ptr(), L, S, 31, q, scratch.data_ptr(), nbytes,
-                                             cuda_stream_ptr()))
-            ss.raise_on_error()
-            pushed = ss.export_lists()
-            check(lib().bsw_logistic_pop_2p(ss.handle, 0, B, *args, out.data_ptr(), L, S, 31, q, scratch.data_ptr(), nbytes,
-                                            cuda_stream_ptr()))
-        ss.raise_on_error()
-        return pushed, out.cpu().numpy().copy(), ss.export_lists()
-    finally:
-        check(lib().bsw_set_rows_mode(-1))
+        res = run_2p(ends, mu, sc, S, q, states, sym, {"generic": 0, "classified": -1, "affine": 1}[coder])
+    check_vs_oracle(res, tabs, states, sym, range(B))
 
 
 ROUNDTRIP_CASES = [("tiny span", S) for S in (32, 256, 1024)] + [("degenerate", S) for S in (32, 1024, 4096)]
@@ -337,15 +214,15 @@ def test_push_then_pop_round_trip_on_tiny_and_degenerate_rows(rows, S, coder):
     q = S.bit_length() - 1
     B = 4
     if rows == "tiny span":
-        ends, mu, sc = _family_case(4, 1024, S, B, seed=5000 + S)
+        ends, mu, sc = family_case(4, 1024, S, B, seed=5000 + S)
     else:
         ends, mu, sc = _degenerate_case(300, S, B, seed=S + 9)
     L = ends.shape[0]
     sym = _symbols(B, L, S, np.random.RandomState(S + 2))
-    states = _states(B, seed=S + 3, n=500)
-    pushed, popped, back = _push_pop(ends, mu, sc, S, q, states, sym, coder)
+    states = initial_states(B, seed=S + 3, n=500)
+    pushed, popped, back = push_pop(ends, mu, sc, S, q, states, sym, coder)
     assert np.array_equal(popped, sym) and back == states
-    tabs = _oracle_tables(ends, mu, sc, S, q)
+    tabs = oracle_tables(ends, mu, sc, S, q)
     for b in range(B):
         assert pushed[b] == O.AnsC(tables=tabs[b]).encode(O.CState.from_list(states[b]), sym[b].astype(np.int64)).to_list()
 
@@ -360,13 +237,13 @@ def test_exported_pmfs_equal_the_reference_expression_on_every_grid_family(famil
         if family == "degenerate":
             ends, mu, sc = _degenerate_case(L, S, 1, seed=S + 3)
         else:
-            ends, mu, sc = _family_case(family, L, S, 1, seed=77 * family + S)
+            ends, mu, sc = family_case(family, L, S, 1, seed=77 * family + S)
         e = torch.from_numpy(np.ascontiguousarray(ends)).to(dev)
         m = torch.from_numpy(mu[0]).double().to(dev)
         s = torch.from_numpy(sc[0]).double().to(dev)
         out = torch.empty((L, S), dtype=torch.float64, device=dev)
         check(lib().bsw_logistic_pmfs(e.data_ptr(), S - 1, m.data_ptr(), s.data_ptr(), 1, L, S, out.data_ptr(), cuda_stream_ptr()))
-        ref = _ref_pmfs_cuda(e, m, s)
+        ref = ref_pmfs_cuda(e, m, s)
         assert torch.equal(out, ref), f"S={S}: {(out != ref).sum().item()} of {out.numel()} pmfs differ from torch-CUDA"
 
 
@@ -416,14 +293,14 @@ def test_codec_on_discretized_bins_with_a_constant_dimension_vs_oracle(name, q, 
     codec = BitSwapCodec(cfg, m, bins, B)
     ss = StreamSet(B, 1 << 15)
     imgs = synthetic.synthetic_images(cfg, B * nimg, seed=31, kind="smooth").reshape(nimg, B, *cfg.xs)
-    states = _states(B, seed=200, n=4000)
+    states = initial_states(B, seed=200, n=4000)
     ss.import_lists(states)
     for xi in range(nimg):
         codec.encode(ss, torch.from_numpy(imgs[xi]).cuda(), scheme=scheme)
     ss.raise_on_error()
     got = ss.export_lists()
     for b in range(B):
-        orc = _oracle_with(cfg, m, sd, zend, zcen)
+        orc = gpu_oracle(cfg, m, sd, zend, zcen, cls=O.BitSwapOracle)
         st = O.CState.from_list(states[b])
         for xi in range(nimg):
             st = (orc.encode_image if scheme == BITSWAP else orc.encode_image_bbans)(st, imgs[xi, b])

@@ -9,7 +9,6 @@
    (tests/golden/make_golden_kw.py).
 """
 import ctypes
-import json
 import os
 import re
 import subprocess
@@ -21,11 +20,10 @@ import torch
 from bitswap_b200 import _lib, synthetic
 from bitswap_b200.config import CodecConfig
 from bitswap_b200.model import Model, _Desc
-from bitswap_b200.rand import ImageBins
+from codec_harness import KW_MODELS, golden_model, model_oracle_vs_golden
 from oracle import oracle as O
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-KW_MODELS = ["kw_k5_w100", "kw_k1_w12", "kw_k7_w16"]
 
 
 @pytest.fixture(scope="module")
@@ -102,43 +100,13 @@ def test_model_create_refuses_other_kernels(ks, rc):
     assert "kernel_size" in _lib.lib().bsw_last_error().decode()
 
 
-def _golden(name):
-    g = np.load(os.path.join(GOLDEN, f"model_{name}.npz"))
-    c = json.loads(str(g["cfg"]))
-    c["xs"] = tuple(c["xs"])
-    return CodecConfig(**c), g
-
-
-def model_oracle_vs_golden(name, net, tol):
-    """Runs net(kind, level, given [1, dim] float64) -> (mu, scale) on the golden inputs of `name`; every output within
-    tol(want) of the reference's."""
-    cfg, g = _golden(name)
-    _, zcen = synthetic.synthetic_bins(cfg, seed=0)
-    xcen = ImageBins(torch.float64, "cpu", cfg.xdim).centres()
-    zr = torch.arange(cfg.zdim)
-    worst = 0.0
-    for i in range(cfg.nz):
-        if i == 0:
-            given = xcen[torch.arange(cfg.xdim), torch.from_numpy(g["x"].astype(np.int64))]
-        else:
-            given = zcen[i - 1, zr, torch.from_numpy(g[f"zsym_in_infer{i}"].astype(np.int64))]
-        z = zcen[i, zr, torch.from_numpy(g[f"zsym_in_gen{i}"].astype(np.int64))]
-        for kind, inp, key in (("infer", given, f"infer{i}"), ("generate", z, f"gen{i}")):
-            mu, sc = net(kind, i, inp.unsqueeze(0))
-            for got, want in ((mu, g[key + "_mu"]), (sc, g[key + "_scale"])):
-                err = np.abs(got[0].detach().cpu().double().numpy() - want)
-                worst = max(worst, float(err.max()))
-                assert np.all(err < tol(want)), f"{name} {key}: max |err| {err.max():.3e}"
-    return worst
-
-
 @pytest.mark.parametrize("name", KW_MODELS)
 def test_kw_model_oracle_matches_reference(name):
     """The oracle builds --kernel 5 / 1 / 7 models as the reference does: float32 within 2e-6 absolute of the golden
     outputs (measured: identical), float64 within 2e-5 relative to max(1, |output|).  The golden outputs carry the
     reference's float32 rounding, which grows with the taps summed: measured 9.6e-7 (1x1), 3.2e-6 (5x5) and 6.9e-6
     (7x7) absolute against the float64 oracle."""
-    cfg, _ = _golden(name)
+    cfg, _ = golden_model(name)
     sd = synthetic.synthetic_state_dict(cfg, seed=50, varied=True)
     for dtype, tol in ((torch.float32, lambda want: 2e-6), (torch.float64, lambda want: 2e-5 * np.maximum(1.0, np.abs(want)))):
         orc = O.ModelOracle(cfg, sd, dtype=dtype)

@@ -1,6 +1,6 @@
 """Models of any kernel size (1, 3, 5, 7) and of padded width 128 or 192 on the tensor cores.
 
-1. P3c per layer: every conv kind on its own against float64, with the harness of test_conv_f64_gpu (same inputs, value
+1. P3c per layer: every conv kind on its own against float64, with the harness of conv_harness.py (same inputs, value
    sets, bars tau = 2^-13 / 2^-14 and exact checks), on [2, MAXB, 256, Wp] plane buffers: widths 65..192 at kernel 3,
    kernels 1 / 5 / 7 at widths 61, 128, 192 and 252.  Conv modes 8 / 15 must be bit-identical to 0 / 7.  The worst
    normalised error is reported per (path, conv kind, kernel size, padded width).
@@ -9,151 +9,67 @@
 4. The Bit-Swap recursion through PipelinedCodec defaults against the oracle, exact round trips, and edge-coded
    containers, for a padded-width-128 and a padded-width-192 model with kernel sizes 5 and 7.
 """
-import os
-import sys
-
 import numpy as np
 import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-
-import test_conv_f64_gpu as F                                          # noqa: E402
-from test_codec_gpu import _tc_case, TOL                               # noqa: E402
-from test_kernel_width_cpu import KW_MODELS, _golden, model_oracle_vs_golden   # noqa: E402
+from codec_harness import KW_MODELS, TOL, golden_model, gpu_oracle, model_oracle_vs_golden, tc_case   # noqa: E402
+from conv_harness import VALUES, Case, conv_cfg, outputs_in_conv_modes, worst_report   # noqa: E402
 from oracle import oracle as O                                         # noqa: E402
 from bitswap_b200 import synthetic                                     # noqa: E402
-from bitswap_b200.config import CodecConfig                            # noqa: E402
 from bitswap_b200.model import Model                                   # noqa: E402
-from bitswap_b200.codec import BitSwapCodec, Bins, PipelinedCodec      # noqa: E402
+from bitswap_b200.codec import Bins, PipelinedCodec                    # noqa: E402
 from bitswap_b200.container import compress_images, decompress_images  # noqa: E402
 from bitswap_b200.streams import StreamSet                             # noqa: E402
-from bitswap_b200._lib import lib, check                               # noqa: E402
-
-
-def _cfg(C, zc, W, ks, cond=False, nz=2):
-    return CodecConfig(xs=(C, 32, 32), nz=nz, zchannels=zc, nprocessing=1, resdepth=2, reswidth=W, kernel_size=ks,
-                       cond_xscale=cond)
-
 
 # (tensor cores?, config).  zchannels <= 32 run the in-conv on the tensor cores, 40 the SIMT in-conv + split; heads of
 # <= 32 outputs run on the tensor cores, 40 and 80 on k_conv_simt after a tensor-core trunk.
 MODELS = {
     # padded width 128 / 192 at kernel 3
-    "tc k3 W65 zc1 C3": (True, _cfg(3, 1, 65, 3)),
-    "tc k3 W100 zc20 C3": (True, _cfg(3, 20, 100, 3)),
-    "tc k3 W128 zc40 C1 cond": (True, _cfg(1, 40, 128, 3, True)),
-    "tc k3 W129 zc2 C1 cond": (True, _cfg(1, 2, 129, 3, True)),
-    "tc k3 W150 zc40 C3": (True, _cfg(3, 40, 150, 3)),
-    "tc k3 W192 zc16 C1": (True, _cfg(1, 16, 192, 3)),
+    "tc k3 W65 zc1 C3": (True, conv_cfg(3, 1, 65, 3)),
+    "tc k3 W100 zc20 C3": (True, conv_cfg(3, 20, 100, 3)),
+    "tc k3 W128 zc40 C1 cond": (True, conv_cfg(1, 40, 128, 3, cond=True)),
+    "tc k3 W129 zc2 C1 cond": (True, conv_cfg(1, 2, 129, 3, cond=True)),
+    "tc k3 W150 zc40 C3": (True, conv_cfg(3, 40, 150, 3)),
+    "tc k3 W192 zc16 C1": (True, conv_cfg(1, 16, 192, 3)),
     # kernel sizes 1 / 5 / 7 at padded widths 64, 128, 192, 256
-    "tc k1 W61 zc8 C3": (True, _cfg(3, 8, 61, 1)),
-    "tc k1 W128 zc20 C1 cond": (True, _cfg(1, 20, 128, 1, True)),
-    "tc k1 W192 zc1 C3": (True, _cfg(3, 1, 192, 1)),
-    "tc k1 W252 zc40 C1": (True, _cfg(1, 40, 252, 1)),
-    "tc k5 W61 zc40 C1": (True, _cfg(1, 40, 61, 5)),
-    "tc k5 W128 zc2 C3 cond": (True, _cfg(3, 2, 128, 5, True)),
-    "tc k5 W192 zc20 C3": (True, _cfg(3, 20, 192, 5)),
-    "tc k5 W252 zc8 C1": (True, _cfg(1, 8, 252, 5)),
-    "tc k7 W61 zc20 C3": (True, _cfg(3, 20, 61, 7)),
-    "tc k7 W128 zc8 C1": (True, _cfg(1, 8, 128, 7)),
-    "tc k7 W192 zc40 C3 cond": (True, _cfg(3, 40, 192, 7, True)),
-    "tc k7 W252 zc2 C1 cond": (True, _cfg(1, 2, 252, 7, True)),
+    "tc k1 W61 zc8 C3": (True, conv_cfg(3, 8, 61, 1)),
+    "tc k1 W128 zc20 C1 cond": (True, conv_cfg(1, 20, 128, 1, cond=True)),
+    "tc k1 W192 zc1 C3": (True, conv_cfg(3, 1, 192, 1)),
+    "tc k1 W252 zc40 C1": (True, conv_cfg(1, 40, 252, 1)),
+    "tc k5 W61 zc40 C1": (True, conv_cfg(1, 40, 61, 5)),
+    "tc k5 W128 zc2 C3 cond": (True, conv_cfg(3, 2, 128, 5, cond=True)),
+    "tc k5 W192 zc20 C3": (True, conv_cfg(3, 20, 192, 5)),
+    "tc k5 W252 zc8 C1": (True, conv_cfg(1, 8, 252, 5)),
+    "tc k7 W61 zc20 C3": (True, conv_cfg(3, 20, 61, 7)),
+    "tc k7 W128 zc8 C1": (True, conv_cfg(1, 8, 128, 7)),
+    "tc k7 W192 zc40 C3 cond": (True, conv_cfg(3, 40, 192, 7, cond=True)),
+    "tc k7 W252 zc2 C1 cond": (True, conv_cfg(1, 2, 252, 7, cond=True)),
     # the float32 SIMT path at kernel sizes 1 and 7 (dense convs too)
-    "simt k1 W100 zc20 C1": (False, _cfg(1, 20, 100, 1)),
-    "simt k7 W63 zc2 C3 cond": (False, _cfg(3, 2, 63, 7, True)),
+    "simt k1 W100 zc20 C1": (False, conv_cfg(1, 20, 100, 1)),
+    "simt k7 W63 zc2 C3 cond": (False, conv_cfg(3, 2, 63, 7, cond=True)),
 }
-MINE = {}                                    # (path, kind, "k{ks} Wp{Wp}") -> worst normalised error
+MINE = {}                                    # ("k{ks} Wp{Wp}", path, kind) -> worst normalised error
+_report = worst_report("P3c per kernel size and padded width: worst |out - f(y)| / s (beyond the ELU/rounding allowance)",
+                       MINE)
 
 
-@pytest.fixture(scope="module", autouse=True)
-def _report(request):
-    yield
-    tr = request.config.pluginmanager.getplugin("terminalreporter")
-    capman = request.config.pluginmanager.getplugin("capturemanager")
-    if tr is None or capman is None or not MINE:
-        return
-    with capman.global_and_fixture_disabled():
-        tr.write_line("")
-        tr.write_line("P3c per kernel size and padded width: worst |out - f(y)| / s (beyond the ELU/rounding allowance)")
-        for (path, kind, tag), v in sorted(MINE.items(), key=lambda kv: (kv[0][2], kv[0][0], kv[0][1])):
-            tr.write_line(f"  {tag:10s} {path:4s} {kind:16s} {v:.3e}  "
-                          f"(2^{np.log2(v) if v > 0 else float('-inf'):.1f}, bar 2^{np.log2(F.TAU[path]):.0f})")
-
-
-def _bits(t):
-    return t.view(torch.int32) if t.dtype == torch.float32 else t
-
-
-class KwCase(F.Case):
-    """F.Case on a model of any kernel size and padded width: Wp-wide plane buffers, the dense conv of the kernel-size
-    blocks reported under its size, and every output of modes 8 / 15 compared bit for bit with modes 0 / 7."""
-
-    def __init__(self, name, vs):
-        self.tc, self.cfg = MODELS[name]
-        self.name, self.vs = name, vs
-        self.seed = 9000 + 17 * list(MODELS).index(name) + F.VALUES.index(vs)
-        self.sd = F._state_dict(self.cfg, vs, self.seed)
-        self.m = Model.from_config(self.cfg, max_batch=F.MAXB, use_tensor_cores=self.tc).load_state_dict(self.sd)
-        self.W, self.Wp = self.cfg.reswidth, -(-self.cfg.reswidth // 64) * 64
-        self.planes = torch.empty((2, F.MAXB, 256, self.Wp), dtype=torch.int16, device="cuda")
-        self.modes = F.MODES if self.tc else (-1,)
-        self._outs = None
-
-    def hook(self, prefix, inp, n, flags, Tb=None, Ab=None, planes=None, mu=None, sc=None):
-        super().hook(prefix, inp, n, flags, Tb, Ab, planes, mu, sc)
-        if self._outs is not None:
-            self._outs.append([t.clone() for t in (Tb, Ab, planes, mu, sc) if t is not None])
-
-    def each_mode(self, fn):
-        outs = {}
-        for mode in self.modes:
-            self._outs = []
-            if mode >= 0:
-                check(lib().bsw_set_conv_mode(mode))
-            try:
-                fn(f"{self.name} / {self.vs} / mode {mode}")
-            finally:
-                check(lib().bsw_set_conv_mode(-1))
-            outs[mode] = self._outs
-        self._outs = None
-        for a, b in ((0, 8), (7, 15)):
-            if a in outs and b in outs:
-                for x, y in zip(sum(outs[a], []), sum(outs[b], [])):
-                    assert torch.equal(_bits(x), _bits(y)), f"{self.name} / {self.vs}: mode {b} differs from mode {a}"
-
-    def run(self):
-        saved = dict(F.WORST)                # the f64 module's table stays its own
-        F.WORST.clear()
-        try:
-            super().run()
-        finally:
-            ks = self.cfg.kernel_size
-            for (path, kind), v in F.WORST.items():
-                if kind == "dense3":         # the kernel-size blocks (F.Case's "dense3" prefix gen_res1.0)
-                    kind = f"dense k{ks}"
-                key = (path, kind, f"k{ks} Wp{self.Wp}")
-                MINE[key] = max(MINE.get(key, 0.0), v)
-            F.WORST.clear()
-            F.WORST.update(saved)
-
-
-@pytest.mark.parametrize("vs", F.VALUES)
+@pytest.mark.parametrize("vs", VALUES)
 @pytest.mark.parametrize("name", list(MODELS))
 def test_kernel_width_conv_kernels_vs_float64(name, vs):
-    KwCase(name, vs).run()
+    Case(MODELS, name, vs, seed_base=9000, worst=MINE, compare_modes=True, per_kernel_width=True).run()
 
 
 NETS = {
-    "k3 W100 nz2": _cfg(3, 8, 100, 3),
-    "k3 W150 nz3 cond": _cfg(3, 8, 150, 3, True, nz=3),
-    "k5 W128 nz2": _cfg(3, 8, 128, 5),
-    "k7 W192 nz2 zc40": _cfg(3, 40, 192, 7),
-    "k1 W252 nz4": _cfg(3, 8, 252, 1, nz=4),
-    "k1 W65 nz3 zc20": _cfg(1, 20, 65, 1, nz=3),
-    "k7 W61 nz2 cond": _cfg(3, 2, 61, 7, True),
+    "k3 W100 nz2": conv_cfg(3, 8, 100, 3),
+    "k3 W150 nz3 cond": conv_cfg(3, 8, 150, 3, True, nz=3),
+    "k5 W128 nz2": conv_cfg(3, 8, 128, 5),
+    "k7 W192 nz2 zc40": conv_cfg(3, 40, 192, 7),
+    "k1 W252 nz4": conv_cfg(3, 8, 252, 1, nz=4),
+    "k1 W65 nz3 zc20": conv_cfg(1, 20, 65, 1, nz=3),
+    "k7 W61 nz2 cond": conv_cfg(3, 2, 61, 7, True),
 }
 
 
@@ -161,7 +77,7 @@ NETS = {
 def test_kernel_width_nets_vs_f64_oracle_and_simt(name):
     """Whole nets on the tensor cores: mu / sigma of every infer(i) / generate(i) within 1e-4 of the float64 oracle and
     of the SIMT path; a row alone equals the same row in the batch, bit for bit."""
-    worst_o, worst_s = _tc_case(NETS[name], 3, dtype=torch.float64)
+    worst_o, worst_s = tc_case(NETS[name], 3, dtype=torch.float64)
     print(f"tensor cores {name}: max |err| vs torch-f64 oracle {worst_o:.2e}, vs SIMT f32 path {worst_s:.2e}")
     assert worst_o < TOL and worst_s < TOL
 
@@ -170,28 +86,8 @@ def test_kernel_width_nets_vs_f64_oracle_and_simt(name):
 def test_kernel_width_persistent_grid_equals_per_tile_grid(name):
     """B = 170: 340 (Wp 128) / 1020 (Wp 192) tiles per dense conv, several per CTA on the persistent grid; in-convs with
     1 / 49 and 25 taps, dense convs, heads.  Bit-identical mu and sigma."""
-    B = 170
-    cfg = {"k7 W128": _cfg(3, 8, 128, 7, nz=3), "k1 W192": _cfg(1, 2, 192, 1, True, nz=3)}[name]
-    sd = synthetic.synthetic_state_dict(cfg, seed=61, varied=True)
-    m = Model.from_config(cfg, max_batch=B, use_tensor_cores=True).load_state_dict(sd)
-    m.compress()
-    rs = np.random.RandomState(4)
-    gx = torch.from_numpy((rs.randint(0, 256, (B, cfg.xdim)) - 127.5) / 127.5).cuda()
-    gz = torch.from_numpy(rs.uniform(-5, 5, (B, cfg.zdim))).cuda()
-    out = {}
-    try:
-        for mode in (0, 7):
-            check(lib().bsw_set_conv_mode(mode))
-            res = []
-            for i in range(cfg.nz):
-                mu, sc = m.infer(i)(gx if i == 0 else gz)
-                res += [mu.clone(), sc.clone()]
-                mu, sc = m.generate(i)(gz)
-                res += [mu.clone(), sc.clone()]
-            torch.cuda.synchronize()
-            out[mode] = res
-    finally:
-        check(lib().bsw_set_conv_mode(-1))
+    cfg = {"k7 W128": conv_cfg(3, 8, 128, 7, nz=3), "k1 W192": conv_cfg(1, 2, 192, 1, True, nz=3)}[name]
+    out = outputs_in_conv_modes(cfg, 170, (0, 7))
     for a, b in zip(out[0], out[7]):
         assert torch.equal(a, b), "conv mode 7"
     assert all(torch.isfinite(t).all() for t in out[7])
@@ -201,7 +97,7 @@ def test_kernel_width_persistent_grid_equals_per_tile_grid(name):
 @pytest.mark.parametrize("name", KW_MODELS)
 def test_kernel_width_model_matches_reference(name, tc):
     """Model (tensor cores and SIMT) within 1e-4 of the reference Model's outputs for --kernel 5 / 1 / 7."""
-    cfg, _ = _golden(name)
+    cfg, _ = golden_model(name)
     sd = synthetic.synthetic_state_dict(cfg, seed=50, varied=True)
     m = Model.from_config(cfg, max_batch=1, use_tensor_cores=tc).load_state_dict(sd)
     m.compress()
@@ -210,7 +106,7 @@ def test_kernel_width_model_matches_reference(name, tc):
     print(f"{name} {'tensor cores' if tc else 'SIMT'}: max |err| vs the reference {worst:.2e}")
 
 
-RECURSION = {"k5 W100": _cfg(3, 8, 100, 5), "k7 W150": _cfg(3, 8, 150, 7, nz=3)}
+RECURSION = {"k5 W100": conv_cfg(3, 8, 100, 5), "k7 W150": conv_cfg(3, 8, 150, 7, nz=3)}
 
 
 @pytest.mark.parametrize("name", list(RECURSION))
@@ -235,13 +131,7 @@ def test_kernel_width_recursion_vs_oracle_and_roundtrip(name):
     ss.raise_on_error()
     got = ss.export_lists()
     m = pc.models[0]
-    orc = O.BitSwapOracle(cfg, O.ModelOracle(cfg, sd), zend, zcen, coder="c", pmf="cuda")
-
-    def gpu_net(kind, level, given):
-        f = m.infer(level) if kind == "infer" else m.generate(level)
-        mu, sc = f(given.cuda())
-        return mu.cpu(), sc.cpu()
-    orc._net = gpu_net
+    orc = gpu_oracle(cfg, m, sd, zend, zcen, cls=O.BitSwapOracle)
     for b in sorted(set(int(v) for v in np.linspace(0, B - 1, nsample).round())):
         want = orc.encode_image(O.CState(w, head), imgs[b]).to_list()
         assert got[b] == want, f"{name}: stream {b} differs from the oracle"

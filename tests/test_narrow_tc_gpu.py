@@ -1,25 +1,20 @@
 """Tensor-core convs of models of padded width 64 (reswidth 1..64: the MNIST models) -- the narrow k_conv_wg tile.
 
-1. P3c on the narrow tile: every conv kind on its own against float64, with the harness of test_conv_f64_gpu (same
+1. P3c on the narrow tile: every conv kind on its own against float64, with the harness of conv_harness.py (same
    inputs, value sets, bar tau = 2^-13 and exact checks), on [2, MAXB, 256, 64] plane buffers; conv modes 8 / 15 (no
    multicast, which narrow launches never use) must be bit-identical to 0 / 7.
 2. Whole nets of mnist2/4/8 against the float64 oracle and the SIMT path, batch invariance, persistent == per-tile grid.
 3. The Bit-Swap recursion of mnist2 / mnist8 through PipelinedCodec with its defaults (tensor cores) against the oracle.
 4. compress_images(edges="code") on 28x28 digits and odd sizes with a tensor-core mnist2 codec: exact round trip.
 """
-import os
-import sys
-
 import numpy as np
 import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-
-import test_conv_f64_gpu as F                                          # noqa: E402
-from test_codec_gpu import _tc_case, TOL                               # noqa: E402
+from codec_harness import TOL, gpu_oracle, tc_case                     # noqa: E402
+from conv_harness import VALUES, Case, conv_cfg, outputs_in_conv_modes, worst_report   # noqa: E402
 from oracle import oracle as O                                         # noqa: E402
 from bitswap_b200 import synthetic                                     # noqa: E402
 from bitswap_b200.config import preset                                 # noqa: E402
@@ -27,96 +22,37 @@ from bitswap_b200.model import Model                                   # noqa: E
 from bitswap_b200.codec import BitSwapCodec, Bins, PipelinedCodec      # noqa: E402
 from bitswap_b200.container import compress_images, decompress_images  # noqa: E402
 from bitswap_b200.streams import StreamSet                             # noqa: E402
-from bitswap_b200._lib import lib, check                               # noqa: E402
 
 # (tensor cores?, config).  zchannels <= 32 run the in-conv on the narrow tile, 40 the SIMT in-conv + split into 64-wide
 # planes; heads of <= 32 outputs run on the tensor cores (cchunks = 2), 40 and 80 on k_conv_simt after a narrow trunk.
 MODELS = {
-    "tc W64 zc1 C1": (True, F._cfg(1, 1, 64)),                 # MNIST default width
-    "tc W61 zc1 C1": (True, F._cfg(1, 1, 61)),                 # mnist8
-    "tc W63 zc2 C3 cond": (True, F._cfg(3, 2, 63, True)),
-    "tc W15 zc8 C3": (True, F._cfg(3, 8, 15)),                 # 49 padded channels
-    "tc W62 zc16 C1": (True, F._cfg(1, 16, 62)),               # 32-output tensor-core heads
-    "tc W20 zc20 C3": (True, F._cfg(3, 20, 20)),               # SIMT heads; the z in-convs have the W -> W shape
-    "tc W64 zc40 C1": (True, F._cfg(1, 40, 64)),               # SIMT in-conv + split into narrow planes
+    "tc W64 zc1 C1": (True, conv_cfg(1, 1, 64)),                   # MNIST default width
+    "tc W61 zc1 C1": (True, conv_cfg(1, 1, 61)),                   # mnist8
+    "tc W63 zc2 C3 cond": (True, conv_cfg(3, 2, 63, cond=True)),
+    "tc W15 zc8 C3": (True, conv_cfg(3, 8, 15)),                   # 49 padded channels
+    "tc W62 zc16 C1": (True, conv_cfg(1, 16, 62)),                 # 32-output tensor-core heads
+    "tc W20 zc20 C3": (True, conv_cfg(3, 20, 20)),                 # SIMT heads; the z in-convs have the W -> W shape
+    "tc W64 zc40 C1": (True, conv_cfg(1, 40, 64)),                 # SIMT in-conv + split into narrow planes
 }
 WP = 64
+WORST = {}                                   # (path, kind) -> worst normalised error
+_report = worst_report("P3c on the narrow tile (padded width 64): worst |out - f(y)| / s (beyond the ELU/rounding allowance)",
+                       WORST)
 
 
-@pytest.fixture(scope="module", autouse=True)
-def _report(request):
-    saved = dict(F.WORST)                    # the f64 module's table stays its own
-    F.WORST.clear()
-    yield
-    mine = dict(F.WORST)
-    F.WORST.clear()
-    F.WORST.update(saved)
-    tr = request.config.pluginmanager.getplugin("terminalreporter")
-    capman = request.config.pluginmanager.getplugin("capturemanager")
-    if tr is None or capman is None or not mine:
-        return
-    with capman.global_and_fixture_disabled():
-        tr.write_line("")
-        tr.write_line("P3c on the narrow tile (padded width 64): worst |out - f(y)| / s (beyond the ELU/rounding allowance)")
-        for (path, kind), v in sorted(mine.items()):
-            tr.write_line(f"  {path:4s} {kind:16s} {v:.3e}  "
-                          f"(2^{np.log2(v) if v > 0 else float('-inf'):.1f}, bar 2^{np.log2(F.TAU[path]):.0f})")
-
-
-def _bits(t):
-    return t.view(torch.int32) if t.dtype == torch.float32 else t
-
-
-class NarrowCase(F.Case):
-    """F.Case on a narrow model: 64-wide plane buffers, and every output of modes 8 / 15 compared bit for bit with the
-    same run in modes 0 / 7."""
-
-    def __init__(self, name, vs):
-        self.tc, self.cfg = MODELS[name]
-        self.name, self.vs = name, vs
-        self.seed = 5000 + 17 * list(MODELS).index(name) + F.VALUES.index(vs)
-        self.sd = F._state_dict(self.cfg, vs, self.seed)
-        self.m = Model.from_config(self.cfg, max_batch=F.MAXB, use_tensor_cores=self.tc).load_state_dict(self.sd)
-        self.W, self.Wp = self.cfg.reswidth, -(-self.cfg.reswidth // 64) * 64
-        assert self.Wp == WP
-        self.planes = torch.empty((2, F.MAXB, 256, self.Wp), dtype=torch.int16, device="cuda")
-        self.modes = F.MODES if self.tc else (-1,)
-        self._outs = None
-
-    def hook(self, prefix, inp, n, flags, Tb=None, Ab=None, planes=None, mu=None, sc=None):
-        super().hook(prefix, inp, n, flags, Tb, Ab, planes, mu, sc)
-        if self._outs is not None:
-            self._outs.append([t.clone() for t in (Tb, Ab, planes, mu, sc) if t is not None])
-
-    def each_mode(self, fn):
-        outs = {}
-        for mode in self.modes:
-            self._outs = []
-            if mode >= 0:
-                check(lib().bsw_set_conv_mode(mode))
-            try:
-                fn(f"{self.name} / {self.vs} / mode {mode}")
-            finally:
-                check(lib().bsw_set_conv_mode(-1))
-            outs[mode] = self._outs
-        self._outs = None
-        for a, b in ((0, 8), (7, 15)):
-            if a in outs and b in outs:
-                for x, y in zip(sum(outs[a], []), sum(outs[b], [])):
-                    assert torch.equal(_bits(x), _bits(y)), f"{self.name} / {self.vs}: mode {b} differs from mode {a}"
-
-
-@pytest.mark.parametrize("vs", F.VALUES)
+@pytest.mark.parametrize("vs", VALUES)
 @pytest.mark.parametrize("name", list(MODELS))
 def test_narrow_conv_kernels_vs_float64(name, vs):
-    NarrowCase(name, vs).run()
+    case = Case(MODELS, name, vs, seed_base=5000, worst=WORST, compare_modes=True)
+    assert case.Wp == WP
+    case.run()
 
 
 @pytest.mark.parametrize("name", ["mnist2", "mnist4", "mnist8"])
 def test_narrow_nets_vs_f64_oracle_and_simt(name):
     """Whole nets on the tensor cores: mu / sigma of every infer(i) / generate(i) within 1e-4 of the float64 oracle and
     of the SIMT path; a row alone equals the same row in the batch, bit for bit."""
-    worst_o, worst_s = _tc_case(preset(name), 3, dtype=torch.float64)
+    worst_o, worst_s = tc_case(preset(name), 3, dtype=torch.float64)
     print(f"tensor cores {name}: max |err| vs torch-f64 oracle {worst_o:.2e}, vs SIMT f32 path {worst_s:.2e}")
     assert worst_o < TOL and worst_s < TOL
 
@@ -124,28 +60,7 @@ def test_narrow_nets_vs_f64_oracle_and_simt(name):
 def test_narrow_persistent_grid_equals_per_tile_grid():
     """B = 170: 340 half-image tiles per narrow conv, up to three per CTA on the persistent grid; in-convs with 1 and
     25 taps, dense 3x3 and 5x5, heads.  Bit-identical mu and sigma."""
-    B = 170
-    cfg = preset("mnist8")
-    sd = synthetic.synthetic_state_dict(cfg, seed=61, varied=True)
-    m = Model.from_config(cfg, max_batch=B, use_tensor_cores=True).load_state_dict(sd)
-    m.compress()
-    rs = np.random.RandomState(4)
-    gx = torch.from_numpy((rs.randint(0, 256, (B, cfg.xdim)) - 127.5) / 127.5).cuda()
-    gz = torch.from_numpy(rs.uniform(-5, 5, (B, cfg.zdim))).cuda()
-    out = {}
-    try:
-        for mode in (0, 7):
-            check(lib().bsw_set_conv_mode(mode))
-            res = []
-            for i in range(cfg.nz):
-                mu, sc = m.infer(i)(gx if i == 0 else gz)
-                res += [mu.clone(), sc.clone()]
-                mu, sc = m.generate(i)(gz)
-                res += [mu.clone(), sc.clone()]
-            torch.cuda.synchronize()
-            out[mode] = res
-    finally:
-        check(lib().bsw_set_conv_mode(-1))
+    out = outputs_in_conv_modes(preset("mnist8"), 170, (0, 7))
     for a, b in zip(out[0], out[7]):
         assert torch.equal(a, b), "conv mode 7"
     assert all(torch.isfinite(t).all() for t in out[7])
@@ -177,13 +92,7 @@ def test_narrow_recursion_vs_oracle_and_batch_roundtrip(name):
     assert got[0] == got[1] and got[0] != got[2]
     sample = sorted(set(int(v) for v in np.linspace(0, B - 1, nsample).round()))
     m = pc.models[0]
-    orc = O.BitSwapOracle(cfg, O.ModelOracle(cfg, sd), zend, zcen, coder="c", pmf="cuda")
-
-    def gpu_net(kind, level, given):
-        f = m.infer(level) if kind == "infer" else m.generate(level)
-        mu, sc = f(given.cuda())
-        return mu.cpu(), sc.cpu()
-    orc._net = gpu_net
+    orc = gpu_oracle(cfg, m, sd, zend, zcen, cls=O.BitSwapOracle)
     for b in sample:
         want = orc.encode_image(O.CState(w, head), imgs[b]).to_list()
         assert got[b] == want, f"{name}: stream {b} differs from the oracle"

@@ -3,33 +3,23 @@ a known-answer test the reference's own classes produced at S = 4096 (tests/gold
 argument checks that refuse quantbits outside [5, 12] before any device work."""
 import ctypes
 import hashlib
-import json
 import os
 
 import numpy as np
 import pytest
 import torch
 
+from coder_harness import KAT, kat_inputs
 from oracle import oracle as O
-from bitswap_b200 import synthetic
 from bitswap_b200.codec import Bins as DeviceBins, check_quantbits, MIN_QUANTBITS, MAX_QUANTBITS
 from bitswap_b200.config import preset, with_
 from bitswap_b200.rand import Bins
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-KAT = json.load(open(os.path.join(GOLDEN, "ans_kat_q12.json")))[0]
 
 
 def _sha(a):
     return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()[:16]
-
-
-def kat_inputs():
-    rs = np.random.RandomState(KAT["seed"])
-    pm = rs.dirichlet(np.ones(KAT["S"]) * 0.5, size=KAT["L"])
-    sym = rs.randint(0, KAT["S"], size=KAT["L"])
-    w, head = synthetic.initial_words(KAT["N"], seed=100)
-    return pm, sym, w, head
 
 
 def test_kat_shape():

@@ -3,6 +3,7 @@ every invalid request refused before any device work."""
 import numpy as np
 import pytest
 
+from codec_harness import NoDevice
 from bitswap_b200.container import (block_grid, chain_sizes, decompress_images, decompress_regions, pack_container,
                                     plan_regions)
 
@@ -13,13 +14,6 @@ def _container(h, w, L=None, seed=0):
     rs = np.random.RandomState(seed)
     sizes = chain_sizes(int(np.prod(block_grid(h, w))), L)
     return pack_container([(rs.randint(0, 1 << 32, 5, dtype=np.uint64).astype(np.uint32), 12345, nb) for nb in sizes], h, w)
-
-
-class NoDevice:
-    """A codec stand-in that fails the test if anything on it is touched."""
-
-    def __getattr__(self, name):
-        raise AssertionError(f"codec.{name} touched")
 
 
 def _plan(h, w, L, boxes):

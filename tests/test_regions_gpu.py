@@ -6,29 +6,15 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
+from codec_harness import Counting, random_images, setup                   # noqa: E402
 from bitswap_b200 import container, synthetic                              # noqa: E402
 from bitswap_b200.config import preset                                     # noqa: E402
-from bitswap_b200.model import Model                                       # noqa: E402
-from bitswap_b200.codec import BitSwapCodec, Bins, PipelinedCodec, BITSWAP, BBANS   # noqa: E402
+from bitswap_b200.codec import Bins, PipelinedCodec, BITSWAP, BBANS                 # noqa: E402
 from bitswap_b200.streams import StreamSet                                 # noqa: E402
 from bitswap_b200.container import (block_grid, chain_sizes, compress_images, decompress_images,   # noqa: E402
                                     decompress_regions, extract_blocks, extract_edge_blocks, plan_regions)
 
 N_INIT = 3000
-
-
-def _setup(name, B):
-    cfg = preset(name)
-    sd = synthetic.synthetic_state_dict(cfg, seed=50, varied=True)
-    m = Model.from_config(cfg, max_batch=B, use_tensor_cores=False).load_state_dict(sd)
-    m.compress()
-    bins = Bins(cfg, *synthetic.synthetic_bins(cfg, seed=0))
-    return cfg, sd, bins, BitSwapCodec(cfg, m, bins, B)
-
-
-def _images(C, sizes, seed):
-    rs = np.random.RandomState(seed)
-    return [rs.randint(0, 256, (h, w, C)).astype(np.uint8) for h, w in sizes]
 
 
 def _regions(rs, shapes, count):
@@ -53,21 +39,6 @@ def _check(codec, conts, regions, full, **kw):
         assert np.array_equal(g, want), (i, y, x, h, w)
 
 
-class Counting:
-    """Codec proxy counting decode calls and the blocks they pop."""
-
-    def __init__(self, codec):
-        self.codec, self.calls, self.blocks = codec, 0, 0
-
-    def __getattr__(self, name):
-        return getattr(self.codec, name)
-
-    def decode(self, ss, count, **kw):
-        self.calls += 1
-        self.blocks += count
-        return self.codec.decode(ss, count, **kw)
-
-
 CASES = [("tiny", BITSWAP, "crop"), ("tiny", BBANS, "code"), ("tiny3", BITSWAP, "code"), ("tiny3", BBANS, "crop")]
 
 
@@ -75,10 +46,10 @@ CASES = [("tiny", BITSWAP, "crop"), ("tiny", BBANS, "code"), ("tiny3", BITSWAP, 
 def test_regions_equal_crops_of_the_whole_image(name, scheme, edges):
     """Many regions in one call and one region per call, at chain_blocks None, 3 and 5; the codec pops exactly the
     planned blocks."""
-    cfg, sd, bins, codec = _setup(name, 8)
+    cfg, _, sd, _, _, bins, codec = setup(name, 8)
     C = cfg.xs[0]
     sizes = [(33, 65), (70, 100), (97, 40), (130, 33)] if edges == "code" else [(70, 100), (64, 96), (130, 33)]
-    images = _images(C, sizes, seed=61)
+    images = random_images(C, sizes, seed=61)
     rs = np.random.RandomState(62)
     for L in (None, 3, 5):
         conts = compress_images(codec, images, excess_state_len=N_INIT, scheme=scheme, edges=edges, chain_blocks=L)
@@ -100,8 +71,8 @@ def test_regions_equal_crops_of_the_whole_image(name, scheme, edges):
 def test_mixed_repeated_and_more_chains_than_max_batch():
     """Single- and multi-chain containers mixed and repeated, more streams than max_batch (three calls per step), through
     a BitSwapCodec and a free-running 2-lane PipelinedCodec; then an hwc_quirk crop container."""
-    cfg, sd, bins, codec = _setup("tiny3", 4)
-    images = _images(3, [(150, 130), (33, 65), (70, 100)], seed=63)             # 5 x 5, 2 x 3 and 3 x 4 blocks
+    cfg, _, sd, _, _, bins, codec = setup("tiny3", 4)
+    images = random_images(3, [(150, 130), (33, 65), (70, 100)], seed=63)             # 5 x 5, 2 x 3 and 3 x 4 blocks
     single = compress_images(codec, images, excess_state_len=N_INIT, edges="code")
     multi = compress_images(codec, images, excess_state_len=N_INIT, edges="code", chain_blocks=2)
     conts = [multi[0], single[1], multi[2], single[0], multi[0], single[2]]
@@ -124,7 +95,7 @@ def test_imagenetcrop4_tensor_cores():
     sd = synthetic.synthetic_state_dict(cfg, seed=50, varied=False)
     bins = Bins(cfg, *synthetic.synthetic_bins(cfg, seed=0))
     pc = PipelinedCodec(cfg, sd, bins, 8, lanes=2, use_tensor_cores=True, free_running=True)
-    images = _images(3, [(100, 200)], seed=65)                                   # 4 x 7 blocks: chains of 7, 7, 7, 7
+    images = random_images(3, [(100, 200)], seed=65)                                   # 4 x 7 blocks: chains of 7, 7, 7, 7
     conts = compress_images(pc, images, excess_state_len=4000, edges="code", chain_blocks=8)
     full = decompress_images(pc, conts)
     assert np.array_equal(full[0], images[0])
@@ -155,8 +126,8 @@ def _lone_states(codec, blocks, extents, scheme, n_init):
 def test_a_chain_stopped_part_way_holds_the_encoders_state(scheme, edges, monkeypatch):
     """After decoding a chain down to its earliest wanted block j, its stream holds the state the encoder had before block
     j, less the never-borrowed initial words the container trims."""
-    cfg, sd, bins, codec = _setup("tiny", 8)
-    img = _images(1, [(130, 97)], seed=66)[0]                                    # 5 x 4 blocks (4 x 3 cropped)
+    cfg, _, sd, _, _, bins, codec = setup("tiny", 8)
+    img = random_images(1, [(130, 97)], seed=66)[0]                                    # 5 x 4 blocks (4 x 3 cropped)
     L = 4
     conts = compress_images(codec, [img], excess_state_len=N_INIT, scheme=scheme, edges=edges, chain_blocks=L)
     if edges == "code":

@@ -1,28 +1,20 @@
 """The oracle's record of the reference's per-chain bookkeeping (restbits, excess_state_len, push depths) against the
 reference-classes golden traces, and StreamSet.bit_accounting's arithmetic against cifar_compress.py:253-259 written out
 literally.  CPU only."""
-import json
-import os
 
 import numpy as np
 import pytest
 import torch
 
+from codec_harness import bitswap_golden
 from oracle import oracle as O
 from bitswap_b200 import synthetic
 from bitswap_b200.config import preset
 from bitswap_b200.streams import StreamSet
 
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-
-
-def _golden(name):
-    return json.load(open(os.path.join(GOLDEN, f"bitswap_{name}.json")))
-
-
 def _chain(name, scheme, nimg=None):
     """The golden run's inputs through the oracle (coder "c", torch-CPU pmfs) -> (record, trace, golden)."""
-    g = _golden(name)
+    g = bitswap_golden(name)
     cfg = preset(name)
     torch.set_num_threads(4)
     m = O.ModelOracle(cfg, synthetic.synthetic_state_dict(cfg, seed=50, varied=True))
@@ -115,7 +107,7 @@ class _Sizes:
 def test_bit_accounting_is_the_reference_arithmetic(name):
     """Per image of the golden chain and of two made-up chains (one per stream), bit_accounting equals the reference's
     nets (as their running mean), cma, total and totaladdedbits."""
-    g = _golden(name)
+    g = bitswap_golden(name)
     cfg = preset(name)
     init = g["trace"][0][1]
     rest = dict((t, n) for t, n, _ in g["trace"])["img0 pop z1"]

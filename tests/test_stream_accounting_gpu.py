@@ -12,46 +12,16 @@ pytestmark = pytest.mark.gpu
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from edge_oracle import EdgeOracle                                     # noqa: E402
+from coder_harness import initial_states                               # noqa: E402
+from codec_harness import gpu_oracle, setup                            # noqa: E402
 from oracle import oracle as O                                         # noqa: E402
 from bitswap_b200 import synthetic                                     # noqa: E402
-from bitswap_b200.config import preset                                 # noqa: E402
 from bitswap_b200.model import Model                                   # noqa: E402
-from bitswap_b200.codec import BitSwapCodec, Bins, PipelinedCodec, BITSWAP, BBANS   # noqa: E402
+from bitswap_b200.codec import BitSwapCodec, PipelinedCodec, BITSWAP, BBANS   # noqa: E402
 from bitswap_b200.streams import StreamSet                             # noqa: E402
 from bitswap_b200 import container                                     # noqa: E402
 
 OVERFLOW = 2                                                           # BSW_E_OVERFLOW
-
-
-def _setup(name, B):
-    cfg = preset(name)
-    sd = synthetic.synthetic_state_dict(cfg, seed=50, varied=True)
-    m = Model.from_config(cfg, max_batch=B).load_state_dict(sd)
-    m.compress()
-    zend, zcen = synthetic.synthetic_bins(cfg, seed=0)
-    bins = Bins(cfg, zend, zcen)
-    return cfg, m, sd, zend, zcen, bins, BitSwapCodec(cfg, m, bins, B)
-
-
-def _oracle(cfg, m, sd, zend, zcen, record=None):
-    """The oracle recursion on the GPU nets and torch-CUDA float64 pmfs: lengths are exact, not statistical."""
-    orc = EdgeOracle(cfg, O.ModelOracle(cfg, sd), zend, zcen, coder="c", pmf="cuda", record=record)
-
-    def gpu_net(kind, level, given):
-        f = m.infer(level) if kind == "infer" else m.generate(level)
-        mu, sc = f(given.cuda())
-        return mu.cpu(), sc.cpu()
-    orc._net = gpu_net
-    return orc
-
-
-def _states(n, base, seed):
-    out = []
-    for b in range(n):
-        w, head = synthetic.initial_words(base + 37 * b, seed=seed + b)
-        out.append([int(v) for v in w] + [head])
-    return out
 
 
 def _reference_accounting(record, state_len, xdim, images):
@@ -78,7 +48,7 @@ def test_rest_min_words_and_accounting_vs_oracle(name, scheme, path):
     edge-coded _ext entry points with partial blocks; a sub-range call, which must leave the other streams alone."""
     B, nimg = 4, 3
     first, nstreams = (1, B + 2) if path == "subrange" else (0, B)
-    cfg, m, sd, zend, zcen, bins, codec = _setup(name, B)
+    cfg, m, sd, zend, zcen, bins, codec = setup(name, B)
     if path == "pipelined":
         codec = PipelinedCodec(cfg, sd, bins, B, lanes=2, use_tensor_cores=False)
         codec.set_dual_stream(True)
@@ -94,12 +64,12 @@ def test_rest_min_words_and_accounting_vs_oracle(name, scheme, path):
         exts = rs.randint(1, 33, size=(nimg, B, 2)).astype(np.int16)
         exts[0, 0] = (32, 32)
         exts[1, 1] = (1, 1)
-    states = _states(nstreams, 2500, seed=600)
+    states = initial_states(nstreams, seed=600, n=2500, step=37)
     ss = StreamSet(nstreams, 1 << 14)
     ss.import_lists(states)
     assert (ss.rest_words() == -1).all()
     records = [{} for _ in range(B)]
-    orcs = [_oracle(cfg, net_model, sd, zend, zcen, record=r) for r in records]
+    orcs = [gpu_oracle(cfg, net_model, sd, zend, zcen, record=r) for r in records]
     ost = [O.CState.from_list(states[first + b]) for b in range(B)]
     enc = "encode_image" if scheme == BITSWAP else "encode_image_bbans"
     for xi in range(nimg):
@@ -133,7 +103,7 @@ def test_fill_import_and_unpack_start_a_new_chain():
     """rest words go back to -1 wherever a new chain starts -- fill, import_lists, the plain and the trimmed unpack -- so
     that the next encode records the new chain's restbits instead of keeping the old chain's."""
     B = 3
-    cfg, m, sd, zend, zcen, bins, codec = _setup("tiny", B)
+    cfg, m, sd, zend, zcen, bins, codec = setup("tiny", B)
     imgs = torch.from_numpy(synthetic.synthetic_images(cfg, B, seed=63)).cuda()
     w, head = synthetic.initial_words(2000, seed=100)
     ss = StreamSet(B, 1 << 13)
@@ -152,7 +122,7 @@ def test_fill_import_and_unpack_start_a_new_chain():
     ss.fill(w, head)
     assert (ss.rest_words() == -1).all()
     assert np.array_equal(coded(), r0)                    # the same chain again: the same restbits
-    ss.import_lists(_states(B, 1500, seed=7))
+    ss.import_lists(initial_states(B, seed=7, n=1500, step=37))
     assert (ss.rest_words() == -1).all()
     coded()
     words, offs, heads = (a.copy() for a in ss.export_packed())
@@ -324,11 +294,11 @@ def test_capacity_is_exact_to_the_word(name, scheme, two_phase):
     pushes).  A stream is flagged BSW_E_OVERFLOW exactly when pad + peak > capacity, and every other stream -- each
     flagged one is followed by one that is not -- is bit-identical to the same run with ample capacity."""
     nimg = 2
-    cfg, m, sd, zend, zcen, bins, _ = _setup(name, 1)
+    cfg, m, sd, zend, zcen, bins, _ = setup(name, 1)
     imgs = synthetic.synthetic_images(cfg, nimg, seed=65)
     w0, head0 = synthetic.initial_words(800, seed=101)
     record = {}
-    orc = _oracle(cfg, m, sd, zend, zcen, record=record)
+    orc = gpu_oracle(cfg, m, sd, zend, zcen, record=record)
     st = O.CState(w0, head0)
     for xi in range(nimg):
         st = (orc.encode_image if scheme == BITSWAP else orc.encode_image_bbans)(st, imgs[xi])
@@ -453,7 +423,7 @@ def test_compress_images_retries_until_the_chains_fit():
     (four attempts).  With too little room for the first attempts the containers equal those of an ample run; with too
     little room for every attempt OverflowError is raised."""
     name = "tiny"
-    cfg, m, sd, zend, zcen, bins, codec = _setup(name, 3)
+    cfg, m, sd, zend, zcen, bins, codec = setup(name, 3)
     rs = np.random.RandomState(67)
     images = [rs.randint(0, 256, (h, w, 1)).astype(np.uint8) for h, w in [(64, 64), (32, 96), (32, 32)]]
     made = []

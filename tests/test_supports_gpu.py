@@ -14,16 +14,15 @@ import torch
 pytestmark = pytest.mark.gpu
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from coder_harness import (check_vs_oracle, coder_paths, dev, hostile_rows, initial_states, oracle_tables, pad_big,   # noqa: E402
+                           run_2p)
+from codec_harness import gpu_oracle, setup                            # noqa: E402
 from oracle import oracle as O                                         # noqa: E402
 from bitswap_b200 import synthetic                                     # noqa: E402
 from bitswap_b200.config import preset, with_                          # noqa: E402
 from bitswap_b200.codec import Bins, PipelinedCodec, BITSWAP, BBANS    # noqa: E402
 from bitswap_b200.streams import StreamSet                             # noqa: E402
 from bitswap_b200._lib import lib, check, cuda_stream_ptr              # noqa: E402
-from test_quantbits_gpu import (_rows, _states, _run_2p, _oracle_tables, _check_vs_oracle, _setup,   # noqa: E402
-                                _oracle_with, _pad_big)
-
-dev = "cuda"
 
 
 def _q_of(S):
@@ -40,10 +39,10 @@ def test_affine_supports_not_powers_of_two_vs_oracle(S, mode):
     bins -- must leave every stream and symbol bit-identical to the oracle.  mode -1 classifies the rows (uniform grids:
     the affine kernels), mode 1 forces the affine kernels; the generic kernels would refuse these supports."""
     B, L, q = 16, 77, _q_of(S)
-    ends, mu, sc, sym = _rows(L, S, q, B, seed=1000 + S)
-    states = _states(B, seed=40 + S)
-    res = _run_2p(ends, mu, sc, S, q, states, sym, mode)
-    _check_vs_oracle(res, _oracle_tables(ends, mu, sc, S, q), states, sym, range(B))
+    ends, mu, sc, sym = hostile_rows(L, S, q, B, seed=1000 + S)
+    states = initial_states(B, seed=40 + S)
+    res = run_2p(ends, mu, sc, S, q, states, sym, mode)
+    check_vs_oracle(res, oracle_tables(ends, mu, sc, S, q), states, sym, range(B))
 
 
 @pytest.mark.parametrize("S", [8, 16, 32, 64, 128, 256, 512, 1024])
@@ -62,45 +61,39 @@ def test_affine_verify_mode_at_every_power_of_two(S):
     mu[:, ::11] *= 3
     mu[:, 5::13] = np.float32(20.0)
     sym = rs.randint(0, S, size=(B, L)).astype(np.int16)
-    states = _states(B, seed=700 + S, n=6000)
-    check(lib().bsw_rows6_set_verify(1))
+    states = initial_states(B, seed=700 + S, n=6000)
     stats = np.zeros(4, dtype=np.uint64)
-    try:
-        got = _run_2p(ends, mu, sc, S, q, states, sym, mode=-1)
+    with coder_paths(verify=1):
+        got = run_2p(ends, mu, sc, S, q, states, sym, mode=-1)
         check(lib().bsw_rows6_verify_read(stats.ctypes.data))
-    finally:
-        check(lib().bsw_rows6_set_verify(0))
     mism, worst, checked, exact_path = (int(v) for v in stats)
     print(f"verify S={S}: {checked} bins evaluated of {2 * B * L * S}, {exact_path} exact path, worst trusted error "
           f"{worst / 10:.1f} % of the window, {mism} mismatches")
     assert checked > 0 and mism == 0
     assert worst <= 250, worst
     if S >= 32:
-        ref = _run_2p(ends, mu, sc, S, q, states, sym, mode=0)
+        ref = run_2p(ends, mu, sc, S, q, states, sym, mode=0)
         assert got[0] == ref[0] and np.array_equal(got[1], ref[1]) and got[2] == ref[2]
     else:
-        _check_vs_oracle(got, _oracle_tables(ends, mu, sc, S, q), states, sym, range(B))
+        check_vs_oracle(got, oracle_tables(ends, mu, sc, S, q), states, sym, range(B))
 
 
 # ---- refusals ------------------------------------------------------------------------------------------------------------
 def _abi_2p_rc(S, q, mode, B=2, L=4):
     ends = np.linspace(-6.0, 6.0, S + 1)[None, 1:-1].repeat(L, 0)
-    e_pad = torch.from_numpy(_pad_big(ends)).to(dev)
+    e_pad = torch.from_numpy(pad_big(ends)).to(dev)
     mu = torch.zeros((B, L), dtype=torch.float32, device=dev)
     sc = torch.ones((B, L), dtype=torch.float32, device=dev)
     sym = torch.zeros((B, L), dtype=torch.int16, device=dev)
     nbytes = int(lib().bsw_logistic_scratch_bytes(B, L, S, 0))
     scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     ss = StreamSet(B, 4096)
-    ss.import_lists(_states(B, seed=3))
-    check(lib().bsw_set_rows_mode(mode))
-    try:
+    ss.import_lists(initial_states(B, seed=3))
+    with coder_paths(rows_mode=mode):
         rcs = [fn(ss.handle, 0, B, mu.data_ptr(), L, sc.data_ptr(), L, e_pad.data_ptr(), S, sym.data_ptr(), L, S, 31, q,
                   scratch.data_ptr(), nbytes, cuda_stream_ptr()) for fn in (lib().bsw_logistic_pop_2p, lib().bsw_logistic_push_2p)]
-    finally:
-        check(lib().bsw_set_rows_mode(-1))
     torch.cuda.synchronize()
-    assert ss.export_lists() == _states(B, seed=3)                 # a refused call leaves the streams alone
+    assert ss.export_lists() == initial_states(B, seed=3)                 # a refused call leaves the streams alone
     return rcs
 
 
@@ -110,7 +103,7 @@ def _fused_rc(S, q, B=2, L=4):
     sc = torch.ones((B, L), dtype=torch.float32, device=dev)
     sym = torch.zeros((B, L), dtype=torch.int16, device=dev)
     ss = StreamSet(B, 4096)
-    ss.import_lists(_states(B, seed=3))
+    ss.import_lists(initial_states(B, seed=3))
     return [fn(ss.handle, 0, B, mu.data_ptr(), L, sc.data_ptr(), L, e_pad.data_ptr(), S, sym.data_ptr(), L, S, 31, q,
                cuda_stream_ptr()) for fn in (lib().bsw_logistic_pop, lib().bsw_logistic_push)]
 
@@ -156,9 +149,9 @@ def test_fused_coder_equals_two_phase_at_low_quantbits(name, scheme, q):
     """set_two_phase(False) codes every level with the fused one-warp-per-stream kernels (launch_fused<S/32>): the streams
     must be bit-identical to the two-phase coder's, and the fused decode must restore images and states."""
     B, nimg = 4, 2
-    cfg, m, sd, zend, zcen, bins, codec = _setup(name, q, B)
+    cfg, m, sd, zend, zcen, bins, codec = setup(name, B, q=q)
     imgs = synthetic.synthetic_images(cfg, B * nimg, seed=13).reshape(nimg, B, *cfg.xs)
-    states = _states(B, seed=200, n=4000)
+    states = initial_states(B, seed=200, n=4000)
     res = {}
     for two_phase in (True, False):
         codec.set_two_phase(two_phase)
@@ -188,7 +181,7 @@ def test_pipelined_codec_overlap_mode_q9_vs_oracle():
     pc = PipelinedCodec(cfg, sd, Bins(cfg, zend, zcen), B, lanes=2, use_tensor_cores=False)
     ss = StreamSet(B, 1 << 15)
     imgs = synthetic.synthetic_images(cfg, 2 * B, seed=29).reshape(2, B, *cfg.xs)
-    states = _states(B, seed=600, n=5000)
+    states = initial_states(B, seed=600, n=5000)
     res = []
     for mode in (1, 0):
         pc.set_dual_stream(mode)
@@ -200,7 +193,7 @@ def test_pipelined_codec_overlap_mode_q9_vs_oracle():
         res.append(ss.export_lists())
     assert res[0] == res[1]
     for b in range(B):
-        orc = _oracle_with(cfg, pc.models[b // pc.per], sd, zend, zcen)
+        orc = gpu_oracle(cfg, pc.models[b // pc.per], sd, zend, zcen, cls=O.BitSwapOracle)
         st = O.CState.from_list(states[b])
         for xi in range(2):
             st = orc.encode_image(st, imgs[xi, b])

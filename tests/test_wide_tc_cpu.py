@@ -14,9 +14,7 @@ import torch
 from bitswap_b200 import synthetic
 from bitswap_b200.config import CodecConfig
 from oracle import oracle as O
-from test_kernel_width_cpu import _golden, model_oracle_vs_golden
-
-WIDE_MODELS = ["wide_k3_w320", "wide_k7_w512"]
+from codec_harness import WIDE_MODELS, golden_model, model_oracle_vs_golden
 
 
 @pytest.mark.parametrize("W,ks", [(257, 3), (320, 5), (448, 1), (512, 7)])
@@ -38,7 +36,7 @@ def test_state_dict_spec_at_wide_widths(W, ks):
 def test_wide_model_oracle_matches_reference(name):
     """The oracle builds width-320 and width-512 models as the reference does: float32 within 2e-6 absolute of the golden
     outputs, float64 within 2e-5 relative to max(1, |output|)."""
-    cfg, _ = _golden(name)
+    cfg, _ = golden_model(name)
     sd = synthetic.synthetic_state_dict(cfg, seed=50, varied=True)
     for dtype, tol in ((torch.float32, lambda want: 2e-6), (torch.float64, lambda want: 2e-5 * np.maximum(1.0, np.abs(want)))):
         orc = O.ModelOracle(cfg, sd, dtype=dtype)

@@ -1,7 +1,7 @@
 """Models wider than 256 channels (reswidth 257..512, padded widths 320, 384, 448, 512) on the tensor cores and on SIMT.
 
-1. P3c per layer: every conv kind on its own against float64, with the harness of test_conv_f64_gpu (same inputs, value
-   sets, bars tau = 2^-13 / 2^-14 and exact checks) and the per-kernel-size bookkeeping of test_kernel_width_gpu, on
+1. P3c per layer: every conv kind on its own against float64, with the harness of conv_harness.py (same inputs, value
+   sets, bars tau = 2^-13 / 2^-14 and exact checks) and the per-kernel-size bookkeeping of test_kernel_width_gpu.py, on
    [2, MAXB, 256, Wp] plane buffers: widths 257..512 at kernel 3, kernels 1 / 5 / 7 at widths 320, 384 and 512 (7x7 at
    512 is the longest sum of any model), and the float32 SIMT path at widths 320 and 512.  Conv modes 8 / 15 must be
    bit-identical to 0 / 7.  The worst normalised error is reported per (path, conv kind, kernel size, padded width).
@@ -11,120 +11,66 @@
    edge-coded container.
 5. Widths above 512 are refused on the tensor cores with a message that names the supported range.
 """
-import os
-import sys
-
 import numpy as np
 import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-
-import test_conv_f64_gpu as F                                          # noqa: E402
-import test_kernel_width_gpu as KW                                     # noqa: E402
-from test_codec_gpu import _tc_case, TOL                               # noqa: E402
-from test_kernel_width_cpu import model_oracle_vs_golden, _golden      # noqa: E402
-from test_wide_tc_cpu import WIDE_MODELS                               # noqa: E402
+from codec_harness import TOL, WIDE_MODELS, golden_model, gpu_oracle, model_oracle_vs_golden, tc_case   # noqa: E402
+from conv_harness import VALUES, Case, conv_cfg, outputs_in_conv_modes, worst_report   # noqa: E402
 from oracle import oracle as O                                         # noqa: E402
 from bitswap_b200 import synthetic                                     # noqa: E402
 from bitswap_b200.model import Model                                   # noqa: E402
 from bitswap_b200.codec import Bins, PipelinedCodec, BITSWAP, BBANS    # noqa: E402
 from bitswap_b200.container import compress_images, decompress_images  # noqa: E402
 from bitswap_b200.streams import StreamSet                             # noqa: E402
-from bitswap_b200._lib import lib, check, BswError                     # noqa: E402
-
-_cfg = KW._cfg
+from bitswap_b200._lib import BswError                                 # noqa: E402
 
 # (tensor cores?, config).  zchannels <= 32 run the in-conv on the tensor cores, 40 the SIMT in-conv + split; heads of
 # <= 32 outputs run on the tensor cores, 40 and 80 on k_conv_simt after a wide tensor-core trunk.
 MODELS = {
     # padded widths 320 .. 512 at kernel 3
-    "tc k3 W257 zc1 C3": (True, _cfg(3, 1, 257, 3)),
-    "tc k3 W300 zc20 C1": (True, _cfg(1, 20, 300, 3)),
-    "tc k3 W320 zc40 C3 cond": (True, _cfg(3, 40, 320, 3, True)),
-    "tc k3 W384 zc2 C1 cond": (True, _cfg(1, 2, 384, 3, True)),
-    "tc k3 W400 zc16 C3": (True, _cfg(3, 16, 400, 3)),
-    "tc k3 W448 zc8 C1": (True, _cfg(1, 8, 448, 3)),
-    "tc k3 W500 zc32 C3": (True, _cfg(3, 32, 500, 3)),
-    "tc k3 W512 zc40 C1": (True, _cfg(1, 40, 512, 3)),
+    "tc k3 W257 zc1 C3": (True, conv_cfg(3, 1, 257, 3)),
+    "tc k3 W300 zc20 C1": (True, conv_cfg(1, 20, 300, 3)),
+    "tc k3 W320 zc40 C3 cond": (True, conv_cfg(3, 40, 320, 3, cond=True)),
+    "tc k3 W384 zc2 C1 cond": (True, conv_cfg(1, 2, 384, 3, cond=True)),
+    "tc k3 W400 zc16 C3": (True, conv_cfg(3, 16, 400, 3)),
+    "tc k3 W448 zc8 C1": (True, conv_cfg(1, 8, 448, 3)),
+    "tc k3 W500 zc32 C3": (True, conv_cfg(3, 32, 500, 3)),
+    "tc k3 W512 zc40 C1": (True, conv_cfg(1, 40, 512, 3)),
     # kernel sizes 1 / 5 / 7 at padded widths 320, 384, 512
-    "tc k1 W320 zc8 C3": (True, _cfg(3, 8, 320, 1)),
-    "tc k1 W384 zc40 C1 cond": (True, _cfg(1, 40, 384, 1, True)),
-    "tc k1 W512 zc2 C3": (True, _cfg(3, 2, 512, 1)),
-    "tc k5 W320 zc2 C1": (True, _cfg(1, 2, 320, 5)),
-    "tc k5 W384 zc20 C3 cond": (True, _cfg(3, 20, 384, 5, True)),
-    "tc k5 W512 zc8 C3": (True, _cfg(3, 8, 512, 5)),
-    "tc k7 W320 zc16 C3 cond": (True, _cfg(3, 16, 320, 7, True)),
-    "tc k7 W384 zc1 C1": (True, _cfg(1, 1, 384, 7)),
-    "tc k7 W512 zc2 C3 cond": (True, _cfg(3, 2, 512, 7, True)),
+    "tc k1 W320 zc8 C3": (True, conv_cfg(3, 8, 320, 1)),
+    "tc k1 W384 zc40 C1 cond": (True, conv_cfg(1, 40, 384, 1, cond=True)),
+    "tc k1 W512 zc2 C3": (True, conv_cfg(3, 2, 512, 1)),
+    "tc k5 W320 zc2 C1": (True, conv_cfg(1, 2, 320, 5)),
+    "tc k5 W384 zc20 C3 cond": (True, conv_cfg(3, 20, 384, 5, cond=True)),
+    "tc k5 W512 zc8 C3": (True, conv_cfg(3, 8, 512, 5)),
+    "tc k7 W320 zc16 C3 cond": (True, conv_cfg(3, 16, 320, 7, cond=True)),
+    "tc k7 W384 zc1 C1": (True, conv_cfg(1, 1, 384, 7)),
+    "tc k7 W512 zc2 C3 cond": (True, conv_cfg(3, 2, 512, 7, cond=True)),
     # the float32 SIMT path above 256 (dense convs too)
-    "simt k3 W320 zc8 C3": (False, _cfg(3, 8, 320, 3)),
-    "simt k3 W512 zc20 C1 cond": (False, _cfg(1, 20, 512, 3, True)),
-    "simt k7 W320 zc2 C1 cond": (False, _cfg(1, 2, 320, 7, True)),
-    "simt k7 W512 zc40 C3": (False, _cfg(3, 40, 512, 7)),
+    "simt k3 W320 zc8 C3": (False, conv_cfg(3, 8, 320, 3)),
+    "simt k3 W512 zc20 C1 cond": (False, conv_cfg(1, 20, 512, 3, cond=True)),
+    "simt k7 W320 zc2 C1 cond": (False, conv_cfg(1, 2, 320, 7, cond=True)),
+    "simt k7 W512 zc40 C3": (False, conv_cfg(3, 40, 512, 7)),
 }
-MINE = {}                                    # (path, kind, "k{ks} Wp{Wp}") -> worst normalised error
+MINE = {}                                    # ("k{ks} Wp{Wp}", path, kind) -> worst normalised error
+_report = worst_report("P3c wide models: worst |out - f(y)| / s (beyond the ELU/rounding allowance)", MINE)
 
 
-@pytest.fixture(scope="module", autouse=True)
-def _report(request):
-    yield
-    tr = request.config.pluginmanager.getplugin("terminalreporter")
-    capman = request.config.pluginmanager.getplugin("capturemanager")
-    if tr is None or capman is None or not MINE:
-        return
-    with capman.global_and_fixture_disabled():
-        tr.write_line("")
-        tr.write_line("P3c wide models: worst |out - f(y)| / s (beyond the ELU/rounding allowance)")
-        for (path, kind, tag), v in sorted(MINE.items(), key=lambda kv: (kv[0][2], kv[0][0], kv[0][1])):
-            tr.write_line(f"  {tag:10s} {path:4s} {kind:16s} {v:.3e}  "
-                          f"(2^{np.log2(v) if v > 0 else float('-inf'):.1f}, bar 2^{np.log2(F.TAU[path]):.0f})")
-
-
-class WideCase(KW.KwCase):
-    """KwCase on the wide models, with its own seeds and report table."""
-
-    def __init__(self, name, vs):
-        self.tc, self.cfg = MODELS[name]
-        self.name, self.vs = name, vs
-        self.seed = 12000 + 17 * list(MODELS).index(name) + F.VALUES.index(vs)
-        self.sd = F._state_dict(self.cfg, vs, self.seed)
-        self.m = Model.from_config(self.cfg, max_batch=F.MAXB, use_tensor_cores=self.tc).load_state_dict(self.sd)
-        self.W, self.Wp = self.cfg.reswidth, -(-self.cfg.reswidth // 64) * 64
-        self.planes = torch.empty((2, F.MAXB, 256, self.Wp), dtype=torch.int16, device="cuda")
-        self.modes = F.MODES if self.tc else (-1,)
-        self._outs = None
-
-    def run(self):
-        saved = dict(F.WORST)
-        F.WORST.clear()
-        try:
-            F.Case.run(self)
-        finally:
-            ks = self.cfg.kernel_size
-            for (path, kind), v in F.WORST.items():
-                if kind == "dense3":         # the kernel-size blocks (F.Case's "dense3" prefix gen_res1.0)
-                    kind = f"dense k{ks}"
-                key = (path, kind, f"k{ks} Wp{self.Wp}")
-                MINE[key] = max(MINE.get(key, 0.0), v)
-            F.WORST.clear()
-            F.WORST.update(saved)
-
-
-@pytest.mark.parametrize("vs", F.VALUES)
+@pytest.mark.parametrize("vs", VALUES)
 @pytest.mark.parametrize("name", list(MODELS))
 def test_wide_conv_kernels_vs_float64(name, vs):
-    WideCase(name, vs).run()
+    Case(MODELS, name, vs, seed_base=12000, worst=MINE, compare_modes=True, per_kernel_width=True).run()
 
 
 NETS = {
-    "k3 W320 nz2": _cfg(3, 8, 320, 3),
-    "k5 W384 nz3 cond": _cfg(3, 8, 384, 5, True, nz=3),
-    "k1 W448 nz2 zc20": _cfg(1, 20, 448, 1),
-    "k7 W512 nz2 zc40": _cfg(3, 40, 512, 7),
-    "k3 W257 nz2 cond": _cfg(3, 2, 257, 3, True),
+    "k3 W320 nz2": conv_cfg(3, 8, 320, 3),
+    "k5 W384 nz3 cond": conv_cfg(3, 8, 384, 5, True, nz=3),
+    "k1 W448 nz2 zc20": conv_cfg(1, 20, 448, 1),
+    "k7 W512 nz2 zc40": conv_cfg(3, 40, 512, 7),
+    "k3 W257 nz2 cond": conv_cfg(3, 2, 257, 3, True),
 }
 
 
@@ -132,7 +78,7 @@ NETS = {
 def test_wide_nets_vs_f64_oracle_and_simt(name):
     """Whole nets on the tensor cores: mu / sigma of every infer(i) / generate(i) within 1e-4 of the float64 oracle and
     of the SIMT path; a row alone equals the same row in the batch, bit for bit."""
-    worst_o, worst_s = _tc_case(NETS[name], 3, dtype=torch.float64)
+    worst_o, worst_s = tc_case(NETS[name], 3, dtype=torch.float64)
     print(f"tensor cores {name}: max |err| vs torch-f64 oracle {worst_o:.2e}, vs SIMT f32 path {worst_s:.2e}")
     assert worst_o < TOL and worst_s < TOL
 
@@ -141,28 +87,8 @@ def test_wide_nets_vs_f64_oracle_and_simt(name):
 def test_wide_persistent_grid_equals_per_tile_grid(name):
     """B = 170: 2040 (Wp 384) / 2720 (Wp 512) tiles per dense conv, many per CTA on the persistent grid; in-convs, dense
     convs with the per-tap fold, heads.  Bit-identical mu and sigma in modes 0, 7, 8 and 15."""
-    B = 170
-    cfg = {"k5 W384": _cfg(3, 8, 384, 5, nz=3), "k3 W512": _cfg(1, 2, 512, 3, True, nz=3)}[name]
-    sd = synthetic.synthetic_state_dict(cfg, seed=61, varied=True)
-    m = Model.from_config(cfg, max_batch=B, use_tensor_cores=True).load_state_dict(sd)
-    m.compress()
-    rs = np.random.RandomState(4)
-    gx = torch.from_numpy((rs.randint(0, 256, (B, cfg.xdim)) - 127.5) / 127.5).cuda()
-    gz = torch.from_numpy(rs.uniform(-5, 5, (B, cfg.zdim))).cuda()
-    out = {}
-    try:
-        for mode in (0, 7, 8, 15):
-            check(lib().bsw_set_conv_mode(mode))
-            res = []
-            for i in range(cfg.nz):
-                mu, sc = m.infer(i)(gx if i == 0 else gz)
-                res += [mu.clone(), sc.clone()]
-                mu, sc = m.generate(i)(gz)
-                res += [mu.clone(), sc.clone()]
-            torch.cuda.synchronize()
-            out[mode] = res
-    finally:
-        check(lib().bsw_set_conv_mode(-1))
+    cfg = {"k5 W384": conv_cfg(3, 8, 384, 5, nz=3), "k3 W512": conv_cfg(1, 2, 512, 3, True, nz=3)}[name]
+    out = outputs_in_conv_modes(cfg, 170, (0, 7, 8, 15))
     for mode in (7, 8, 15):
         for a, b in zip(out[0], out[mode]):
             assert torch.equal(a, b), f"conv mode {mode}"
@@ -173,7 +99,7 @@ def test_wide_persistent_grid_equals_per_tile_grid(name):
 @pytest.mark.parametrize("name", WIDE_MODELS)
 def test_wide_model_matches_reference(name, tc):
     """Model (tensor cores and SIMT) within 1e-4 of the reference Model's outputs at widths 320 and 512."""
-    cfg, _ = _golden(name)
+    cfg, _ = golden_model(name)
     sd = synthetic.synthetic_state_dict(cfg, seed=50, varied=True)
     m = Model.from_config(cfg, max_batch=1, use_tensor_cores=tc).load_state_dict(sd)
     m.compress()
@@ -182,7 +108,7 @@ def test_wide_model_matches_reference(name, tc):
     print(f"{name} {'tensor cores' if tc else 'SIMT'}: max |err| vs the reference {worst:.2e}")
 
 
-RECURSION = {"k5 W320": _cfg(3, 8, 320, 5), "k3 W512": _cfg(3, 8, 512, 3, nz=3)}
+RECURSION = {"k5 W320": conv_cfg(3, 8, 320, 5), "k3 W512": conv_cfg(3, 8, 512, 3, nz=3)}
 
 
 @pytest.mark.parametrize("scheme", [BITSWAP, BBANS], ids=["bitswap", "bbans"])
@@ -207,13 +133,7 @@ def test_wide_recursion_vs_oracle_and_roundtrip(name, scheme):
     ss.raise_on_error()
     got = ss.export_lists()
     m = pc.models[0]
-    orc = O.BitSwapOracle(cfg, O.ModelOracle(cfg, sd), zend, zcen, coder="c", pmf="cuda")
-
-    def gpu_net(kind, level, given):
-        f = m.infer(level) if kind == "infer" else m.generate(level)
-        mu, sc = f(given.cuda())
-        return mu.cpu(), sc.cpu()
-    orc._net = gpu_net
+    orc = gpu_oracle(cfg, m, sd, zend, zcen, cls=O.BitSwapOracle)
     enc = orc.encode_image if scheme == BITSWAP else orc.encode_image_bbans
     for b in sorted(set(int(v) for v in np.linspace(0, B - 1, nsample).round())):
         want = enc(O.CState(w, head), imgs[b]).to_list()
@@ -239,7 +159,7 @@ def test_wide_containers_edge_coded_roundtrip():
 
 
 def test_wide_width_above_512_is_refused_on_the_tensor_cores():
-    cfg = _cfg(3, 2, 513, 3)
+    cfg = conv_cfg(3, 2, 513, 3)
     sd = synthetic.synthetic_state_dict(cfg, seed=50, varied=False)
     with pytest.raises(BswError, match=r"reswidth 1\.\.512"):
         Model.from_config(cfg, max_batch=1, use_tensor_cores=True).load_state_dict(sd)
