@@ -129,6 +129,7 @@ def _set_argtypes(L):
         "bsw_model_load_conv": [P, ctypes.c_char_p, P, P, P, I, I, I, I],
         "bsw_model_load_gen_std": [P, P],
         "bsw_model_finalize": [P],
+        "bsw_model_set_tc_precision": [P, I],
         "bsw_vae_infer": [P, I, P, L64, P, P, P],
         "bsw_vae_generate": [P, I, P, L64, P, P, I, P],
         "bsw_codec_create": [PP, P, P, I],
@@ -162,7 +163,7 @@ EXPORTS = ["bsw_last_error", "bsw_version", "bsw_has_tensor_cores", "bsw_measure
            "bsw_logistic_pop_2p", "bsw_bins_create",
            "bsw_bins_destroy", "bsw_bins_device_ptrs", "bsw_gather_zcentres", "bsw_gather_xcentres",
            "bsw_model_create", "bsw_model_destroy", "bsw_model_load_conv", "bsw_model_load_gen_std",
-           "bsw_model_finalize", "bsw_vae_infer", "bsw_vae_generate", "bsw_codec_create", "bsw_codec_destroy",
+           "bsw_model_finalize", "bsw_model_set_tc_precision", "bsw_vae_infer", "bsw_vae_generate", "bsw_codec_create", "bsw_codec_destroy",
            "bsw_codec_encode", "bsw_codec_decode", "bsw_codec_encode_ext", "bsw_codec_decode_ext", "bsw_codec_last_launches", "bsw_codec_profile", "bsw_codec_set_two_phase", "bsw_codec_set_dual_stream",
            "bsw_discretize_reset", "bsw_discretize_sample", "bsw_discretize_fold", "bsw_discretize_edges"]
 

@@ -162,10 +162,11 @@ class PipelinedCodec:
     The coder's row-table kernel is FP64-pipe bound and the dense convs are tensor-pipe bound; chains of
     different sub-batches drift apart in phase, so their kernels share SMs and the two pipes overlap
     (4 lanes by default).  Results are identical to a single BitSwapCodec: every stream is independent and every kernel is
-    batch-invariant.  Each lane owns a model replica (activations are per-lane anyway)."""
+    batch-invariant.  Each lane owns a model replica (activations are per-lane anyway).  tc_precision: the arithmetic of
+    every lane's tensor-core convs ("split" or "bf16", see Model); it changes the bitstreams."""
 
     def __init__(self, cfg: CodecConfig, state_dict, bins: Bins, max_batch: int, lanes: int = 4, use_tensor_cores=True, lane_size: int = 0,
-                 free_running: bool = False):
+                 free_running: bool = False, tc_precision: str = "split"):
         self.cfg, self.bins, self.max_batch = cfg, bins, int(max_batch)
         self.device = bins.device
         self.lanes = max(1, min(int(lanes), self.max_batch))
@@ -182,7 +183,8 @@ class PipelinedCodec:
         # their own within a step.)
         self.free_running = bool(free_running)
         for _ in range(self.lanes):
-            m = Model.from_config(cfg, max_batch=self.per, use_tensor_cores=use_tensor_cores, device=self.device).load_state_dict(state_dict)
+            m = Model.from_config(cfg, max_batch=self.per, use_tensor_cores=use_tensor_cores, device=self.device,
+                                  tc_precision=tc_precision).load_state_dict(state_dict)
             m.compress()
             self.models.append(m)
             self.codecs.append(BitSwapCodec(cfg, m, bins, self.per))

@@ -41,9 +41,15 @@
 //     every shift; a 1x1 in-conv tile is a single k-block.
 //   * fixed k order, no split-K, no atomics: results are bit-identical for any batch size, position in the batch
 //     or grid (the decoder must regenerate the encoder's tables exactly, SURVEY.md H3).
+//   * single-pass bf16 arithmetic (BSW_TC_BF16, Bf16<Args>): one hi*hi MMA per k16 step into the main accumulator, no
+//     cross accumulator, only the hi boxes loaded (the stage layout stays the split tile's, its lo halves unused), and only
+//     the hi plane of the next conv's input written.  The hi planes are RNE(x) in both arithmetics, so the two share the
+//     weights, planes and tensor maps.  Four-CTA clusters issue one box per CTA: A_hi of pixel half h by the CTA of
+//     channel block h, W_hi of channel block b by the CTA of pixel half 1 - b.  Folding tiles still fold per tap.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdlib.h>
+#include <type_traits>
 #include <vector>
 #include "bsw_common.cuh"
 #include "nets.cuh"
@@ -257,6 +263,7 @@ __device__ __forceinline__ uint32_t pack_bf16x2(__nv_bfloat16 a, __nv_bfloat16 b
 template <int WP> struct DenseArgs {
     static constexpr int kN = (WP == 128 || WP == 256) ? BN : NW, kCoBlocks = WP / kN;
     static constexpr bool kFold = WP > 256;
+    static constexpr bool kBf16 = false;
     int taps, ks;
     int cchunks;             // 32-channel chunks per tap: WP / 32 for the dense W->W convs, 1 for the in-convs
     const float *bias;       // [WP]
@@ -275,8 +282,8 @@ template <int WP> struct DenseArgs {
 template <int N> __device__ __forceinline__ int hand_idx(int r, int c) { return r * N + (((c >> 3) ^ (r & 3)) << 3) + (c & 7); }
 
 // Folding tiles: s = (outer + main) + cross, in that order for every element, so the result does not depend on the grid.
-// The other tiles pass a one-element `outer` that is never read.
-template <int WP, int O>
+// The other tiles pass a one-element `outer` that is never read.  BF16: s = outer + main or main (`dc` is never read).
+template <bool BF16, int WP, int O>
 __device__ __forceinline__ void hand_store(const DenseArgs<WP> &, float *hand, const float (&outer)[O],
                                            const float (&dm)[DenseArgs<WP>::kN / 2], const float (&dc)[DenseArgs<WP>::kN / 2],
                                            int row, int lane) {
@@ -287,7 +294,9 @@ __device__ __forceinline__ void hand_store(const DenseArgs<WP> &, float *hand, c
         for (int h = 0; h < 2; ++h) {
             const int i = 4 * j + 2 * h;
             float2 s;
-            if constexpr (DenseArgs<WP>::kFold) s = make_float2((outer[i] + dm[i]) + dc[i], (outer[i + 1] + dm[i + 1]) + dc[i + 1]);
+            if constexpr (BF16 && DenseArgs<WP>::kFold) s = make_float2(outer[i] + dm[i], outer[i + 1] + dm[i + 1]);
+            else if constexpr (BF16) s = make_float2(dm[i], dm[i + 1]);
+            else if constexpr (DenseArgs<WP>::kFold) s = make_float2((outer[i] + dm[i]) + dc[i], (outer[i + 1] + dm[i + 1]) + dc[i + 1]);
             else s = make_float2(dm[i] + dc[i], dm[i + 1] + dc[i + 1]);
             *reinterpret_cast<float2 *>(hand + hand_idx<N>(row + 8 * h, 8 * j + 2 * (lane & 3))) = s;
         }
@@ -299,8 +308,8 @@ __device__ __forceinline__ void hand_store(const DenseArgs<WP> &, float *hand, c
 // (N = 128: 128 channels of one row per step; N = 64: two 64-channel rows), at channel block co0.  Warp ew takes row
 // steps ew, ew + 3, ..., so a warp stores 512 contiguous bytes of the trunk and 256 of each plane per step.  The
 // residual is the trunk itself (updated in place: resid == T): each element is read and then written by the same
-// thread, and the loads of the next RD steps are issued before the current step's stores.
-template <int WP>
+// thread, and the loads of the next RD steps are issued before the current step's stores.  BF16: the hi plane only.
+template <bool BF16, int WP>
 __device__ __forceinline__ void epilogue(const DenseArgs<WP> &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
     constexpr int N = DenseArgs<WP>::kN, ROWS = 128 / N;
     constexpr int RD = 3, LPR = 32 / ROWS;
@@ -330,7 +339,14 @@ __device__ __forceinline__ void epilogue(const DenseArgs<WP> &a, const float *ha
                 for (int e = 0; e < 4; ++e) x[e] = elu1(x[e]);
             const int64_t off = base + ROWS * rs * WP;
             if (a.T) *reinterpret_cast<float4 *>(a.T + off) = make_float4(x[0], x[1], x[2], x[3]);
-            if (a.A_hi) {
+            if constexpr (BF16) {
+                if (a.A_hi) {
+                    __nv_bfloat16 hi[4];
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) hi[e] = __float2bfloat16_rn(a.A_elu ? elu1(x[e]) : x[e]);
+                    *reinterpret_cast<uint2 *>(a.A_hi + off) = make_uint2(pack_bf16x2(hi[0], hi[1]), pack_bf16x2(hi[2], hi[3]));
+                }
+            } else if (a.A_hi) {
                 __nv_bfloat16 hi[4], lo[4];
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
@@ -351,6 +367,7 @@ __device__ __forceinline__ void epilogue(const DenseArgs<WP> &a, const float *ha
 template <bool FOLD> struct HeadArgs {
     static constexpr int kN = HD_N, kCoBlocks = 1;
     static constexpr bool kFold = FOLD;
+    static constexpr bool kBf16 = false;
     int taps, ks;
     int cchunks;             // Wp / 32: K = taps x Wp
     const float *bias;       // [>= n_mu + n_sc]
@@ -371,8 +388,8 @@ __device__ __forceinline__ float hd_scale(float r, int kind) {      // same expr
 
 // Heads' hand-off tile: channel-major [32 ch][HD_LD], so the epilogue's lanes read consecutive pixels of one channel; the
 // row stride of 132 floats also spreads the consumers' writes (8 rows x 4 channels per register) over 32 banks.  The sum
-// is the dense tiles': (outer + main) + cross when folding, main + cross otherwise.
-template <bool FOLD, int O>
+// is the dense tiles': (outer + main) + cross when folding, main + cross otherwise (BF16: without the cross term).
+template <bool BF16, bool FOLD, int O>
 __device__ __forceinline__ void hand_store(const HeadArgs<FOLD> &, float *hand, const float (&outer)[O], const float (&dm)[HD_N / 2],
                                            const float (&dc)[HD_N / 2], int row, int lane) {
 #pragma unroll
@@ -383,14 +400,16 @@ __device__ __forceinline__ void hand_store(const HeadArgs<FOLD> &, float *hand, 
             for (int e = 0; e < 2; ++e) {
                 const int i = 4 * j + 2 * h + e;
                 float s;
-                if constexpr (FOLD) s = (outer[i] + dm[i]) + dc[i];
+                if constexpr (BF16 && FOLD) s = outer[i] + dm[i];
+                else if constexpr (BF16) s = dm[i];
+                else if constexpr (FOLD) s = (outer[i] + dm[i]) + dc[i];
                 else s = dm[i] + dc[i];
                 hand[(8 * j + 2 * (lane & 3) + e) * HD_LD + row + 8 * h] = s;
             }
 }
 
-// Heads' epilogue: lane = pixel, so the flat CHW stores dst[o * 256 + p] of a warp are coalesced.
-template <bool FOLD>
+// Heads' epilogue: lane = pixel, so the flat CHW stores dst[o * 256 + p] of a warp are coalesced.  Both arithmetics.
+template <bool BF16, bool FOLD>
 __device__ __forceinline__ void epilogue(const HeadArgs<FOLD> &a, const float *hand, int img, int mh, int co0, int ew, int lane) {
     float *mu_row = a.mu + (int64_t)img * a.out_dim;
     float *sc_row = a.scale ? a.scale + (int64_t)img * a.out_dim : nullptr;
@@ -408,6 +427,11 @@ __device__ __forceinline__ void epilogue(const HeadArgs<FOLD> &a, const float *h
     }
 }
 
+// The tile of Args in single-pass bf16 arithmetic (BSW_TC_BF16): same arguments, shared memory and launch shape.
+template <class Args> struct Bf16 : Args {
+    static constexpr bool kBf16 = true;
+};
+
 // Tile t -> image t / (2 * kCoBlocks), output-channel block, pixel half (t & 1): the tiles of one image run on
 // neighbouring SMs at about the same time, so the activation planes they share come out of L2.
 // Launched as four-CTA clusters (DenseArgs<256> only, see the file comment), gridDim.x is a multiple of 4: t & 3 is the
@@ -419,147 +443,19 @@ template <class Args>
 __global__ void __maxnreg__(128)
 k_conv_wg(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ CUtensorMap amap_lo,
           const __grid_constant__ CUtensorMap wmap_hi, const __grid_constant__ CUtensorMap wmap_lo, const Args a, int ntiles) {
-    constexpr int N = Args::kN;
-    using C = TileCfg<N>;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    float *hand = (float *)(smem + C::NSTAGE * C::STAGE);
-    uint64_t *full_bar = (uint64_t *)(smem + C::NSTAGE * C::STAGE + C::HAND);
-    uint64_t *empty_bar = full_bar + C::NSTAGE;
-    uint64_t *acc_full = empty_bar + C::NSTAGE, *acc_empty = acc_full + 1;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int nkb = a.taps * a.cchunks;
-    const bool mc = Args::kCoBlocks == 2 && cluster_nctarank() == 4;
-    const uint32_t rank = mc ? cluster_ctarank() : 0;
-
-    if (warp == PRODUCER_WARP && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&amap_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&amap_lo) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap_lo) : "memory");
-        // empty: both consumer warpgroups of this CTA and, with multicast, of the two peers that write into its stages
-        for (int s = 0; s < C::NSTAGE; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], mc ? 6 : 2); }
-        mbar_init(acc_full, 256);
-        mbar_init(acc_empty, EPI_WARPS * 32);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    // peers arrive on these barriers and multicast into this CTA's stages: all barriers of the cluster are initialised first
-    if (mc) cluster_sync();
-    else __syncthreads();
-
-    if (warp >= PRODUCER_WARP) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS_EPILOGUE));
-        if (warp >= EPI_WARP0) {     // ===== epilogue warps =====
-            int it = 0;
-            for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++it) {
-                const int img = t / (2 * Args::kCoBlocks), co0 = ((t >> 1) % Args::kCoBlocks) * N, mh = t & 1;
-                mbar_wait(acc_full, it & 1);
-                epilogue(a, hand, img, mh, co0, warp - EPI_WARP0, lane);
-                mbar_arrive(acc_empty);
-            }
-        } else if (lane == 0) {     // ===== TMA producer =====
-            const int r = a.ks / 2;
-            const uint16_t amask = (uint16_t)(0x5u << (rank & 1)), wmask = (uint16_t)(0x3u << (rank & 2));
-            int stage = 0, phase = 0;
-            for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
-                const int img = t / (2 * Args::kCoBlocks), co0 = ((t >> 1) % Args::kCoBlocks) * N, mh = t & 1;
-                for (int kb = 0; kb < nkb; ++kb) {
-                    const int tap = kb / a.cchunks, c0 = (kb - tap * a.cchunks) * BK;
-                    const int dy = tap / a.ks, dx = tap - dy * a.ks;
-                    mbar_wait(&empty_bar[stage], phase ^ 1);
-                    uint8_t *st = smem + stage * C::STAGE;
-                    mbar_expect_tx(&full_bar[stage], C::STAGE);       // whole stage: the peers' boxes complete here too
-                    if (mc) {
-                        // A_hi by channel block 0, A_lo by block 1 of this pixel half; W_hi by pixel half 0, W_lo by half 1
-                        const int ao = (rank & 2) ? A_BYTES : 0, wo = (rank & 1) ? C::W_BYTES : 0;
-                        tma_load_4d_mc(st + ao, (rank & 2) ? &amap_lo : &amap_hi, &full_bar[stage], amask, c0, dx - r,
-                                       dy - r + 8 * mh, img);
-                        tma_load_3d_mc(st + 2 * A_BYTES + wo, (rank & 1) ? &wmap_lo : &wmap_hi, &full_bar[stage], wmask, c0,
-                                       co0, tap);
-                    } else {
-                        tma_load_4d(st, &amap_hi, &full_bar[stage], c0, dx - r, dy - r + 8 * mh, img);
-                        tma_load_4d(st + A_BYTES, &amap_lo, &full_bar[stage], c0, dx - r, dy - r + 8 * mh, img);
-                        tma_load_3d(st + 2 * A_BYTES, &wmap_hi, &full_bar[stage], c0, co0, tap);
-                        tma_load_3d(st + 2 * A_BYTES + C::W_BYTES, &wmap_lo, &full_bar[stage], c0, co0, tap);
-                    }
-                    if (++stage == C::NSTAGE) { stage = 0; phase ^= 1; }
-                }
-            }
-            // Drain: wait for the last release of every stage.  With multicast, peers arrive on this CTA's barriers
-            // until then, so the CTA must not exit before (a stage never filled passes at once: parity phase ^ 1).
-            for (int s = 0; s < C::NSTAGE; ++s) {
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                if (++stage == C::NSTAGE) { stage = 0; phase ^= 1; }
-            }
-        }
-        return;
-    }
-
-    // ===== consumers: warpgroup wg owns tile rows [64 wg, 64 wg + 64) =====
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS_CONSUMER));
-    const int wg = warp >> 2;
-    const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);          // this thread's first accumulator row
-    // one thread per warpgroup releases a stage: to this CTA's producer and, with multicast, to the two peers writing into it
-    auto release = [&](int s) {
-        if ((threadIdx.x & 127) != 0) return;
-        if (mc) { mbar_arrive_cluster(&empty_bar[s], rank); mbar_arrive_cluster(&empty_bar[s], rank ^ 1); mbar_arrive_cluster(&empty_bar[s], rank ^ 2); }
-        else mbar_arrive(&empty_bar[s]);
-    };
-    // Folding tiles (Args::kFold): after the last k-block of every tap but the last, the consumers retire the MMAs in
-    // flight, add the main accumulator into `outer` (float32 RNE adds) and restart it from zero, so the tensor core's
-    // truncating accumulate never sums more than one tap's Wp terms into it.  In-convs (one k-block per tap) do not fold.
-    constexpr bool fold = Args::kFold;
-    const bool fold_taps = fold && a.cchunks > 1;
-    int stage = 0, phase = 0, it = 0;
-    for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++it) {
-        float dm[N / 2], dc[N / 2], outer[fold ? N / 2 : 1];
-#pragma unroll
-        for (int i = 0; i < N / 2; ++i) { dm[i] = 0.f; dc[i] = 0.f; }
-        if constexpr (fold) {
-#pragma unroll
-            for (int i = 0; i < N / 2; ++i) outer[i] = 0.f;
-        }
-        int prev = -1, kc = 0;
-        for (int kb = 0; kb < nkb; ++kb) {
-            mbar_wait(&full_bar[stage], phase);
-            const uint32_t sbase = smem_u32(smem + stage * C::STAGE);
-            wg_fence();
-#pragma unroll
-            for (int kk = 0; kk < BK / 16; ++kk) {
-                const uint64_t a_hi = make_desc_sw64(sbase + wg * (64 * BK * 2) + kk * 32);
-                const uint64_t a_lo = make_desc_sw64(sbase + A_BYTES + wg * (64 * BK * 2) + kk * 32);
-                const uint64_t b_hi = make_desc_sw64(sbase + 2 * A_BYTES + kk * 32);
-                const uint64_t b_lo = make_desc_sw64(sbase + 2 * A_BYTES + C::W_BYTES + kk * 32);
-                Wgmma<N>::mma(dm, a_hi, b_hi);
-                Wgmma<N>::mma(dc, a_lo, b_hi);
-                Wgmma<N>::mma(dc, a_hi, b_lo);
-            }
-            wg_commit();
-            if (fold_taps && ++kc == a.cchunks && kb + 1 < nkb) {
-                kc = 0;
-                wg_wait<0>();                              // this tap's MMAs are done: both stages can go
-                fence_regs(dm);
-#pragma unroll
-                for (int i = 0; i < N / 2; ++i) { outer[i] += dm[i]; dm[i] = 0.f; }
-                if (prev >= 0) release(prev);
-                release(stage);
-                prev = -1;
-            } else {
-                wg_wait<1>();                              // the previous k-block's MMAs have read their stage
-                if (prev >= 0) release(prev);
-                prev = stage;
-            }
-            if (++stage == C::NSTAGE) { stage = 0; phase ^= 1; }
-        }
-        wg_wait<0>();
-        fence_regs(dm);
-        fence_regs(dc);
-        if (prev >= 0) release(prev);
-        mbar_wait(acc_empty, (it & 1) ^ 1);            // the epilogue has read the previous tile
-        hand_store(a, hand, outer, dm, dc, row0, lane);
-        mbar_arrive(acc_full);
-    }
+#include "conv_wg_body.cuh"
+}
+// The same tile in single-pass bf16 arithmetic (Args = Bf16<DenseArgs<WP>> or Bf16<HeadArgs<FOLD>>), a kernel of its own name.
+template <class Args>
+__global__ void __maxnreg__(128)
+k_conv_bf16(const __grid_constant__ CUtensorMap amap_hi, const __grid_constant__ CUtensorMap amap_lo,
+            const __grid_constant__ CUtensorMap wmap_hi, const __grid_constant__ CUtensorMap wmap_lo, const Args a, int ntiles) {
+#include "conv_wg_body.cuh"
+}
+// The kernel of tile type Args.
+template <class Args> auto conv_kernel() {
+    if constexpr (Args::kBf16) return k_conv_bf16<Args>;
+    else return k_conv_wg<Args>;
 }
 
 // float32 NHWC -> bf16 hi/lo planes (used once per net, after the SIMT in-conv)
@@ -638,6 +534,13 @@ template <class F> int with_width(int Wp, F &&f) {
     BSW_REQUIRE(false, "tensor-core conv path needs a padded width of 64, 128, ..., 512 (reswidth 1..512)");
 }
 
+// Calls f(Args{}) with the dense tile of the model's padded width in the model's arithmetic: DenseArgs<Wp>, or
+// Bf16<DenseArgs<Wp>> when bsw_model_set_tc_precision chose BSW_TC_BF16.  The heads take HeadT<Args>.
+template <class F> int with_tile(const bsw_model *m, F &&f) {
+    return with_width(m->Wp, [&](auto t) { return m->tc_precision == BSW_TC_BF16 ? f(Bf16<decltype(t)>{}) : f(t); });
+}
+template <class Args> using HeadT = std::conditional_t<Args::kBf16, Bf16<HeadArgs<Args::kFold>>, HeadArgs<Args::kFold>>;
+
 }  // namespace
 
 struct TcSlot { CUtensorMap map_hi, map_lo; };
@@ -655,6 +558,11 @@ int bsw_model_tc_prepare(bsw_model *m) {
             BSW_CUDA(cudaFuncSetAttribute(k_conv_wg<Head>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<HD_N>::SMEM));
             bsw_prefer_max_shared(k_conv_wg<Args>);
             bsw_prefer_max_shared(k_conv_wg<Head>);
+            // the bf16 tiles: same shared memory (bsw_model_set_tc_precision may switch at any net call)
+            BSW_CUDA(cudaFuncSetAttribute(k_conv_bf16<Bf16<Args>>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<Args::kN>::SMEM));
+            BSW_CUDA(cudaFuncSetAttribute(k_conv_bf16<Bf16<Head>>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileCfg<HD_N>::SMEM));
+            bsw_prefer_max_shared(k_conv_bf16<Bf16<Args>>);
+            bsw_prefer_max_shared(k_conv_bf16<Bf16<Head>>);
             return BSW_OK;
         }))
         return rc;
@@ -790,7 +698,8 @@ static unsigned tc_grid(int ntiles, bool persistent) {   // one CTA per tile, or
     return (unsigned)(ntiles < sms[dev] ? ntiles : sms[dev]);
 }
 
-// One dense conv or in-conv on the tile of the model's padded width, reading the planes behind amap_hi / amap_lo;
+// One dense conv or in-conv on the tile of the model's padded width and arithmetic, reading the planes behind amap_hi /
+// amap_lo (bf16: amap_hi only);
 // cchunks = 32-channel chunks per tap of those planes.  The tile with two channel blocks (padded width 256) runs one
 // four-CTA cluster per image (TMA multicast, see k_conv_wg), or single CTAs with mode bit 8; its persistent grid is as
 // many clusters as the device holds at once (GPCs of 16-18 SMs leave some SMs out), cluster c walking images c, c + C,
@@ -799,12 +708,12 @@ static int launch_dense(bsw_model *m, const CUtensorMap &amap_hi, const CUtensor
                         const ConvSlot &c, const ConvArgs &a, const float *resid, int cchunks, int64_t n, bool persistent,
                         cudaStream_t st) {
     TcState *ts = (TcState *)m->tc_state;
-    return with_width(m->Wp, [&](auto t) {
+    return with_tile(m, [&](auto t) {
         using Args = decltype(t);
         t.taps = c.ks * c.ks; t.ks = c.ks; t.cchunks = cchunks;
         t.bias = c.bias; t.resid = resid; t.T = a.T; t.T_elu = a.T_elu;
         t.A_hi = a.A_planes >= 0 ? ts->act[a.A_planes][0] : nullptr;
-        t.A_lo = a.A_planes >= 0 ? ts->act[a.A_planes][1] : nullptr;
+        t.A_lo = a.A_planes >= 0 && !Args::kBf16 ? ts->act[a.A_planes][1] : nullptr;
         t.A_elu = a.A_elu;
         const int ntiles = (int)n * 2 * Args::kCoBlocks;
         if constexpr (Args::kCoBlocks == 2) {
@@ -825,16 +734,16 @@ static int launch_dense(bsw_model *m, const CUtensorMap &amap_hi, const CUtensor
                 const int dev = cur_device();
                 if (!clusters[dev]) {
                     int v = 0;
-                    BSW_CUDA(cudaOccupancyMaxActiveClusters(&v, k_conv_wg<Args>, &cfg));
+                    BSW_CUDA(cudaOccupancyMaxActiveClusters(&v, conv_kernel<Args>(), &cfg));
                     BSW_REQUIRE(v > 0, "launch_dense: a cluster of four conv CTAs does not fit this device");
                     clusters[dev] = v;
                 }
                 cfg.gridDim = dim3(4u * (unsigned)(n < clusters[dev] ? n : clusters[dev]));
             }
-            BSW_CUDA(cudaLaunchKernelEx(&cfg, k_conv_wg<Args>, amap_hi, amap_lo, s.map_hi, s.map_lo, t, ntiles));
+            BSW_CUDA(cudaLaunchKernelEx(&cfg, conv_kernel<Args>(), amap_hi, amap_lo, s.map_hi, s.map_lo, t, ntiles));
         } else {
-            k_conv_wg<Args><<<tc_grid(ntiles, persistent), WG_THREADS, TileCfg<Args::kN>::SMEM, st>>>(amap_hi, amap_lo, s.map_hi,
-                                                                                                      s.map_lo, t, ntiles);
+            conv_kernel<Args>()<<<tc_grid(ntiles, persistent), WG_THREADS, TileCfg<Args::kN>::SMEM, st>>>(amap_hi, amap_lo, s.map_hi,
+                                                                                                          s.map_lo, t, ntiles);
             BSW_LAUNCH_CHECK();
         }
         return BSW_OK;
@@ -862,12 +771,12 @@ int bsw_conv_tc_head(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t
     const TcSlot &s = (*(std::vector<TcSlot> *)m->tc_slots)[c.tc_index];
     const int ntiles = (int)n * 2;
     const unsigned grid = tc_grid(ntiles, tc_persistent(4));
-    return with_width(m->Wp, [&](auto t) {
-        using Head = HeadArgs<decltype(t)::kFold>;      // the heads fold where the model's dense convs do
+    return with_tile(m, [&](auto t) {
+        using Head = HeadT<decltype(t)>;                 // the heads fold where the model's dense convs do
         Head h;
         h.taps = c.ks * c.ks; h.ks = c.ks; h.cchunks = m->Wp / BK; h.bias = c.bias; h.mu = a.mu; h.scale = a.scale; h.n_mu = a.n_mu; h.n_sc = a.n_sc;
         h.scale_kind = a.scale_kind; h.out_mode = a.out_mode; h.out_dim = a.out_dim;
-        k_conv_wg<Head><<<grid, WG_THREADS, TileCfg<HD_N>::SMEM, st>>>(ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1],
+        conv_kernel<Head>()<<<grid, WG_THREADS, TileCfg<HD_N>::SMEM, st>>>(ts->act_map[a.in_planes][0], ts->act_map[a.in_planes][1],
                                                                         s.map_hi, s.map_lo, h, ntiles);
         BSW_LAUNCH_CHECK();
         return BSW_OK;

@@ -425,6 +425,15 @@ extern "C" int bsw_model_finalize(bsw_model *m) {
     return BSW_OK;
 }
 
+extern "C" int bsw_model_set_tc_precision(bsw_model *m, int precision) {
+    BSW_REQUIRE(m, "null model");
+    BSW_REQUIRE(precision == BSW_TC_SPLIT || precision == BSW_TC_BF16,
+                "bsw_model_set_tc_precision: BSW_TC_SPLIT (0) or BSW_TC_BF16 (1)");
+    BSW_REQUIRE(m->d.use_tensor_cores, "bsw_model_set_tc_precision: a model without tensor cores has no tensor-core arithmetic");
+    m->tc_precision = precision;        // read by every tensor-core launch; every net call writes the planes it reads
+    return BSW_OK;
+}
+
 // ------------------------------------------------------------------------------------------------
 // Running a net.  Value flow (h = trunk, all float32):
 //   in-conv:            h = ELU(conv(given))                                   cifar_train.py:89-102 (Sequential(..., act))

@@ -56,6 +56,7 @@ struct bsw_model {
     float *xscale;                   // [xdim] unconditional x-scale
     bool have_gen_std, finalized;
     bool tc_ready = false;
+    int tc_precision = BSW_TC_SPLIT; // arithmetic of the tensor-core convs (bsw_model_set_tc_precision)
     void *tc_state = nullptr;        // owned by conv_tc.cu
     void *tc_slots = nullptr;
 };

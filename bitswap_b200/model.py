@@ -24,12 +24,28 @@ class _Desc(ctypes.Structure):
                                               "reswidth", "cond_xscale", "max_batch", "use_tensor_cores")]
 
 
+# Arithmetic of the tensor-core convs (BSW_TC_SPLIT / BSW_TC_BF16 of include/bitswap_b200.h)
+TC_PRECISIONS = {"split": 0, "bf16": 1}
+
+
 class Model:
+    """tc_precision (tensor-core models only): "split" (default) runs every multiply-add as three bf16 MMAs on hi/lo
+    operand planes, mu/sigma within 1e-4 of the float32 reference model; "bf16" runs one MMA on the RNE-rounded bf16
+    operands, faster, mu/sigma a few 1e-3 off.  The two arithmetics give different bitstreams: a stream decodes only with
+    a model of the arithmetic that encoded it."""
+
     def __init__(self, xs=(3, 32, 32), nz=1, zchannels=16, nprocessing=1, kernel_size=3, resdepth=2, reswidth=256,
-                 dropout_p=0., tag='', root_process=True, cond_xscale=False, max_batch=1, use_tensor_cores=False, device=None):
+                 dropout_p=0., tag='', root_process=True, cond_xscale=False, max_batch=1, use_tensor_cores=False, device=None,
+                 tc_precision="split"):
         # the config validates the architecture (kernel_size: ValueError) before any device work
         self.cfg = CodecConfig(xs=tuple(xs), nz=nz, zchannels=zchannels, nprocessing=nprocessing, kernel_size=kernel_size,
                                resdepth=resdepth, reswidth=reswidth, cond_xscale=cond_xscale)
+        if tc_precision not in TC_PRECISIONS:
+            raise ValueError(f"tc_precision must be one of {sorted(TC_PRECISIONS)}, got {tc_precision!r}")
+        if tc_precision != "split" and not use_tensor_cores:
+            raise ValueError(f"tc_precision={tc_precision!r} needs use_tensor_cores=True: the float32 SIMT path has one "
+                             "arithmetic")
+        self._tc_precision = tc_precision
         if not torch.cuda.is_available():
             raise RuntimeError("bitswap_b200.Model needs a CUDA device (no CPU fallback)")
         assert tuple(xs[1:]) == (32, 32), "blocks are always 32x32 (latents 16x16)"
@@ -48,6 +64,8 @@ class Model:
         self._destroy()
         with on_device(self.device):
             check(lib().bsw_model_create(ctypes.byref(self._h), ctypes.byref(self._desc)))
+            if self._desc.use_tensor_cores:
+                check(lib().bsw_model_set_tc_precision(self._h, TC_PRECISIONS[self._tc_precision]))
         self._loaded = False
 
     def _destroy(self):
@@ -71,6 +89,11 @@ class Model:
     @property
     def handle(self):
         return self._h
+
+    @property
+    def tc_precision(self):
+        """"split" or "bf16": the arithmetic of the tensor-core convs (fixed at construction)."""
+        return self._tc_precision
 
     # -- nn.Module-shaped no-ops the compression scripts call ---------------------------------------
     def to(self, device=None, *a, **k):

@@ -298,6 +298,18 @@ int bsw_model_load_conv(bsw_model *m, const char *prefix, const float *v_host, c
 int bsw_model_load_gen_std(bsw_model *m, const float *gen_std_host);
 /* Call after all tensors are loaded; checks completeness. */
 int bsw_model_finalize(bsw_model *m);
+/* Arithmetic of a tensor-core model's tensor-core convs, from the next net call on:
+ *   BSW_TC_SPLIT (default): every operand split into bf16 hi + lo planes, three MMAs per multiply-add (hi*hi, lo*hi,
+ *     hi*lo); mu/sigma within 1e-4 of the float32 reference model.
+ *   BSW_TC_BF16: one MMA per multiply-add on the RNE-rounded bf16 operands (float32 accumulate, float32 trunk and
+ *     residual stream); faster, mu/sigma a few 1e-3 off the reference.
+ * The two give different mu/sigma, so a bitstream decodes only with a model in the arithmetic it was encoded in (as with
+ * SIMT against tensor cores).  Convs a tensor-core model runs on the float32 SIMT kernel (in-convs with more than 32
+ * input channels, heads with more than 32 outputs) stay float32 in both.  BSW_E_INVALID for any other value and for a
+ * model created with use_tensor_cores = 0. */
+#define BSW_TC_SPLIT 0
+#define BSW_TC_BF16  1
+int bsw_model_set_tc_precision(bsw_model *m, int precision);
 
 /* given_dev float32 [n, dim_in] flat CHW (what `given.float()` is in the reference);
  * mu_dev/scale_dev float32 [n, dim_out] flat CHW.  For generate(0) without cond_xscale the scale does
