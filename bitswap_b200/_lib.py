@@ -119,6 +119,9 @@ def _set_argtypes(L):
         "bsw_rows6_verify_read": [P],
         "bsw_logistic_push_2p": [P, I, I, P, L64, P, L64, P, L64, P, L64, I, I, I, P, L64, P],
         "bsw_logistic_pop_2p": [P, I, I, P, L64, P, L64, P, L64, P, L64, I, I, I, P, L64, P],
+        "bsw_direct_push": [P, I, I, P, L64, P, L64, P, L64, P, L64, I, I, I, P, L64, P],
+        "bsw_direct_pop": [P, I, I, P, L64, P, L64, P, L64, P, L64, I, I, I, P, L64, P],
+        "bsw_direct_tables": [P, L64, P, P, L64, L64, I, I, I, P, P, P],
         "bsw_bins_create": [PP, I, I, I, I, P, P],
         "bsw_bins_destroy": [P],
         "bsw_bins_device_ptrs": [P, I, PP, PP, PP],
@@ -142,6 +145,7 @@ def _set_argtypes(L):
         "bsw_codec_profile": [P, I, P, P],
         "bsw_codec_set_two_phase": [P, I],
         "bsw_codec_set_dual_stream": [P, I],
+        "bsw_codec_set_coder": [P, I],
         "bsw_discretize_reset": [P, I, P],
         "bsw_discretize_sample": [P, P, L64, P, ctypes.c_float, P, P, L64, I, P],
         "bsw_discretize_fold": [P, P, L64, I, P],
@@ -160,11 +164,11 @@ EXPORTS = ["bsw_last_error", "bsw_version", "bsw_has_tensor_cores", "bsw_measure
            "bsw_streams_capacity", "bsw_streams_import", "bsw_streams_fill", "bsw_streams_sizes", "bsw_streams_min_words", "bsw_streams_rest_words", "bsw_streams_export",
            "bsw_streams_device_ptrs", "bsw_streams_pack", "bsw_streams_unpack", "bsw_streams_pack_trimmed", "bsw_streams_unpack_trimmed", "bsw_streams_total_words", "bsw_ans_tables", "bsw_ans_push", "bsw_ans_pop",
            "bsw_logistic_pmfs", "bsw_logistic_tables", "bsw_logistic_push", "bsw_logistic_pop", "bsw_logistic_scratch_bytes", "bsw_set_rows_mode", "bsw_bins_level_is_uniform", "bsw_rows6_set_verify", "bsw_rows6_verify_read", "bsw_rows6_set_lanes_per_row", "bsw_set_conv_mode", "bsw_logistic_push_2p",
-           "bsw_logistic_pop_2p", "bsw_bins_create",
+           "bsw_logistic_pop_2p", "bsw_direct_push", "bsw_direct_pop", "bsw_direct_tables", "bsw_bins_create",
            "bsw_bins_destroy", "bsw_bins_device_ptrs", "bsw_gather_zcentres", "bsw_gather_xcentres",
            "bsw_model_create", "bsw_model_destroy", "bsw_model_load_conv", "bsw_model_load_gen_std",
            "bsw_model_finalize", "bsw_model_set_tc_precision", "bsw_vae_infer", "bsw_vae_generate", "bsw_codec_create", "bsw_codec_destroy",
-           "bsw_codec_encode", "bsw_codec_decode", "bsw_codec_encode_ext", "bsw_codec_decode_ext", "bsw_codec_last_launches", "bsw_codec_profile", "bsw_codec_set_two_phase", "bsw_codec_set_dual_stream",
+           "bsw_codec_encode", "bsw_codec_decode", "bsw_codec_encode_ext", "bsw_codec_decode_ext", "bsw_codec_last_launches", "bsw_codec_profile", "bsw_codec_set_two_phase", "bsw_codec_set_dual_stream", "bsw_codec_set_coder",
            "bsw_discretize_reset", "bsw_discretize_sample", "bsw_discretize_fold", "bsw_discretize_edges"]
 
 

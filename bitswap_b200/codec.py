@@ -19,6 +19,14 @@ BITSWAP, BBANS = 0, 1
 MIN_QUANTBITS = 5           # narrowest latent support of the device codec: 32 bins (every coder kernel owns S/32 bins per lane)
 MAX_QUANTBITS = 12          # widest latent support of the device codec: 4096 bins
 FUSED_MAX_SUPPORT = 1024    # the fused coder keeps a row table in one warp's registers
+# Quantiser of the coder (BSW_CODER_REFERENCE / BSW_CODER_DIRECT of include/bitswap_b200.h)
+CODERS = {"reference": 0, "direct": 1}
+
+
+def check_coder(coder):
+    """ValueError unless `coder` is "reference" or "direct" (raised before any device work)."""
+    if not (isinstance(coder, str) and coder in CODERS):
+        raise ValueError(f"coder must be one of {sorted(CODERS)}, got {coder!r}")
 
 
 def check_quantbits(q):
@@ -63,7 +71,12 @@ class Bins:
 
 
 class BitSwapCodec:
-    def __init__(self, cfg: CodecConfig, model: Model, bins: Bins, max_batch: int):
+    """coder: "reference" (default) quantises every level as the reference's ANS.__init__ does, so its bitstreams are the
+    reference's; "direct" quantises each bin's cdf on its own (see bsw_direct_push), which needs no whole-row table and
+    codes faster at the same rate, with its own bitstreams: a stream decodes only with the coder that encoded it."""
+
+    def __init__(self, cfg: CodecConfig, model: Model, bins: Bins, max_batch: int, coder: str = "reference"):
+        check_coder(coder)
         self.cfg, self.model, self.bins, self.max_batch = cfg, model, bins, int(max_batch)
         self.device = model.device
         if bins.device != self.device:
@@ -71,6 +84,13 @@ class BitSwapCodec:
         self._h = ctypes.c_void_p()
         with on_device(self.device):
             check(lib().bsw_codec_create(ctypes.byref(self._h), model.handle, bins.handle, self.max_batch))
+            check(lib().bsw_codec_set_coder(self._h, CODERS[coder]))
+        self._coder = coder
+
+    @property
+    def coder(self):
+        """The quantiser this codec codes with: "reference" or "direct"."""
+        return self._coder
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -141,7 +161,11 @@ class BitSwapCodec:
 
     def set_two_phase(self, on=True):
         """True (default): parallel row-table kernel + serial coder; False: fused one-warp-per-stream kernels, which hold a
-        row's table in registers and so take at most 1024 bins (quantbits <= 10): ValueError above that."""
+        row's table in registers and so take at most 1024 bins (quantbits <= 10): ValueError above that.  The switch picks
+        between reference coders: ValueError on a direct codec."""
+        if not on and self._coder != "reference":
+            raise ValueError("set_two_phase(False): the direct coder has only its two-phase kernels; the fused coder is a "
+                             "reference coder")
         if not on and self.cfg.zsupport > FUSED_MAX_SUPPORT:
             raise ValueError(f"set_two_phase(False): the fused coder takes at most {FUSED_MAX_SUPPORT} bins per row, these bins "
                              f"have {self.cfg.zsupport} (quantbits {self.cfg.quantbits}); keep the two-phase coder")
@@ -163,10 +187,12 @@ class PipelinedCodec:
     different sub-batches drift apart in phase, so their kernels share SMs and the two pipes overlap
     (4 lanes by default).  Results are identical to a single BitSwapCodec: every stream is independent and every kernel is
     batch-invariant.  Each lane owns a model replica (activations are per-lane anyway).  tc_precision: the arithmetic of
-    every lane's tensor-core convs ("split" or "bf16", see Model); it changes the bitstreams."""
+    every lane's tensor-core convs ("split" or "bf16", see Model); coder: the quantiser of every lane ("reference" or
+    "direct", see BitSwapCodec).  Both change the bitstreams."""
 
     def __init__(self, cfg: CodecConfig, state_dict, bins: Bins, max_batch: int, lanes: int = 4, use_tensor_cores=True, lane_size: int = 0,
-                 free_running: bool = False, tc_precision: str = "split"):
+                 free_running: bool = False, tc_precision: str = "split", coder: str = "reference"):
+        check_coder(coder)
         self.cfg, self.bins, self.max_batch = cfg, bins, int(max_batch)
         self.device = bins.device
         self.lanes = max(1, min(int(lanes), self.max_batch))
@@ -187,7 +213,7 @@ class PipelinedCodec:
                                   tc_precision=tc_precision).load_state_dict(state_dict)
             m.compress()
             self.models.append(m)
-            self.codecs.append(BitSwapCodec(cfg, m, bins, self.per))
+            self.codecs.append(BitSwapCodec(cfg, m, bins, self.per, coder=coder))
             self.streams.append(torch.cuda.Stream(device=self.device))
 
     def _ranges(self, count):
@@ -231,7 +257,14 @@ class PipelinedCodec:
                                                   extent=None if extent is None else extent[b:b + n]))
         return out
 
+    @property
+    def coder(self):
+        return self.codecs[0].coder
+
     def set_two_phase(self, on=True):
+        if not on and self.coder != "reference":
+            raise ValueError("set_two_phase(False): the direct coder has only its two-phase kernels; the fused coder is a "
+                             "reference coder")
         if not on and self.cfg.zsupport > FUSED_MAX_SUPPORT:
             raise ValueError(f"set_two_phase(False): the fused coder takes at most {FUSED_MAX_SUPPORT} bins per row, these bins "
                              f"have {self.cfg.zsupport} (quantbits {self.cfg.quantbits}); keep the two-phase coder")

@@ -579,6 +579,12 @@ int launch_rows(int phase, bool pop, bsw_streams *s, int first, int count, const
 
 }  // namespace
 
+// The serial push of the two-phase coder on (P_s, C_s, reciprocal) rows made elsewhere (the direct coder's phase A).
+int bsw_push_pairs(bsw_streams *s, int first, int count, const void *pairs, int64_t L, int bits, const int16_t *ext,
+                   cudaStream_t st) {
+    return launch_push_pairs(s, first, count, pairs, L, bits, ext, st);
+}
+
 // Pop from ONE materialised table shared by every stream (the Logistic(0,1) prior): P [L][S] with the remnant already
 // applied, coarse[L][S/32] = C[i][32 r], fix = zeros.
 __global__ void k_coarse_from_cdf(const uint32_t *__restrict__ C, int64_t L, int S, uint32_t *__restrict__ coarse, uint2 *__restrict__ fix) {

@@ -28,6 +28,8 @@ struct bsw_codec {
     uint32_t *priorP, *priorC;
     uint32_t *priorCoarse = nullptr;    // prior cdf at every 32nd bin + dummy fix: lets the prior pop use k_pop_full
     uint2 *priorFix = nullptr;          // Logistic(0,1) prior tables over zendpoints[-1], shared by all streams
+    int coder = BSW_CODER_REFERENCE;    // quantiser of every level and the prior (bsw_codec_set_coder)
+    uint32_t *priorPd = nullptr, *priorCd = nullptr;   // the prior's direct tables, built at the first switch to direct
     int64_t launches;
     BswProf prof;
     // overlap mode (bsw_codec_set_dual_stream(c, 1)): the recursion is enqueued as a DAG on three internal streams --
@@ -136,6 +138,7 @@ extern "C" int bsw_codec_destroy(bsw_codec *c) {
     cudaFree(c->sym[0]); cudaFree(c->sym[1]); cudaFree(c->xsym);
     for (auto p : c->zs) cudaFree(p);
     cudaFree(c->priorP); cudaFree(c->priorC); cudaFree(c->scratch); cudaFree(c->priorCoarse); cudaFree(c->priorFix);
+    cudaFree(c->priorPd); cudaFree(c->priorCd);
     for (cudaStream_t st : {c->st_conv, c->st_rows, c->st_ser}) if (st) cudaStreamDestroy(st);
     for (auto &e : c->ev) cudaEventDestroy(e);
     delete c;
@@ -153,6 +156,8 @@ extern "C" int bsw_codec_set_dual_stream(bsw_codec *c, int on) {
 
 extern "C" int bsw_codec_set_two_phase(bsw_codec *c, int on) {
     BSW_REQUIRE(c, "null codec");
+    BSW_REQUIRE(on || c->coder == BSW_CODER_REFERENCE,
+                "bsw_codec_set_two_phase: the direct coder has only its two-phase kernels; the switch picks a reference coder");
     // the fused kernels keep a whole row table in one warp's registers (S/32 bins per lane): 1024 bins at most
     if (!on && c->S > 1024) {
         bsw_set_error("bsw_codec_set_two_phase: the fused coder holds at most 1024 bins per row in registers; these bins "
@@ -160,6 +165,26 @@ extern "C" int bsw_codec_set_two_phase(bsw_codec *c, int on) {
         return BSW_E_INVALID;
     }
     c->two_phase = on ? 1 : 0;
+    return BSW_OK;
+}
+
+extern "C" int bsw_codec_set_coder(bsw_codec *c, int coder) {
+    BSW_REQUIRE(c, "null codec");
+    BSW_REQUIRE(coder == BSW_CODER_REFERENCE || coder == BSW_CODER_DIRECT, "bsw_codec_set_coder: unknown coder");
+    if (coder == BSW_CODER_DIRECT && !c->priorPd) {
+        // the prior's rows are the same for every stream: its direct tables are built once, as the reference ones are
+        BSW_CUDA(cudaMalloc(&c->priorPd, sizeof(uint32_t) * (size_t)c->zdim * c->S));
+        BSW_CUDA(cudaMalloc(&c->priorCd, sizeof(uint32_t) * (size_t)c->zdim * (c->S + 1)));
+        double ms[2] = {0.0, 1.0}, *dms = nullptr;
+        BSW_CUDA(cudaMalloc(&dms, sizeof(ms)));
+        BSW_CUDA(cudaMemcpy(dms, ms, sizeof(ms), cudaMemcpyHostToDevice));
+        const double *zend = c->b->zend + (size_t)(c->nz - 1) * c->zdim * c->S;
+        int rc = bsw_direct_tables_st(zend, c->S, dms, dms + 1, 0, c->zdim, c->S, c->priorPd, c->priorCd, nullptr);
+        BSW_CUDA(cudaDeviceSynchronize());
+        cudaFree(dms);
+        if (rc) { cudaFree(c->priorPd); cudaFree(c->priorCd); c->priorPd = c->priorCd = nullptr; return rc; }
+    }
+    c->coder = coder;
     return BSW_OK;
 }
 
@@ -252,6 +277,20 @@ struct Ctx {
         const int cat_rows = x ? CAT_ROWS_X : CAT_ROWS_Z;
         const int cat_ser = x ? (pop ? CAT_POP_X : CAT_PUSH_X) : (pop ? CAT_POP_Z : CAT_PUSH_Z);
         const int16_t *lext = x ? ext : nullptr;
+        if (c->coder == BSW_CODER_DIRECT) {
+            void *scr = (!pop && c->dual_stream) ? c->scratch_push : c->scratch;
+            const size_t scr_bytes = (!pop && c->dual_stream) ? c->scratch_push_bytes : c->scratch_bytes;
+            nl += 2;
+            c->prof.begin(cat_rows, rows);
+            int rc = bsw_direct_2p(0, pop, s, first, count, mu, L, sc, sss, endp, ers, sym, L, S, scr, scr_bytes, nullptr, rows);
+            c->prof.end(rows);
+            if (rc) return rc;
+            hop(rows, ser);
+            c->prof.begin(cat_ser, ser);
+            rc = bsw_direct_2p(1, pop, s, first, count, mu, L, sc, sss, endp, ers, sym, L, S, scr, scr_bytes, lext, ser);
+            c->prof.end(ser);
+            return rc;
+        }
         if (!c->two_phase) {
             hop(rows, ser);
             ++nl;
@@ -294,14 +333,18 @@ struct Ctx {
     int push_prior(const int16_t *sym) {
         ++nl;
         c->prof.begin(CAT_PRIOR, ser);
-        int rc = bsw_ans_push_i16(s, first, count, c->priorP, c->priorC, 0, 0, sym, c->zdim, c->S, 31, ser);
+        int rc = c->coder == BSW_CODER_DIRECT
+            ? bsw_ans_push_i16(s, first, count, c->priorPd, c->priorCd, 0, 0, sym, c->zdim, c->S, 31, ser)
+            : bsw_ans_push_i16(s, first, count, c->priorP, c->priorC, 0, 0, sym, c->zdim, c->S, 31, ser);
         c->prof.end(ser);
         return rc;
     }
     int pop_prior(int16_t *sym) {
         ++nl;
         c->prof.begin(CAT_PRIOR, ser);
-        int rc = c->priorCoarse
+        int rc = c->coder == BSW_CODER_DIRECT
+            ? bsw_ans_pop_i16(s, first, count, c->priorPd, c->priorCd, 0, 0, sym, c->zdim, c->S, 31, ser)
+            : c->priorCoarse
             ? bsw_pop_shared_table(s, first, count, c->priorP, c->priorCoarse, c->priorFix, sym, c->zdim, c->S, 31, ser)
             : bsw_ans_pop_i16(s, first, count, c->priorP, c->priorC, 0, 0, sym, c->zdim, c->S, 31, ser);
         c->prof.end(ser);

@@ -143,6 +143,14 @@ int bsw_pop_shared_table(bsw_streams *s, int first, int count, const uint32_t *P
 int bsw_logistic_2p(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
                     int64_t sss, const double *endp, int64_t ers, const void *meta, int16_t *sym, int64_t L, int S, int bits, int q,
                     void *scratch, size_t scratch_bytes, const int16_t *ext, cudaStream_t st);
+int bsw_push_pairs(bsw_streams *s, int first, int count, const void *pairs, int64_t L, int bits, const int16_t *ext,
+                   cudaStream_t st);
+// ans_direct.cu: the direct-cdf coder
+int bsw_direct_2p(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,
+                  int64_t sss, const double *endp, int64_t ers, int16_t *sym, int64_t L, int S, void *scratch,
+                  size_t scratch_bytes, const int16_t *ext, cudaStream_t st);
+int bsw_direct_tables_st(const double *endp, int64_t ers, const double *mu, const double *sc, int64_t ms, int64_t L, int S,
+                         uint32_t *P, uint32_t *C, cudaStream_t st);
 // ans_rows6.cu: the affine-row kernels
 int bsw_rows6_build_meta(const double *endp, int64_t ers, int64_t L, int S, void *meta_dev, int *n_affine_host, cudaStream_t st);
 int bsw_rows6_launch(int phase, bool pop, bsw_streams *s, int first, int count, const float *mu, int64_t mss, const float *sc,

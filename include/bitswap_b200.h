@@ -225,6 +225,31 @@ int bsw_logistic_pop_2p(bsw_streams *s, int first, int count, const float *mu_de
                         void *scratch_dev, int64_t scratch_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * The direct-cdf coder: an opt-in quantiser with its OWN bitstreams (not the reference's).  Each bin's integer cdf
+ * comes from that bin's float cdf alone, so no call needs a whole-row table:
+ *     F_k = the float64 logistic cdf at endpoint k (== torch.sigmoid((e_k - mu) / sigma)), a NaN argument counting as 0
+ *     C_0 = 0,  C_S = 2^31,  C_k = floor(RN(F_{k-1} * (2^31 - 2S))) + 2k  (k = 1 .. S-1),  P_k = C_{k+1} - C_k
+ * Every P_k >= 1; the endpoint row's pad is never read.  The same formula codes latents, pixels (S = 256) and the prior.
+ * bsw_direct_push / bsw_direct_pop take the arguments of bsw_logistic_*_2p (bits must be 31; quantbits does not enter the
+ * quantiser) and the same scratch size.  The rows mode, the k_rows6 lanes-per-row and verify switches and the fused
+ * coder do not apply to them.  bsw_direct_tables exports P [L,S] and C [L,S+1] as bsw_logistic_tables does (mu, scale
+ * as double; the rows need only S-1 endpoints).
+ * ---------------------------------------------------------------------------------------------- */
+#define BSW_CODER_REFERENCE 0
+#define BSW_CODER_DIRECT    1
+int bsw_direct_push(bsw_streams *s, int first, int count, const float *mu_dev, int64_t mu_stream_stride,
+                    const float *scale_dev, int64_t scale_stream_stride, const double *endpoints_dev,
+                    int64_t endp_row_stride, const int16_t *sym_dev, int64_t L, int S, int bits, int quantbits,
+                    void *scratch_dev, int64_t scratch_bytes, void *stream);
+int bsw_direct_pop(bsw_streams *s, int first, int count, const float *mu_dev, int64_t mu_stream_stride,
+                   const float *scale_dev, int64_t scale_stream_stride, const double *endpoints_dev,
+                   int64_t endp_row_stride, int16_t *sym_dev, int64_t L, int S, int bits, int quantbits,
+                   void *scratch_dev, int64_t scratch_bytes, void *stream);
+int bsw_direct_tables(const double *endpoints_dev, int64_t endp_row_stride, const double *mu_dev,
+                      const double *scale_dev, int64_t ms, int64_t L, int S, int bits, int quantbits,
+                      uint32_t *P_dev, uint32_t *C_dev, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Bin tables on the device.
  * Replaces: the tensors returned by discretize() (discretization.py:9-99) and ImageBins
  * (utils/torch/rand.py:134-153); the library keeps its own padded copy (each endpoint row padded
@@ -354,8 +379,13 @@ int bsw_codec_set_dual_stream(bsw_codec *c, int on);
 /* Coder variant: 1 (default) = two-phase (ans_rows.cu: fully parallel float64 row tables, then the serial integer
  * coder), 0 = fused one-warp-per-stream kernels (bsw_logistic_push/pop).  Bit-identical results.  0 is refused
  * (BSW_E_INVALID) when the codec's bins have more than 1024 bins per row (quantbits 11 and 12): the fused kernels
- * cannot hold such a table in registers. */
+ * cannot hold such a table in registers, and on a codec set to the direct coder (the switch picks between reference
+ * coders). */
 int bsw_codec_set_two_phase(bsw_codec *c, int on);
+/* Quantiser of every level and the prior, from the next encode or decode on: BSW_CODER_REFERENCE (default, the
+ * reference's bitstreams) or BSW_CODER_DIRECT (see bsw_direct_push; its own bitstreams, decodable only by a direct codec).
+ * The first switch to direct builds the direct prior tables and synchronises.  BSW_E_INVALID for any other value. */
+int bsw_codec_set_coder(bsw_codec *c, int coder);
 /* Per-kernel-category device time (CUDA events on the launching stream) accumulated since profiling was
  * enabled.  ms_out/n_out: 12 entries {misc, conv_in, conv_dense3x3, conv_dense5x5, conv_head, pop_z, push_z,
  * pop_x, push_x, prior, rows_z, rows_x} (rows_* = phase A of the two-phase coder; pop/push = phase B).  enable: 1 = reset and start, 0 = reset and stop, -1 = read only.  Synchronises. */
