@@ -153,6 +153,11 @@ def _set_argtypes(L):
         "bsw_selftest_cdf": [L64, U64, P, P],
         "bsw_selftest_cdf_apx": [L64, U64, P],
         "bsw_selftest_conv": [P, ctypes.c_char_p, P, L64, I, P, P, P, P, P, P],
+        "bsw_bitstream_revision": [],
+        "bsw_digest": [P, L64, P, P],
+        "bsw_model_digest": [P, P, P],
+        "bsw_bins_digest": [P, P, P],
+        "bsw_codec_fingerprint": [P, P, P],
     }
     for name, args in sig.items():
         fn = getattr(L, name, None)
@@ -169,7 +174,8 @@ EXPORTS = ["bsw_last_error", "bsw_version", "bsw_has_tensor_cores", "bsw_measure
            "bsw_model_create", "bsw_model_destroy", "bsw_model_load_conv", "bsw_model_load_gen_std",
            "bsw_model_finalize", "bsw_model_set_tc_precision", "bsw_vae_infer", "bsw_vae_generate", "bsw_codec_create", "bsw_codec_destroy",
            "bsw_codec_encode", "bsw_codec_decode", "bsw_codec_encode_ext", "bsw_codec_decode_ext", "bsw_codec_last_launches", "bsw_codec_profile", "bsw_codec_set_two_phase", "bsw_codec_set_dual_stream", "bsw_codec_set_coder",
-           "bsw_discretize_reset", "bsw_discretize_sample", "bsw_discretize_fold", "bsw_discretize_edges"]
+           "bsw_discretize_reset", "bsw_discretize_sample", "bsw_discretize_fold", "bsw_discretize_edges",
+           "bsw_bitstream_revision", "bsw_digest", "bsw_model_digest", "bsw_bins_digest", "bsw_codec_fingerprint"]
 
 
 def device_index(device=None):
@@ -203,6 +209,11 @@ def measure_fp64_peak():
     v = ctypes.c_double()
     check(lib().bsw_measure_fp64_peak(ctypes.byref(v)))
     return v.value
+
+
+def digest_hex(out4):
+    """A bsw_digest result (four uint32) as 32 hex digits: its 16 bytes, little-endian."""
+    return bytes(b for v in out4 for b in int(v).to_bytes(4, "little")).hex()
 
 
 def has_tensor_core_path():

@@ -5,14 +5,15 @@ Replaces the sender/receiver loop bodies of the reference's compress()
 a whole batch of independent chains; the ANS state never leaves the GPU between
 latent levels.  Chain more images onto the same streams by calling again.
 """
+import collections
 import ctypes
 
 import numpy as np
 import torch
 
-from ._lib import lib, check, cuda_stream_ptr, device_index, on_device
+from ._lib import lib, check, cuda_stream_ptr, device_index, digest_hex, on_device
 from .config import CodecConfig
-from .model import Model
+from .model import TC_PRECISIONS, Model
 from .streams import StreamSet
 
 BITSWAP, BBANS = 0, 1
@@ -21,6 +22,29 @@ MAX_QUANTBITS = 12          # widest latent support of the device codec: 4096 bi
 FUSED_MAX_SUPPORT = 1024    # the fused coder keeps a row table in one warp's registers
 # Quantiser of the coder (BSW_CODER_REFERENCE / BSW_CODER_DIRECT of include/bitswap_b200.h)
 CODERS = {"reference": 0, "direct": 1}
+
+
+Fingerprint = collections.namedtuple(
+    "Fingerprint", "revision xc nz zchannels nprocessing kernel_size resdepth reswidth cond_xscale quantbits "
+                   "use_tensor_cores tc_precision tc_heads coder model_digest bins_digest")
+Fingerprint.__doc__ = """Everything that decides a codec's bitstreams (bsw_codec_fingerprint): the bitstream revision of the library, the
+model's architecture, quantbits, the conv path (use_tensor_cores, tc_precision "split" / "bf16", tc_heads: whether the heads
+run on the tensor cores), the coder ("reference" / "direct") and 32-hex-digit digests of the folded weights and of the bin
+tables the kernels read.  Two codecs with equal fingerprints write and read the same bitstreams."""
+
+
+class _Fp(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int32) for n in Fingerprint._fields[:14]] + [("model_digest", ctypes.c_uint32 * 4),
+                                                                          ("bins_digest", ctypes.c_uint32 * 4)]
+
+
+def device_digest(t):
+    """bsw_digest of a contiguous CUDA tensor's bytes, as 32 hex digits (see include/bitswap_b200.h for the definition)."""
+    assert t.is_cuda and t.is_contiguous()
+    out = (ctypes.c_uint32 * 4)()
+    with on_device(t.device.index):
+        check(lib().bsw_digest(ctypes.c_void_p(t.data_ptr()), t.numel() * t.element_size(), out, cuda_stream_ptr()))
+    return digest_hex(out)
 
 
 def check_coder(coder):
@@ -59,6 +83,13 @@ class Bins:
     @property
     def handle(self):
         return self._h
+
+    def digest(self):
+        """Digest of these bin tables as stored on the device (bsw_bins_digest), 32 hex digits; computed once."""
+        out = (ctypes.c_uint32 * 4)()
+        with on_device(self.device):
+            check(lib().bsw_bins_digest(self._h, out, cuda_stream_ptr()))
+        return digest_hex(out)
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -149,6 +180,18 @@ class BitSwapCodec:
     @property
     def last_launches(self):
         return int(lib().bsw_codec_last_launches(self._h))
+
+    def fingerprint(self):
+        """The Fingerprint of this codec as it is now (the coder it was last set to).  The digests are computed on the
+        device the first time and kept with the model and the bins."""
+        f = _Fp()
+        with on_device(self.device):
+            check(lib().bsw_codec_fingerprint(self._h, ctypes.byref(f), cuda_stream_ptr()))
+        precision = {v: k for k, v in TC_PRECISIONS.items()}
+        coders = {v: k for k, v in CODERS.items()}
+        return Fingerprint(f.revision, f.xc, f.nz, f.zchannels, f.nprocessing, f.kernel_size, f.resdepth, f.reswidth,
+                           bool(f.cond_xscale), f.quantbits, bool(f.use_tensor_cores), precision[f.tc_precision],
+                           bool(f.tc_heads), coders[f.coder], digest_hex(f.model_digest), digest_hex(f.bins_digest))
 
     CATEGORIES = ("misc", "conv_in", "conv_dense3x3", "conv_dense5x5", "conv_head", "pop_z", "push_z", "pop_x",
                   "push_x", "prior", "rows_z", "rows_x")
@@ -260,6 +303,14 @@ class PipelinedCodec:
     @property
     def coder(self):
         return self.codecs[0].coder
+
+    def fingerprint(self):
+        """The lanes' common Fingerprint; RuntimeError if two lanes would write different bitstreams."""
+        fps = [c.fingerprint() for c in self.codecs]
+        for i, f in enumerate(fps[1:], 1):
+            if f != fps[0]:
+                raise RuntimeError(f"lane {i} of this PipelinedCodec has fingerprint {f}, lane 0 {fps[0]}")
+        return fps[0]
 
     def set_two_phase(self, on=True):
         if not on and self.coder != "reference":

@@ -41,6 +41,15 @@ Read as a reference tail its width is ARCHIVE_MARK >= 2^31 and as a multi-chain 
 so unpack_container refuses it.  Decoding an image pops, in each chain holding its blocks, from the chain's end down to its
 first block there; a chain popped to its first block must come back to the seeded initial state (cifar_compress.py:356).
 Containers and archives share one encode loop (_encode) and one decode loop (_decode_regions) over a block sequence.
+
+Stamps (opt-in: stamp=True): any of the three layouts above may carry, after its last word, what the codec that wrote it was
+    [ inner array, byte-identical to the unstamped one | fields (uint32) | nfields, STAMP_VERSION, STAMP_MARK ]
+with the fields of version 1, in order: the Fingerprint (revision, xc, nz, zchannels, nprocessing, kernel_size, resdepth,
+reswidth, cond_xscale, quantbits, use_tensor_cores, tc_precision 0 split / 1 bf16, tc_heads, coder 0 reference / 1 direct,
+model digest [4], bins digest [4]), then scheme, hwc_quirk, excess_state_len and seed.  STAMP_MARK >= 2^31 sits where the
+reference layout has w and the archive its ARCHIVE_MARK, so a reader of the unstamped layouts refuses a stamped array.  The
+decoders compare a stamp with codec.fingerprint() and their own scheme, hwc_quirk and channels before any stream is
+created, and refuse it naming every field that differs; a stamped container also gets the archives' initial-state check.
 """
 import collections
 import numbers
@@ -48,7 +57,8 @@ import numbers
 import numpy as np
 import torch
 
-from .codec import BBANS, BITSWAP
+from .codec import BBANS, BITSWAP, CODERS, Fingerprint
+from .model import TC_PRECISIONS
 from .streams import StreamSet
 from .synthetic import initial_words
 
@@ -57,6 +67,94 @@ MAX_BLOCKS = 1 << 20                     # blocks per image a container may decl
 ARCHIVE_MARK = 0x80415243                # bit 31 | "ARC": last word of an archive
 MAX_ARCHIVE_BLOCKS = 1 << 24             # blocks an archive may declare in all
 MAX_INITIAL_WORDS = 1 << 24              # largest excess_state_len an archive may declare
+STAMP_MARK = 0x80535450                  # bit 31 | "STP": last word of a stamped container or archive
+STAMP_VERSION = 1
+_STAMP_NFIELDS = {1: 26}                 # per version: 14 fingerprint words, two 4-word digests, 4 coding arguments
+
+Stamp = collections.namedtuple("Stamp", "fingerprint scheme hwc_quirk excess_state_len seed")
+Stamp.__doc__ = """What a stamped container or archive records about its writer: the codec's Fingerprint, the scheme (BITSWAP /
+BBANS), hwc_quirk and the seeded initial state (excess_state_len, seed) every chain started from."""
+
+
+def _stamp_words(fp, scheme, hwc_quirk, excess_state_len, seed):
+    """The stamp appended to an array: fields, nfields, STAMP_VERSION, STAMP_MARK."""
+    f = list(fp[:14])
+    f[Fingerprint._fields.index("tc_precision")] = TC_PRECISIONS[fp.tc_precision]
+    f[Fingerprint._fields.index("coder")] = CODERS[fp.coder]
+    digests = [np.frombuffer(bytes.fromhex(d), dtype="<u4") for d in (fp.model_digest, fp.bins_digest)]
+    fields = np.concatenate([np.array([int(v) for v in f], dtype=np.uint32)] + digests
+                            + [np.array([scheme, int(hwc_quirk), excess_state_len, seed], dtype=np.uint32)])
+    return np.concatenate([fields, np.array([fields.size, STAMP_VERSION, STAMP_MARK], dtype=np.uint32)])
+
+
+def _check_stamp_args(scheme, excess_state_len, seed):
+    if scheme not in (BITSWAP, BBANS):
+        raise ValueError(f"scheme must be BITSWAP or BBANS, got {scheme!r}")
+    for name, v, lo, hi in (("excess_state_len", excess_state_len, 2, MAX_INITIAL_WORDS), ("seed", seed, 0, (1 << 32) - 1)):
+        if isinstance(v, bool) or not isinstance(v, numbers.Integral) or not lo <= v <= hi:
+            raise ValueError(f"{name} must be an int in [{lo}, {hi}], got {v!r}")
+
+
+def _split_stamp(a):
+    """(inner array, Stamp) of a stamped array, (a, None) of any other.  Every stamp field is checked here, before anything
+    is sized from it: a truncated or malformed stamp is a ValueError."""
+    if a.ndim != 1 or a.size < 3 or int(a[-1]) != STAMP_MARK:
+        return a, None
+    nfields, version = int(a[-3]), int(a[-2])
+    if version not in _STAMP_NFIELDS:
+        raise ValueError(f"stamp of unknown version {version} (this reader knows {sorted(_STAMP_NFIELDS)})")
+    if nfields != _STAMP_NFIELDS[version]:
+        raise ValueError(f"stamp version {version} has {_STAMP_NFIELDS[version]} fields, this one claims {nfields}")
+    if a.size < nfields + 4:
+        raise ValueError(f"stamped array of {a.size} words cannot hold its {nfields} stamp fields and a stamped array")
+    f = [int(v) for v in a[a.size - 3 - nfields:-3]]
+    inner = a[:a.size - 3 - nfields]
+    if int(inner[-1]) == STAMP_MARK:
+        raise ValueError("a stamp inside a stamp")
+    n = len(Fingerprint._fields) - 2
+    head, digests, (scheme, hwc_quirk, excess_state_len, seed) = f[:n], f[n:n + 8], f[n + 8:]
+    names = Fingerprint._fields
+    for name, ok in (("cond_xscale", (0, 1)), ("kernel_size", (1, 3, 5, 7)), ("quantbits", range(5, 13)),
+                     ("use_tensor_cores", (0, 1)), ("tc_precision", TC_PRECISIONS.values()), ("tc_heads", (0, 1)),
+                     ("coder", CODERS.values())):
+        if head[names.index(name)] not in ok:
+            raise ValueError(f"stamp: {name} = {head[names.index(name)]} is out of range")
+    if scheme not in (BITSWAP, BBANS) or hwc_quirk not in (0, 1):
+        raise ValueError(f"stamp: scheme = {scheme}, hwc_quirk = {hwc_quirk} out of range")
+    if not 2 <= excess_state_len <= MAX_INITIAL_WORDS:
+        raise ValueError(f"stamp: excess_state_len {excess_state_len} outside [2, {MAX_INITIAL_WORDS}]")
+    precision = {v: k for k, v in TC_PRECISIONS.items()}
+    coders = {v: k for k, v in CODERS.items()}
+    for name, conv in (("cond_xscale", bool), ("use_tensor_cores", bool), ("tc_precision", precision.get),
+                       ("tc_heads", bool), ("coder", coders.get)):
+        head[names.index(name)] = conv(head[names.index(name)])
+    fp = Fingerprint(*head, *(np.asarray(digests[k:k + 4], dtype="<u4").tobytes().hex() for k in (0, 4)))
+    return inner, Stamp(fp, scheme, bool(hwc_quirk), excess_state_len, seed)
+
+
+def read_stamp(array):
+    """The Stamp of a stamped container or archive, None for an unstamped one; on the host only, so that a user can see
+    which codec decodes it before building one.  A malformed stamp is a ValueError."""
+    return _split_stamp(np.asarray(array, dtype=np.uint32))[1]
+
+
+def _check_stamps(codec, stamps, scheme, hwc_quirk, channels, what):
+    """ValueError naming every field in which a stamp differs from this codec and these arguments (stamps: one Stamp or
+    None per array).  The codec is asked for its fingerprint only when some array is stamped."""
+    if all(st is None for st in stamps):
+        return
+    fp = codec.fingerprint()
+    for i, st in enumerate(stamps):
+        if st is None:
+            continue
+        want = list(zip(Fingerprint._fields, st.fingerprint, fp)) + [("scheme", st.scheme, scheme),
+                                                                    ("hwc_quirk", st.hwc_quirk, bool(hwc_quirk))]
+        if channels is not None:
+            want.append(("channels", st.fingerprint.xc, channels))
+        diff = [f"{name}: stamped {a!r}, here {b!r}" for name, a, b in want if a != b]
+        if diff:
+            raise ValueError(f"{what} {i} was written by a different codec or with other arguments; it cannot be decoded "
+                             f"here: " + "; ".join(diff))
 
 
 def extract_blocks(arr, block_size=(32, 32)):
@@ -150,7 +248,7 @@ def _active(nblk):
 
 
 def compress_images(codec, images, excess_state_len=10000, seed=100, scheme=BITSWAP, hwc_quirk=False, words_per_block=1400,
-                    edges="crop", chain_blocks=None):
+                    edges="crop", chain_blocks=None, stamp=False):
     """images: list of HWC uint8 arrays.  Returns one container array per image.
     Every chain starts from the reference's initial state: `excess_state_len` random words drawn with
     np.random.seed(100) (demo_compress.py:113-115, :202).
@@ -158,12 +256,17 @@ def compress_images(codec, images, excess_state_len=10000, seed=100, scheme=BITS
     edges="code": the whole image (any H, W >= 1) is coded, with partial blocks at the bottom and right edges;
     decompress_images returns it exactly.
     chain_blocks: None (the reference's one chain per image) or a positive int L: an image of n > L blocks is coded as
-    ceil(n / L) chains of contiguous blocks (chain_sizes), which run side by side.  Fewer serial steps, more initial bits."""
+    ceil(n / L) chains of contiguous blocks (chain_sizes), which run side by side.  Fewer serial steps, more initial bits.
+    stamp=True: every container is followed by a stamp of codec.fingerprint() and these arguments (module docstring),
+    which decompress_images checks; the container before it is unchanged."""
     if edges not in ("crop", "code"):
         raise ValueError(f"edges must be 'crop' or 'code', got {edges!r}")
     if edges == "code" and hwc_quirk:
         raise ValueError("edges='code' needs the CHW block layout: hwc_quirk scrambles the rows and columns the extents refer to")
     chain_blocks = _check_chain_blocks(chain_blocks)
+    if stamp:
+        _check_stamp_args(scheme, excess_state_len, seed)
+        tail = _stamp_words(codec.fingerprint(), scheme, hwc_quirk, excess_state_len, seed)
     images = [np.asarray(im) for im in images]
     if edges == "code":
         tiled = [extract_edge_blocks(im) for im in images]
@@ -182,6 +285,8 @@ def compress_images(codec, images, excess_state_len=10000, seed=100, scheme=BITS
     for t in tiled:
         K = len(chain_sizes(t[0].shape[0], chain_blocks))
         out.append(pack_container(coded[k:k + K], t[2], t[3]))
+        if stamp:
+            out[-1] = np.concatenate([out[-1], tail])
         k += K
     return out
 
@@ -263,8 +368,8 @@ def _check_header(nblocks, h, w, hwc_quirk):
 def unpack_container(c, hwc_quirk=False):
     """Inverse of pack_container: (words uint32, offsets int64 [K+1], heads uint64 [K], nblocks int64 [K], h, w), chain k's
     words being words[offsets[k]:offsets[k+1]].  Every field is checked here, before anything is sized from it: a truncated
-    or inconsistent container is a ValueError."""
-    c = np.asarray(c, dtype=np.uint32)
+    or inconsistent container is a ValueError.  A stamped container is accepted: its stamp is checked and stripped."""
+    c = _split_stamp(np.asarray(c, dtype=np.uint32))[0]
     if c.ndim != 1 or c.size < 5:
         raise ValueError(f"container too short ({c.size} words): needs at least head_lo, head_hi, nblocks, h, w")
     if int(c[-1]) != CHAIN_MARK:
@@ -354,27 +459,46 @@ def plan_regions(containers, regions, hwc_quirk=False):
             for i in range(len(job.shapes))]
 
 
+def _stamped_job(codec, containers, channels, scheme, hwc_quirk):
+    """The decode job of a list of containers, every stamp checked against the codec and the arguments, and each chain's
+    seeded initial state (words, head) where its container is stamped (None where it is not; None alone when no
+    container is stamped)."""
+    split = [_split_stamp(np.asarray(c, dtype=np.uint32)) for c in containers]
+    parsed = [unpack_container(inner, hwc_quirk) for inner, _ in split]
+    _check_stamps(codec, [st for _, st in split], scheme, hwc_quirk, channels, "container")
+    states, initial = {}, []
+    for (_, st), p in zip(split, parsed):
+        if st is not None and (st.excess_state_len, st.seed) not in states:
+            states[st.excess_state_len, st.seed] = initial_words(st.excess_state_len, seed=st.seed)
+        initial += [None if st is None else states[st.excess_state_len, st.seed]] * len(p[3])
+    return _containers_job(parsed), initial if states else None
+
+
 def decompress_regions(codec, containers, regions, channels=3, scheme=BITSWAP, hwc_quirk=False, headroom_words=None):
     """regions: list of (i, y, x, h, w) -> one HWC uint8 array per region, equal to decompress_images(...)[i][y:y+h, x:x+w].
     Only the chains holding a wanted block are imported, and each is popped only down to the earliest block any region on
     its container wants (plan_regions): a chain of n blocks whose earliest wanted block is j costs n - j block decodes.
-    Blocks are row-major, so a window near an image's bottom is cheapest, and a single-chain container gains only there."""
-    job = _containers_job([unpack_container(c, hwc_quirk) for c in containers])
-    return _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_words)
+    Blocks are row-major, so a window near an image's bottom is cheapest, and a single-chain container gains only there.
+    A stamped container must match the codec's fingerprint, scheme, hwc_quirk and channels (ValueError naming every field
+    that differs, before any decoding), and each of its chains popped down to its first block must come back to the
+    stamp's initial state."""
+    job, initial = _stamped_job(codec, containers, channels, scheme, hwc_quirk)
+    return _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_words, initial)
 
 
 def decompress_images(codec, containers, channels=3, scheme=BITSWAP, hwc_quirk=False, headroom_words=None):
     """Inverse of compress_images: list of container arrays -> list of HWC uint8 images (the cropped size for a crop-mode
     container, the full size for an edge-coded one: a header whose h or w is not a multiple of 32).  Single- and
-    multi-chain containers can be mixed in one call."""
-    job = _containers_job([unpack_container(c, hwc_quirk) for c in containers])
+    multi-chain containers can be mixed in one call, and so can stamped and unstamped ones (see decompress_regions)."""
+    job, initial = _stamped_job(codec, containers, channels, scheme, hwc_quirk)
     return _decode_regions(codec, job, [(i, 0, 0, h, w) for i, (h, w) in enumerate(job.shapes)], channels, scheme,
-                           hwc_quirk, headroom_words)
+                           hwc_quirk, headroom_words, initial)
 
 
 def _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_words, initial=None):
-    """Decodes the job's regions.  channels None: the codec's.  initial (words, head): the seeded initial state every chain
-    started from; each chain popped down to its first block must then hold its top words and head, or ValueError."""
+    """Decodes the job's regions.  channels None: the codec's.  initial: per chain, None or the seeded initial state
+    (words, head) it started from; such a chain popped down to its first block must then hold its top words and head, or
+    ValueError."""
     regions, plan = _plan(job, regions)
     if not regions:
         return []
@@ -417,7 +541,7 @@ def _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_w
     host = _model_to_blocks(dev.view(-1, channels, 32, 32).index_select(0, idx).cpu().numpy(), hwc_quirk)
     ss.raise_on_error()
     if initial is not None:
-        _check_initial_state(ss, order, plan.first[order] == 0, *initial)
+        _check_initial_state(ss, order, plan.first[order] == 0, initial)
     out = []
     for i, y, x, h, w in regions:
         gw = block_grid(*job.shapes[i])[1]
@@ -427,15 +551,19 @@ def _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_w
     return out
 
 
-def _check_initial_state(ss, order, done, words, head):
+def _check_initial_state(ss, order, done, initial):
     """A chain popped down to its first block holds what it started from: the top words of the seeded initial stack and
-    its head (cifar_compress.py:356).  done: bool per stream, the streams popped that far; order: each stream's chain."""
+    its head (cifar_compress.py:356).  done: bool per stream, the streams popped that far; order: each stream's chain;
+    initial: per chain, its (words, head) or None (not checked)."""
     got, offs, heads, _ = ss.export()
     for j in np.flatnonzero(done).tolist():
+        if initial[order[j]] is None:
+            continue
+        words, head = initial[order[j]]
         m = int(offs[j + 1] - offs[j])
         if not (m <= words.size and int(heads[j]) == head and np.array_equal(got[offs[j]:offs[j + 1]], words[words.size - m:])):
             raise ValueError(f"chain {int(order[j])} decoded to a state other than the initial one it was coded from: a "
-                             f"different model, bins or conv path than the encoder's, or a corrupt archive")
+                             f"different model, bins or conv path than the encoder's, or a corrupt archive or container")
 
 
 def pack_archive(chains, shapes, excess_state_len, seed, scheme):
@@ -451,8 +579,14 @@ def pack_archive(chains, shapes, excess_state_len, seed, scheme):
 def unpack_archive(a):
     """Inverse of pack_archive: (words uint32, offsets int64 [K+1], heads uint64 [K], nblocks int64 [K], shapes int64 [N, 2],
     excess_state_len, seed, scheme), chain k's words being words[offsets[k]:offsets[k+1]].  Every field is checked here,
-    before anything is sized from it: a truncated or inconsistent archive is a ValueError."""
-    a = np.asarray(a, dtype=np.uint32)
+    before anything is sized from it: a truncated or inconsistent archive is a ValueError.  A stamped archive is accepted:
+    its stamp is checked, must agree with the header's scheme and initial state, and is stripped."""
+    return _unpack_archive(a)[:-1]
+
+
+def _unpack_archive(a):
+    """unpack_archive's tuple and the archive's Stamp (or None)."""
+    a, stamp = _split_stamp(np.asarray(a, dtype=np.uint32))
     if a.ndim != 1 or a.size < 6 or int(a[-1]) != ARCHIVE_MARK:
         raise ValueError("not an archive: it must be a 1-D uint32 array ending in ARCHIVE_MARK")
     k, n, n_init, seed, scheme = (int(v) for v in a[-6:-1])
@@ -478,36 +612,40 @@ def unpack_archive(a):
         raise ValueError(f"archive: excess_state_len {n_init} outside [2, {MAX_INITIAL_WORDS}]")
     if scheme not in (BITSWAP, BBANS):
         raise ValueError(f"archive: unknown scheme {scheme}")
+    if stamp is not None and (stamp.scheme, stamp.excess_state_len, stamp.seed) != (scheme, n_init, seed):
+        raise ValueError(f"archive: the stamp's scheme, excess_state_len and seed "
+                         f"{(stamp.scheme, stamp.excess_state_len, stamp.seed)} disagree with the header's {(scheme, n_init, seed)}")
+    if stamp is not None and stamp.hwc_quirk:
+        raise ValueError("archive: the stamp has hwc_quirk set, which archives never use")
     offsets = np.zeros(k + 1, dtype=np.int64)
     np.cumsum(nwords, out=offsets[1:])
     heads = (table[:, 2].astype(np.uint64) << np.uint64(32)) | table[:, 1].astype(np.uint64)
-    return a[:body], offsets, heads, nblocks, shapes, n_init, seed, scheme
+    return a[:body], offsets, heads, nblocks, shapes, n_init, seed, scheme, stamp
 
 
 def _archive_job(a):
-    words, offsets, heads, nblocks, shapes, n_init, seed, scheme = unpack_archive(a)
+    words, offsets, heads, nblocks, shapes, n_init, seed, scheme, stamp = _unpack_archive(a)
     ioff = np.zeros(len(shapes) + 1, dtype=np.int64)
     np.cumsum(-(-shapes[:, 0] // 32) * -(-shapes[:, 1] // 32), out=ioff[1:])
     job = _Job([words[offsets[k]:offsets[k + 1]] for k in range(len(heads))], heads, np.cumsum(nblocks) - nblocks, nblocks,
                [(int(h), int(w)) for h, w in shapes], ioff)
-    return job, n_init, seed, scheme
+    return job, n_init, seed, scheme, stamp
 
 
-def compress_archive(codec, images, chain_blocks=64, scheme=BITSWAP, excess_state_len=10000, seed=100, words_per_block=1400):
+def compress_archive(codec, images, chain_blocks=64, scheme=BITSWAP, excess_state_len=10000, seed=100, words_per_block=1400,
+                     stamp=False):
     """images: a sequence of HWC uint8 arrays of any sizes (H, W >= 1, C = the model's) -> one np.uint32 archive.
     Each image is tiled as compress_images(edges="code") tiles it; the row-major blocks of all images, in the order given,
     form one sequence, cut into chain_sizes(total blocks, chain_blocks) contiguous runs, each coded as a chain from the seeded
     initial state.  A chain may start or end inside an image, so the initial words are paid once per chain, not once per
-    image.  chain_blocks None: one chain over everything (the reference's experiment layout, cifar_compress.py)."""
+    image.  chain_blocks None: one chain over everything (the reference's experiment layout, cifar_compress.py).
+    stamp=True: the archive is followed by a stamp of codec.fingerprint() and these arguments (module docstring), which
+    decompress_archive checks; the archive before it is unchanged."""
     chain_blocks = _check_chain_blocks(chain_blocks)
     images = [np.asarray(im) for im in images]
     if not images:
         raise ValueError("an archive holds at least one image")
-    if scheme not in (BITSWAP, BBANS):
-        raise ValueError(f"scheme must be BITSWAP or BBANS, got {scheme!r}")
-    for name, v, lo, hi in (("excess_state_len", excess_state_len, 2, MAX_INITIAL_WORDS), ("seed", seed, 0, (1 << 32) - 1)):
-        if isinstance(v, bool) or not isinstance(v, numbers.Integral) or not lo <= v <= hi:
-            raise ValueError(f"{name} must be an int in [{lo}, {hi}], got {v!r}")
+    _check_stamp_args(scheme, excess_state_len, seed)
     C = codec.cfg.xs[0]
     for i, im in enumerate(images):
         if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != C or im.shape[0] < 1 or im.shape[1] < 1:
@@ -521,9 +659,11 @@ def compress_archive(codec, images, chain_blocks=64, scheme=BITSWAP, excess_stat
     sizes = chain_sizes(total, chain_blocks)
     chains = list(zip(np.cumsum([0] + sizes[:-1]).tolist(), sizes))
     blocks = np.concatenate([_blocks_to_model(t[0], False) for t in tiled])
+    tail = _stamp_words(codec.fingerprint(), scheme, False, int(excess_state_len), int(seed)) if stamp else None
     coded = _encode(codec, blocks, np.concatenate([t[1] for t in tiled]), chains, scheme, int(excess_state_len), int(seed),
                     words_per_block)
-    return pack_archive(coded, [(t[2], t[3]) for t in tiled], int(excess_state_len), int(seed), scheme)
+    a = pack_archive(coded, [(t[2], t[3]) for t in tiled], int(excess_state_len), int(seed), scheme)
+    return a if tail is None else np.concatenate([a, tail])
 
 
 def plan_archive(archive, regions=None):
@@ -537,10 +677,13 @@ def decompress_archive(codec, archive, regions=None):
     """regions None -> every image of the archive, exactly as given; else a list of (i, y, x, h, w) over image i -> one HWC
     uint8 array per region, byte-identical to the crop of the full decode.  Each chain holding a wanted block is popped
     from its end down to the earliest wanted block in it (plan_archive).  Every chain popped down to its first block must
-    come back to the seeded initial state it was coded from; otherwise ValueError naming the chain."""
-    job, n_init, seed, scheme = _archive_job(archive)
+    come back to the seeded initial state it was coded from; otherwise ValueError naming the chain.  A stamped archive must
+    match the codec's fingerprint (ValueError naming every field that differs, before any decoding)."""
+    job, n_init, seed, scheme, stamp = _archive_job(archive)
     regions = _all_images(job) if regions is None else regions
-    return _decode_regions(codec, job, regions, None, scheme, False, None, initial=initial_words(n_init, seed=seed))
+    _check_stamps(codec, [stamp], scheme, False, None, "archive")
+    return _decode_regions(codec, job, regions, None, scheme, False, None,
+                           initial=[initial_words(n_init, seed=seed)] * len(job.cnb))
 
 
 def _all_images(job):

@@ -188,6 +188,24 @@ extern "C" int bsw_codec_set_coder(bsw_codec *c, int coder) {
     return BSW_OK;
 }
 
+extern "C" int bsw_codec_fingerprint(bsw_codec *c, bsw_fingerprint *out, void *stream) {
+    BSW_REQUIRE(c && out, "bsw_codec_fingerprint: null argument");
+    const bsw_model_desc &d = c->m->d;
+    bsw_fingerprint f = {};
+    f.revision = BSW_BITSTREAM_REVISION;
+    f.xc = d.xc; f.nz = d.nz; f.zchannels = d.zchannels; f.nprocessing = d.nprocessing; f.kernel_size = d.kernel_size;
+    f.resdepth = d.resdepth; f.reswidth = d.reswidth; f.cond_xscale = d.cond_xscale;
+    f.quantbits = c->q;
+    f.use_tensor_cores = d.use_tensor_cores;
+    f.tc_precision = c->m->tc_precision;
+    f.tc_heads = bsw_model_tc_heads(c->m);
+    f.coder = c->coder;
+    if (int rc = bsw_model_digest(c->m, f.model_digest, stream)) return rc;
+    if (int rc = bsw_bins_digest(c->b, f.bins_digest, stream)) return rc;
+    *out = f;
+    return BSW_OK;
+}
+
 // Per-category kernel timing for bench.py's roofline (CUDA events on the launching stream).
 extern "C" int bsw_codec_profile(bsw_codec *c, int enable, double *ms_out, int64_t *n_out) {
     BSW_REQUIRE(c, "null codec");

@@ -387,6 +387,7 @@ extern "C" int bsw_model_load_conv(bsw_model *m, const char *prefix, const float
     BSW_CUDA(cudaMemcpy(s.w, s.host_w.data(), sizeof(float) * s.host_w.size(), cudaMemcpyHostToDevice));
     BSW_CUDA(cudaMemcpy(s.bias, s.host_b.data(), sizeof(float) * s.host_b.size(), cudaMemcpyHostToDevice));
     s.loaded_mask |= (co_off == 0) ? 1 : 2;
+    m->digest_ok = false;
     return BSW_OK;
 }
 
@@ -401,6 +402,7 @@ extern "C" int bsw_model_load_gen_std(bsw_model *m, const float *gen_std) {
     }
     BSW_CUDA(cudaMemcpy(m->xscale, sc.data(), sizeof(float) * m->xdim, cudaMemcpyHostToDevice));
     m->have_gen_std = true;
+    m->digest_ok = false;
     return BSW_OK;
 }
 
@@ -458,6 +460,13 @@ static bool net_on_tc(const bsw_model *m) { return m->d.use_tensor_cores && m->t
 static bool in_writes_planes(const bsw_model *m, const NetPlan &np) { return net_on_tc(m) && !np.blocks.empty(); }
 static bool head_on_tc(bsw_model *m, const NetPlan &np) {
     return in_writes_planes(m, np) && bsw_conv_tc_head_available(m, m->convs[np.head]);
+}
+// 1 if any net's head runs on the tensor cores (part of the codec fingerprint: BSW_TC_HEADS=0 changes mu/sigma)
+int bsw_model_tc_heads(bsw_model *m) {
+    for (const auto *nets : {&m->infer, &m->gen})
+        for (const NetPlan &np : *nets)
+            if (head_on_tc(m, np)) return 1;
+    return 0;
 }
 
 // Runs one conv of net `np` in its role: the one place that picks its kernel(s).  `a` holds the input, the epilogue and,

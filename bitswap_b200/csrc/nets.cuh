@@ -59,6 +59,8 @@ struct bsw_model {
     int tc_precision = BSW_TC_SPLIT; // arithmetic of the tensor-core convs (bsw_model_set_tc_precision)
     void *tc_state = nullptr;        // owned by conv_tc.cu
     void *tc_slots = nullptr;
+    bool digest_ok = false;          // digest holds bsw_model_digest of the weights loaded now (digest.cu)
+    uint32_t digest[4];
 };
 
 // Per-kernel-category device timing (CUDA events on the launching stream), used by bench.py's roofline.
@@ -106,6 +108,7 @@ int bsw_model_tc_prepare(bsw_model *m);
 void bsw_model_tc_release(bsw_model *m);
 int bsw_conv_tc(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t n, cudaStream_t st);
 bool bsw_conv_tc_head_available(bsw_model *m, const ConvSlot &c);
+int bsw_model_tc_heads(bsw_model *m);
 int bsw_conv_tc_head(bsw_model *m, const ConvSlot &c, const ConvArgs &a, int64_t n, cudaStream_t st);
 int bsw_tc_split(bsw_model *m, const float *in, int which, int64_t n, cudaStream_t st);
 void bsw_tc_planes(bsw_model *m, int which, void **hi, void **lo);

@@ -14,7 +14,7 @@ import ctypes
 import numpy as np
 import torch
 
-from ._lib import lib, check, cuda_stream_ptr, device_index, on_device
+from ._lib import lib, check, cuda_stream_ptr, device_index, digest_hex, on_device
 from .config import CodecConfig
 from .synthetic import state_dict_spec
 
@@ -89,6 +89,16 @@ class Model:
     @property
     def handle(self):
         return self._h
+
+    def digest(self):
+        """Digest of the folded weights the kernels read (bsw_model_digest), 32 hex digits: equal for every instance of
+        one state dict, whatever its max_batch, conv path or tc_precision.  Computed once per loaded handle, so
+        load_state_dict() and to(), which re-create it, start afresh."""
+        assert self._loaded, "load_state_dict() first"
+        out = (ctypes.c_uint32 * 4)()
+        with on_device(self.device):
+            check(lib().bsw_model_digest(self._h, out, cuda_stream_ptr()))
+        return digest_hex(out)
 
     @property
     def tc_precision(self):

@@ -391,6 +391,58 @@ int bsw_codec_set_coder(bsw_codec *c, int coder);
  * pop_x, push_x, prior, rows_z, rows_x} (rows_* = phase A of the two-phase coder; pop/push = phase B).  enable: 1 = reset and start, 0 = reset and stop, -1 = read only.  Synchronises. */
 int bsw_codec_profile(bsw_codec *c, int enable, double *ms_out, int64_t *n_out);
 
+/* ------------------------------------------------------------------------------------------------
+ * Digests and the codec fingerprint (digest.cu): what a stored bitstream records about the codec that made it, so that a
+ * decoder can refuse a bitstream it would decode into wrong pixels.  The digests catch accidental mismatches (another
+ * checkpoint, other bins, a one-ulp difference in one weight); they are NOT cryptographic and do not resist tampering.
+ *
+ * bsw_digest: a 128-bit digest of `bytes` bytes at `dev` (device memory, 8-byte aligned), defined with integer operations
+ * only, so it does not depend on the grid, the device or the batch:
+ *   - the bytes are zero-padded to a multiple of 8 and read as little-endian uint64 words w[0 .. n);
+ *   - chunk c holds words [8192 c, min(8192 (c + 1), n)); in it, lane l (0..31) starts from a = mix(64 c + 2 l),
+ *     b = mix(64 c + 2 l + 1) and takes words 8192 c + l, + 32, + 64, ... in order:
+ *         a = rotl(a ^ w, 29) * 0x9E3779B97F4A7C15,   b = (rotl(b, 23) + w) * 0xC2B2AE3D27D4EB4F;
+ *   - the chunk's hash is ha = mix(c ^ 0x5354414D50484131), hb = mix(c + 0x5354414D50484232), then for l = 0 .. 31 in
+ *     order ha = mix(ha ^ a_l), hb = mix(hb + b_l);
+ *   - the digest starts from da = mix(bytes ^ 0x4449474553544131), db = mix(bytes + 0x4449474553544232) and folds the
+ *     chunks in order: da = mix(da ^ ha_c), db = mix(db + hb_c);  out4 = {lo(da), hi(da), lo(db), hi(db)}.
+ *   mix is the splitmix64 finaliser (z ^= z >> 30; z *= 0xBF58476D1CE4E5B9; z ^= z >> 27; z *= 0x94D049BB133111EB;
+ *   z ^= z >> 31), arithmetic mod 2^64.  Every step is a bijection of the word it takes, so a change of one word always
+ *   changes the digest.  Enqueued on `stream`; synchronises.
+ * bsw_model_digest: the digest of the folded model the kernels read: the descriptor (xc, nz, zchannels, nprocessing,
+ *   kernel_size, resdepth, reswidth, cond_xscale: not max_batch, not use_tensor_cores), then every conv slot in slot order
+ *   (Cin, Cout, ks, CinP, CoutP, parts, the digests of its float32 weights w [taps][CinP][CoutP] and bias [CoutP]), then,
+ *   without a conditional x-scale head, the digest of the folded x-scale [xdim].  The bf16 hi/lo planes are a function of
+ *   w and are left out, as are activations.  Needs a finalized model; computed once and kept until a weight is reloaded.
+ * bsw_bins_digest: the digest of (quantbits, nz, zdim) and of the padded z endpoints, the z centres and the x endpoints as
+ *   stored on the device.  Computed once (bin tables are immutable).
+ * ---------------------------------------------------------------------------------------------- */
+/* Bump whenever a change alters mu/sigma or the integer tables under settings that exist already: bitstreams written by
+ * an older revision then no longer match the codec, and stamped ones are refused instead of decoding into wrong pixels. */
+#define BSW_BITSTREAM_REVISION 1
+int bsw_bitstream_revision(void);
+int bsw_digest(const void *dev, int64_t bytes, uint32_t out4[4], void *stream);
+int bsw_model_digest(bsw_model *m, uint32_t out4[4], void *stream);
+int bsw_bins_digest(bsw_bins *b, uint32_t out4[4], void *stream);
+
+/* Everything that decides a codec's bitstreams.  Settings the parity tests show to be result-neutral are not in it: the
+ * conv mode bits, the rows mode, the k_rows6 lanes per row and verify mode, two-phase vs fused reference coder, dual stream,
+ * PipelinedCodec lanes and max_batch (see bsw_set_conv_mode, bsw_set_rows_mode, bsw_rows6_set_lanes_per_row,
+ * bsw_codec_set_two_phase, bsw_codec_set_dual_stream). */
+typedef struct {
+    int32_t revision;                   /* BSW_BITSTREAM_REVISION of the library */
+    int32_t xc, nz, zchannels, nprocessing, kernel_size, resdepth, reswidth, cond_xscale;   /* the model descriptor */
+    int32_t quantbits;
+    int32_t use_tensor_cores;           /* conv path: 1 = tensor cores, 0 = float32 SIMT */
+    int32_t tc_precision;               /* BSW_TC_SPLIT / BSW_TC_BF16 (BSW_TC_SPLIT on a SIMT model) */
+    int32_t tc_heads;                   /* 1 if any head runs on the tensor cores (0 with BSW_TC_HEADS=0) */
+    int32_t coder;                      /* BSW_CODER_REFERENCE / BSW_CODER_DIRECT */
+    uint32_t model_digest[4];           /* bsw_model_digest */
+    uint32_t bins_digest[4];            /* bsw_bins_digest */
+} bsw_fingerprint;
+/* The codec as it is now (the coder it was last set to).  Synchronises the first time the digests are computed. */
+int bsw_codec_fingerprint(bsw_codec *c, bsw_fingerprint *out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
