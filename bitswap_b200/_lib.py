@@ -158,6 +158,8 @@ def _set_argtypes(L):
         "bsw_model_digest": [P, P, P],
         "bsw_bins_digest": [P, P, P],
         "bsw_codec_fingerprint": [P, P, P],
+        "bsw_tile_blocks": [P, I, I, I, P, P, I, L64, P, P, P],
+        "bsw_untile_regions": [P, I, I, I, P, P, I, I, L64, P, P, I, P, P],
     }
     for name, args in sig.items():
         fn = getattr(L, name, None)
@@ -175,7 +177,8 @@ EXPORTS = ["bsw_last_error", "bsw_version", "bsw_has_tensor_cores", "bsw_measure
            "bsw_model_finalize", "bsw_model_set_tc_precision", "bsw_vae_infer", "bsw_vae_generate", "bsw_codec_create", "bsw_codec_destroy",
            "bsw_codec_encode", "bsw_codec_decode", "bsw_codec_encode_ext", "bsw_codec_decode_ext", "bsw_codec_last_launches", "bsw_codec_profile", "bsw_codec_set_two_phase", "bsw_codec_set_dual_stream", "bsw_codec_set_coder",
            "bsw_discretize_reset", "bsw_discretize_sample", "bsw_discretize_fold", "bsw_discretize_edges",
-           "bsw_bitstream_revision", "bsw_digest", "bsw_model_digest", "bsw_bins_digest", "bsw_codec_fingerprint"]
+           "bsw_bitstream_revision", "bsw_digest", "bsw_model_digest", "bsw_bins_digest", "bsw_codec_fingerprint",
+           "bsw_tile_blocks", "bsw_untile_regions"]
 
 
 def device_index(device=None):

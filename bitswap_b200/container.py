@@ -57,6 +57,7 @@ import numbers
 import numpy as np
 import torch
 
+from ._lib import check, cuda_stream_ptr, lib, on_device
 from .codec import BBANS, BITSWAP, CODERS, Fingerprint
 from .model import TC_PRECISIONS
 from .streams import StreamSet
@@ -211,11 +212,6 @@ def _blocks_to_model(blocks, hwc_quirk):
     return blocks.reshape(n, c, bh, bw) if hwc_quirk else blocks.transpose(0, 3, 1, 2)
 
 
-def _model_to_blocks(x, hwc_quirk):
-    n, c, bh, bw = x.shape
-    return np.ascontiguousarray(x).reshape(n, bh, bw, c) if hwc_quirk else np.ascontiguousarray(x.transpose(0, 2, 3, 1))
-
-
 def chain_sizes(nblocks, chain_blocks=None):
     """Block counts of the chains an image of `nblocks` row-major blocks is coded as, in block order: K = ceil(nblocks /
     chain_blocks) contiguous runs whose sizes differ by at most one, larger runs first.  None, or chain_blocks >= nblocks:
@@ -247,9 +243,128 @@ def _active(nblk):
     return np.searchsorted(-np.asarray(nblk), -np.arange(max(nblk)), side="left")
 
 
+# bsw_image_view and the tiling modes of bsw_tile_blocks / bsw_untile_regions (include/bitswap_b200.h)
+_VIEW = np.dtype([("pixels", "<u8"), ("h", "<i4"), ("w", "<i4"), ("sy", "<i8"), ("sx", "<i8"), ("sc", "<i8")])
+TILE_CROP, TILE_CODE, TILE_QUIRK = 0, 1, 2
+
+
+def _is_cuda(x):
+    return torch.is_tensor(x) and x.is_cuda
+
+
+def _grid(shapes, mode):
+    """Block grid (gh, gw) int64 [N] of images of these (h, w) [N, 2]: floor in crop and quirk mode, ceil in code mode."""
+    h, w = shapes[:, 0], shapes[:, 1]
+    return (-(-h // 32), -(-w // 32)) if mode == TILE_CODE else (h // 32, w // 32)
+
+
+class _Blocks:
+    """The block sequence of a writer call, still as the images it was given: the tile kernel lays it out on the device
+    (_tile).  images: a list of HWC arrays, CPU tensors or CUDA tensors, or one [N, H, W, C] array or tensor.  CUDA images
+    are checked here, before any device work (ValueError); host images too when `strict`, else as far as tiling needs.
+    np.asarray of it is the same sequence by the reference tiling, [n, C, 32, 32] in the model's layout."""
+
+    def __init__(self, codec, images, mode, strict):
+        C = codec.cfg.xs[0]
+        side = 1 if mode == TILE_CODE else 32
+        self.mode = mode
+        self.batch = (torch.is_tensor(images) or isinstance(images, np.ndarray)) and images.ndim == 4
+        if self.batch:
+            self.images = images if _is_cuda(images) else np.asarray(images)
+            n, H, W = self.images.shape[:3]
+            if _is_cuda(images):
+                _check_cuda_image(codec, "images", images[0] if n else images.reshape(-1), C, side)
+            elif strict:
+                _check_host_image("images", self.images[0] if n else self.images.reshape(-1), C)
+            self.shapes = np.tile(np.array([[H, W]], dtype=np.int64), (n, 1))
+            self.C = int(self.images.shape[3])
+            return
+        self.images = [im if _is_cuda(im) else np.asarray(im) for im in images]
+        for i, im in enumerate(self.images):
+            if _is_cuda(im):
+                _check_cuda_image(codec, f"image {i}", im, C, side)
+            elif strict:
+                _check_host_image(f"image {i}", im, C)
+            elif im.ndim != 3:
+                raise ValueError(f"image {i}: expected an H x W x C array, got shape {im.shape}")
+        chans = {int(im.shape[2]) for im in self.images}
+        if len(chans) > 1:
+            raise ValueError(f"the images have different channel counts {sorted(chans)}")
+        self.C = chans.pop() if chans else C
+        self.shapes = np.array([im.shape[:2] for im in self.images], dtype=np.int64).reshape(-1, 2)
+
+    def views(self, codec):
+        """(bsw_image_view records on the codec's device, the tensors they point into).  Host images go up as one flat
+        copy on the current stream."""
+        dev = torch.device("cuda", codec.device)
+        v = np.zeros(len(self.shapes), dtype=_VIEW)
+        v["h"], v["w"] = self.shapes[:, 0], self.shapes[:, 1]
+        if self.batch:
+            t = self.images if _is_cuda(self.images) else torch.from_numpy(np.ascontiguousarray(self.images, np.uint8)).to(dev)
+            s0, v["sy"], v["sx"], v["sc"] = t.stride()
+            v["pixels"] = np.uint64(t.data_ptr()) + np.uint64(s0) * np.arange(len(v), dtype=np.uint64)
+            return v, [t]
+        keep = []
+        host = [k for k, im in enumerate(self.images) if not _is_cuda(im)]
+        if host:
+            t = torch.from_numpy(np.concatenate([np.ascontiguousarray(self.images[k], np.uint8).reshape(-1) for k in host])).to(dev)
+            keep.append(t)
+            n = self.shapes[host, 0] * self.shapes[host, 1] * self.C
+            v["pixels"][host] = np.uint64(t.data_ptr()) + (np.cumsum(n) - n).astype(np.uint64)
+            v["sy"][host], v["sx"][host], v["sc"][host] = self.shapes[host, 1] * self.C, self.C, 1
+        for k, im in enumerate(self.images):
+            if _is_cuda(im):
+                v[k] = (im.data_ptr(), im.shape[0], im.shape[1]) + tuple(im.stride())
+                keep.append(im)
+        return v, keep
+
+    def __array__(self, dtype=None, copy=None):
+        ims = [np.asarray(im.cpu()) if torch.is_tensor(im) else np.asarray(im) for im in self.images]
+        tiles = [extract_edge_blocks(im)[0] if self.mode == TILE_CODE else extract_blocks(im)[0] for im in ims]
+        a = np.concatenate([_blocks_to_model(t, self.mode == TILE_QUIRK) for t in tiles])
+        return a if dtype is None else a.astype(dtype)
+
+
+def _check_cuda_image(codec, what, t, C, side):
+    if (t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != C or t.shape[0] < side or t.shape[1] < side
+            or t.device.index != codec.device):
+        raise ValueError(f"{what}: expected an H x W x {C} uint8 CUDA tensor on cuda:{codec.device} with H, W >= {side}, "
+                         f"got {t.dtype} {tuple(t.shape)} on {t.device}")
+    if np.prod(block_grid(*t.shape[:2])) > MAX_BLOCKS:
+        raise ValueError(f"{what} of {t.shape[0]} x {t.shape[1]} has more than {MAX_BLOCKS} blocks")
+
+
+def _check_host_image(what, im, C):
+    if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != C or im.shape[0] < 1 or im.shape[1] < 1:
+        raise ValueError(f"{what}: expected an H x W x {C} uint8 array with H, W >= 1, got {im.dtype} {im.shape}")
+    if np.prod(block_grid(*im.shape[:2])) > MAX_BLOCKS:
+        raise ValueError(f"{what} of {im.shape[0]} x {im.shape[1]} has more than {MAX_BLOCKS} blocks")
+
+
+def _sequence_extents(shapes):
+    """int16 [n, 2]: block_extents of images of these (h, w) in turn, without a step per image."""
+    gh, gw = _grid(shapes, TILE_CODE)
+    nb = gh * gw
+    img = np.repeat(np.arange(len(nb)), nb)
+    b = np.arange(int(nb.sum())) - np.repeat(np.cumsum(nb) - nb, nb)
+    by, bx = b // gw[img], b % gw[img]
+    return np.stack([np.minimum(32, shapes[img, 0] - 32 * by), np.minimum(32, shapes[img, 1] - 32 * bx)], -1).astype(np.int16)
+
+
+def _chain_runs(nb, chain_blocks):
+    """chain_sizes of every image of nb blocks, without a step per image: (chains per image, block counts in turn)."""
+    k = np.ones_like(nb) if chain_blocks is None else np.where(chain_blocks >= nb, 1, -(-nb // chain_blocks))
+    img = np.repeat(np.arange(len(nb)), k)
+    pos = np.arange(int(k.sum())) - np.repeat(np.cumsum(k) - k, k)
+    q, r = nb // k, nb % k
+    return k, q[img] + (pos < r[img])
+
+
 def compress_images(codec, images, excess_state_len=10000, seed=100, scheme=BITSWAP, hwc_quirk=False, words_per_block=1400,
                     edges="crop", chain_blocks=None, stamp=False):
-    """images: list of HWC uint8 arrays.  Returns one container array per image.
+    """images: list of HWC uint8 images -- numpy arrays, CPU tensors, or CUDA tensors of any strides on the codec's device
+    -- or one [N, H, W, C] array or tensor.  Returns one container array per image (numpy uint32, the same bytes whatever
+    the images were held in).  The images are tiled into blocks on the device; host images go up in one copy.
     Every chain starts from the reference's initial state: `excess_state_len` random words drawn with
     np.random.seed(100) (demo_compress.py:113-115, :202).
     edges="crop" (the reference's behaviour): every image is cropped down to multiples of 32 and must be at least 32x32.
@@ -258,7 +373,9 @@ def compress_images(codec, images, excess_state_len=10000, seed=100, scheme=BITS
     chain_blocks: None (the reference's one chain per image) or a positive int L: an image of n > L blocks is coded as
     ceil(n / L) chains of contiguous blocks (chain_sizes), which run side by side.  Fewer serial steps, more initial bits.
     stamp=True: every container is followed by a stamp of codec.fingerprint() and these arguments (module docstring),
-    which decompress_images checks; the container before it is unchanged."""
+    which decompress_images checks; the container before it is unchanged.
+    A CUDA image that is not a uint8 H x W x C tensor with the codec's C, is on another device, or is empty (under 32 x 32
+    with edges="crop") is a ValueError before any device work."""
     if edges not in ("crop", "code"):
         raise ValueError(f"edges must be 'crop' or 'code', got {edges!r}")
     if edges == "code" and hwc_quirk:
@@ -267,24 +384,20 @@ def compress_images(codec, images, excess_state_len=10000, seed=100, scheme=BITS
     if stamp:
         _check_stamp_args(scheme, excess_state_len, seed)
         tail = _stamp_words(codec.fingerprint(), scheme, hwc_quirk, excess_state_len, seed)
-    images = [np.asarray(im) for im in images]
-    if edges == "code":
-        tiled = [extract_edge_blocks(im) for im in images]
-    else:
-        tiled = [(b, None, h, w) for b, h, w in (extract_blocks(im) for im in images)]
+    mode = TILE_CODE if edges == "code" else TILE_QUIRK if hwc_quirk else TILE_CROP
+    blocks = _Blocks(codec, images, mode, strict=False)
+    if not len(blocks.shapes):
+        raise ValueError("no images")
+    gh, gw = _grid(blocks.shapes, mode)
+    hw = blocks.shapes if mode == TILE_CODE else 32 * np.stack([gh, gw], -1)     # what the containers record
     # one block sequence of every image in turn; each image's chains are runs inside its own blocks
-    chains, off = [], 0
-    for t in tiled:
-        sizes = chain_sizes(t[0].shape[0], chain_blocks)
-        chains += [(off + s, nb) for s, nb in zip(np.cumsum([0] + sizes[:-1]).tolist(), sizes)]
-        off += t[0].shape[0]
-    blocks = np.concatenate([_blocks_to_model(t[0], hwc_quirk) for t in tiled])
-    extents = None if edges == "crop" else np.concatenate([t[1] for t in tiled])
+    per_image, sizes = _chain_runs(gh * gw, chain_blocks)
+    chains = list(zip((np.cumsum(sizes) - sizes).tolist(), sizes.tolist()))
+    extents = None if mode != TILE_CODE else _sequence_extents(blocks.shapes)
     coded = _encode(codec, blocks, extents, chains, scheme, excess_state_len, seed, words_per_block)
     out, k = [], 0
-    for t in tiled:
-        K = len(chain_sizes(t[0].shape[0], chain_blocks))
-        out.append(pack_container(coded[k:k + K], t[2], t[3]))
+    for K, (h, w) in zip(per_image.tolist(), hw.tolist()):
+        out.append(pack_container(coded[k:k + K], h, w))
         if stamp:
             out[-1] = np.concatenate([out[-1], tail])
         k += K
@@ -292,58 +405,60 @@ def compress_images(codec, images, excess_state_len=10000, seed=100, scheme=BITS
 
 
 def _encode(codec, blocks, extents, chains, scheme, excess_state_len, seed, words_per_block):
-    """Codes a block sequence (blocks [n, C, 32, 32] in model layout, extents int16 [n, 2] or None) as the chains (start,
-    nblocks) given, each a run of it, from the seeded initial state.  Returns [(words above the lowest depth, head,
-    nblocks)] in chain order.  Streams hold the chains largest first, so the active streams at each step are a prefix."""
-    order = sorted(range(len(chains)), key=lambda c: (-chains[c][1], c))
-    nblk = [chains[c][1] for c in order]
+    """Codes a block sequence (blocks: a _Blocks; extents int16 [n, 2] or None) as the chains (start, nblocks) given, each a
+    run of it, from the seeded initial state.  Returns [(words above the lowest depth, head, nblocks)] in chain order.
+    Streams hold the chains largest first, so the active streams at each step are a prefix."""
+    cnb = np.array([nb for _, nb in chains], dtype=np.int64)
+    order = np.argsort(-cnb, kind="stable")
+    nblk = cnb[order]
+    stream = np.empty(len(cnb), dtype=np.int32)
+    stream[order] = np.arange(len(cnb))
+    x, ext = _tile(codec, blocks, cnb, stream, int(nblk[0]), extents is not None and not (extents == 32).all())
     w, head = initial_words(excess_state_len, seed=seed)
     # capacity: `words_per_block` words per 32x32 block of the longest chain (1400 = 14.6 bits/dim; 8 bits/dim of raw pixels
     # is 768).  A chain that still overflows is retried with twice the room instead of failing after it was coded.
     for attempt in range(4):
-        ss = StreamSet(len(chains), excess_state_len + (words_per_block << attempt) * max(nblk) + 64, device=codec.device)
+        ss = StreamSet(len(cnb), excess_state_len + (words_per_block << attempt) * int(nblk[0]) + 64, device=codec.device)
         ss.fill(w, head)
         try:
-            return _compress_chains(codec, ss, blocks, extents, chains, order, nblk, scheme)
+            words, offs, heads = _compress_chains(codec, ss, x, ext, nblk, scheme)
         except OverflowError:
             if attempt == 3:
                 raise
+            continue
+        return [(words[offs[j]:offs[j + 1]], int(heads[j]), nb) for j, nb in zip(stream.tolist(), cnb.tolist())]
     raise AssertionError("unreachable")
 
 
-def _compress_chains(codec, ss, blocks, extents, chains, order, nblk, scheme):
-    n = len(order)
-    # all blocks to the device once: [step t, stream j] = block t of the j-th largest chain (CHW, demo_compress.py:120)
-    host = np.zeros((max(nblk), n) + blocks.shape[1:], dtype=np.uint8)
-    for j, c in enumerate(order):
-        s, nb = chains[c]
-        host[:nb, j] = blocks[s:s + nb]
-    dev = torch.from_numpy(host).to(torch.device("cuda", codec.device))
-    ext = _extents_to_device(codec, [None if extents is None else extents[s:s + nb] for s, nb in (chains[c] for c in order)],
-                             nblk)
+def _tile(codec, blocks, cnb, stream, steps, ragged):
+    """The coding buffer [step t, stream j, C, 32, 32] (block t of the chain on stream j; CHW, demo_compress.py:120) and,
+    when `ragged`, the int16 extents [t, j, 2], tiled on the device on the current stream (bsw_tile_blocks).  cnb: int64
+    block counts of the chains in sequence order; stream: int32, the stream of each chain."""
+    dev = torch.device("cuda", codec.device)
+    x = torch.empty((steps, len(cnb), blocks.C, 32, 32), dtype=torch.uint8, device=dev)
+    ext = torch.empty((steps, len(cnb), 2), dtype=torch.int16, device=dev) if ragged else None
+    if steps:
+        views, keep = blocks.views(codec)
+        with on_device(codec.device):
+            check(lib().bsw_tile_blocks(views.ctypes.data, len(views), blocks.C, blocks.mode, cnb.ctypes.data,
+                                        stream.ctypes.data, len(cnb), steps, x.data_ptr(),
+                                        None if ext is None else ext.data_ptr(), cuda_stream_ptr()))
+    return x, ext
+
+
+def _compress_chains(codec, ss, x, ext, nblk, scheme):
+    """Codes x [step, stream] onto the streams (nblk: their block counts, largest first) and reads back only the words above
+    each stream's lowest depth (the never-borrowed initial words stay, demo_compress.py:137,160): (words uint32, offsets
+    int64 [n + 1], heads uint64 [n]) in stream order."""
     active = _active(nblk)
-    for t in range(max(nblk)):
+    for t in range(int(nblk[0])):
         for b, cnt in _sub_ranges(int(active[t]), codec.max_batch):
-            codec.encode(ss, dev[t, b:b + cnt], first=b, scheme=scheme, extent=None if ext is None else ext[t, b:b + cnt])
+            codec.encode(ss, x[t, b:b + cnt], first=b, scheme=scheme, extent=None if ext is None else ext[t, b:b + cnt])
     torch.cuda.synchronize()
     ss.raise_on_error()
-    words, offs, heads, _ = ss.export()
-    lo = ss.min_words()                                       # never-borrowed initial words (demo_compress.py:137,160)
-    stream = np.empty(n, dtype=np.int64)
-    stream[order] = np.arange(n)
-    return [(words[offs[j] + lo[j]:offs[j + 1]], int(heads[j]), nb) for j, (_, nb) in zip(stream.tolist(), chains)]
-
-
-def _extents_to_device(codec, extents, nblk):
-    """[step t, stream j] block extents as one int16 device tensor, or None when every block is full (then the plain
-    calls run, which code exactly what full extents would)."""
-    if all(e is None or (e == 32).all() for e in extents):
-        return None
-    host = np.full((max(nblk), len(nblk), 2), 32, dtype=np.int16)
-    for j, e in enumerate(extents):
-        if e is not None:
-            host[:nblk[j], j] = e
-    return torch.from_numpy(host).to(torch.device("cuda", codec.device))
+    words_d, offs_d, heads_d, _ = ss.pack_device(trim=True)
+    offs = offs_d.cpu().numpy()
+    return words_d[:int(offs[-1])].cpu().numpy().view(np.uint32), offs, heads_d.cpu().numpy().view(np.uint64)
 
 
 def pack_container(chains, h, w):
@@ -474,31 +589,35 @@ def _stamped_job(codec, containers, channels, scheme, hwc_quirk):
     return _containers_job(parsed), initial if states else None
 
 
-def decompress_regions(codec, containers, regions, channels=3, scheme=BITSWAP, hwc_quirk=False, headroom_words=None):
+def decompress_regions(codec, containers, regions, channels=3, scheme=BITSWAP, hwc_quirk=False, headroom_words=None,
+                       as_tensors=False):
     """regions: list of (i, y, x, h, w) -> one HWC uint8 array per region, equal to decompress_images(...)[i][y:y+h, x:x+w].
     Only the chains holding a wanted block are imported, and each is popped only down to the earliest block any region on
     its container wants (plan_regions): a chain of n blocks whose earliest wanted block is j costs n - j block decodes.
     Blocks are row-major, so a window near an image's bottom is cheapest, and a single-chain container gains only there.
     A stamped container must match the codec's fingerprint, scheme, hwc_quirk and channels (ValueError naming every field
     that differs, before any decoding), and each of its chains popped down to its first block must come back to the
-    stamp's initial state."""
+    stamp's initial state.
+    as_tensors=True: contiguous torch.uint8 [h, w, C] tensors on the codec's device instead, the same pixels; no pixel
+    crosses PCIe.  Either way the regions are cut on the device and the decode is complete when this returns."""
     job, initial = _stamped_job(codec, containers, channels, scheme, hwc_quirk)
-    return _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_words, initial)
+    return _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_words, initial, as_tensors)
 
 
-def decompress_images(codec, containers, channels=3, scheme=BITSWAP, hwc_quirk=False, headroom_words=None):
+def decompress_images(codec, containers, channels=3, scheme=BITSWAP, hwc_quirk=False, headroom_words=None, as_tensors=False):
     """Inverse of compress_images: list of container arrays -> list of HWC uint8 images (the cropped size for a crop-mode
     container, the full size for an edge-coded one: a header whose h or w is not a multiple of 32).  Single- and
-    multi-chain containers can be mixed in one call, and so can stamped and unstamped ones (see decompress_regions)."""
+    multi-chain containers can be mixed in one call, and so can stamped and unstamped ones (see decompress_regions).
+    as_tensors=True: contiguous torch.uint8 [h, w, C] CUDA tensors on the codec's device instead of numpy arrays."""
     job, initial = _stamped_job(codec, containers, channels, scheme, hwc_quirk)
     return _decode_regions(codec, job, [(i, 0, 0, h, w) for i, (h, w) in enumerate(job.shapes)], channels, scheme,
-                           hwc_quirk, headroom_words, initial)
+                           hwc_quirk, headroom_words, initial, as_tensors)
 
 
-def _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_words, initial=None):
+def _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_words, initial=None, as_tensors=False):
     """Decodes the job's regions.  channels None: the codec's.  initial: per chain, None or the seeded initial state
     (words, head) it started from; such a chain popped down to its first block must then hold its top words and head, or
-    ValueError."""
+    ValueError.  as_tensors: CUDA tensors instead of numpy arrays."""
     regions, plan = _plan(job, regions)
     if not regions:
         return []
@@ -507,7 +626,7 @@ def _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_w
     cstart, cnb = job.cstart, job.cnb
     order = np.argsort(-plan.depth, kind="stable")[:np.count_nonzero(plan.depth)]  # streams: deepest first, skipped ones out
     pieces = [job.pieces[c] for c in order]
-    depth = plan.depth[order].tolist()
+    depth = plan.depth[order]
     n = len(depth)
     # The receiver pushes too (it returns the borrowed bits, cifar_compress.py:306-313): one block's worth of latents,
     # nz * zdim symbols at <= 31 bits each, can sit on the stack above the chain's own length.
@@ -519,35 +638,54 @@ def _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_w
     ss.import_packed(np.concatenate(pieces), offs, job.heads[order])
     # Steps are aligned at the chains' ends: step s pops block n - 1 - s of every stream deeper than s, so the active
     # streams stay a prefix and [s, stream] holds that block, in the output and in the extents alike.
-    dev = torch.empty((max(depth), n, channels, 32, 32), dtype=torch.uint8, device=torch.device("cuda", codec.device))
-    extents = np.concatenate([block_extents(h, w) for h, w in job.shapes])
-    ext = _extents_to_device(codec, [extents[s + nb - d:s + nb][::-1] for s, nb, d in zip(cstart[order], cnb[order], depth)],
-                             depth)
+    dev = torch.empty((int(depth[0]), n, channels, 32, 32), dtype=torch.uint8, device=torch.device("cuda", codec.device))
+    ext = _decode_extents(codec, job, (cstart + cnb)[order], depth)
     active = _active(depth)
-    for s in range(max(depth)):
+    for s in range(int(depth[0])):
         for b, cnt in _sub_ranges(int(active[s]), codec.max_batch):
             codec.decode(ss, cnt, first=b, scheme=scheme, out=dev[s, b:b + cnt],
                          extent=None if ext is None else ext[s, b:b + cnt])
     if hasattr(codec, "join"):                                             # (free-running multi-lane codec: lanes -> current stream)
         codec.join()
-    # the needed blocks, gathered on the device into one transfer; pos[b]: block b's row in it
-    stream = np.full(len(cnb), -1, dtype=np.int64)
+    stream = np.full(len(cnb), -1, dtype=np.int32)
     stream[order] = np.arange(n)
-    b = np.flatnonzero(plan.needed)
-    c = np.searchsorted(cstart + cnb, b, side="right")
-    pos = np.full(plan.needed.size, -1, dtype=np.int64)
-    pos[b] = np.arange(b.size)
-    idx = torch.from_numpy((cstart[c] + cnb[c] - 1 - b) * n + stream[c]).to(dev.device)
-    host = _model_to_blocks(dev.view(-1, channels, 32, 32).index_select(0, idx).cpu().numpy(), hwc_quirk)
-    ss.raise_on_error()
+    out = _untile(codec, job, regions, stream, dev, TILE_QUIRK if hwc_quirk else TILE_CODE)
+    ss.raise_on_error()                                                    # (synchronises the device)
     if initial is not None:
         _check_initial_state(ss, order, plan.first[order] == 0, initial)
-    out = []
-    for i, y, x, h, w in regions:
-        gw = block_grid(*job.shapes[i])[1]
-        by, bx = np.arange(y // 32, (y + h - 1) // 32 + 1), np.arange(x // 32, (x + w - 1) // 32 + 1)
-        tile = unextract_blocks(host[pos[job.ioff[i] + by[:, None] * gw + bx[None, :]].reshape(-1)], 32 * by.size, 32 * bx.size)
-        out.append(np.ascontiguousarray(tile[y - 32 * by[0]:y - 32 * by[0] + h, x - 32 * bx[0]:x - 32 * bx[0] + w]))
+    size = np.array([h * w * channels for _, _, _, h, w in regions], dtype=np.int64)
+    start = (np.cumsum(size) - size).tolist()
+    if not as_tensors:
+        out = out.cpu().numpy()
+    return [out[o:o + m].view(h, w, channels) if as_tensors else out[o:o + m].reshape(h, w, channels)
+            for o, m, (_, _, _, h, w) in zip(start, size.tolist(), regions)]
+
+
+def _decode_extents(codec, job, cend, depth):
+    """[step s, stream j] int16 extents of block cend_j - 1 - s on the device, or None when every decoded block is full (then
+    the plain calls run, which code exactly what full extents would).  Rows past a stream's depth hold (32, 32)."""
+    s = np.arange(int(depth[0]))[:, None]
+    live = s < depth[None, :]
+    seq = _sequence_extents(np.asarray(job.shapes, dtype=np.int64).reshape(-1, 2))
+    host = np.where(live[..., None], seq[np.where(live, cend[None, :] - 1 - s, 0)], np.int16(32))
+    if (host == 32).all():
+        return None
+    return torch.from_numpy(np.ascontiguousarray(host, dtype=np.int16)).to(torch.device("cuda", codec.device))
+
+
+def _untile(codec, job, regions, stream, x, mode):
+    """The regions cut out of the decoder's buffer x [step, stream, C, 32, 32] on the device, on the current stream
+    (bsw_untile_regions): one flat uint8 CUDA tensor holding each region as contiguous HWC, the regions in turn.  stream:
+    int32 per chain of the job, the stream that decoded it (-1: none)."""
+    shapes = np.ascontiguousarray(np.asarray(job.shapes, dtype=np.int64).reshape(-1, 2), dtype=np.int32)
+    regs = np.ascontiguousarray(regions, dtype=np.int32).reshape(-1, 5)
+    cnb = np.ascontiguousarray(job.cnb, dtype=np.int64)
+    C = x.shape[2]
+    out = torch.empty(int((regs[:, 3].astype(np.int64) * regs[:, 4]).sum()) * C, dtype=torch.uint8, device=x.device)
+    with on_device(codec.device):
+        check(lib().bsw_untile_regions(shapes.ctypes.data, len(shapes), C, mode, cnb.ctypes.data, stream.ctypes.data,
+                                       len(cnb), x.shape[1], x.shape[0], x.data_ptr(), regs.ctypes.data, len(regs),
+                                       out.data_ptr(), cuda_stream_ptr()))
     return out
 
 
@@ -634,7 +772,8 @@ def _archive_job(a):
 
 def compress_archive(codec, images, chain_blocks=64, scheme=BITSWAP, excess_state_len=10000, seed=100, words_per_block=1400,
                      stamp=False):
-    """images: a sequence of HWC uint8 arrays of any sizes (H, W >= 1, C = the model's) -> one np.uint32 archive.
+    """images: a sequence of HWC uint8 images of any sizes (H, W >= 1, C = the model's) -- numpy arrays, CPU tensors, or CUDA
+    tensors of any strides on the codec's device -- or one [N, H, W, C] array or tensor -> one np.uint32 archive.
     Each image is tiled as compress_images(edges="code") tiles it; the row-major blocks of all images, in the order given,
     form one sequence, cut into chain_sizes(total blocks, chain_blocks) contiguous runs, each coded as a chain from the seeded
     initial state.  A chain may start or end inside an image, so the initial words are paid once per chain, not once per
@@ -642,27 +781,22 @@ def compress_archive(codec, images, chain_blocks=64, scheme=BITSWAP, excess_stat
     stamp=True: the archive is followed by a stamp of codec.fingerprint() and these arguments (module docstring), which
     decompress_archive checks; the archive before it is unchanged."""
     chain_blocks = _check_chain_blocks(chain_blocks)
-    images = [np.asarray(im) for im in images]
-    if not images:
+    if not (torch.is_tensor(images) or isinstance(images, np.ndarray)):
+        images = list(images)
+    if not len(images):
         raise ValueError("an archive holds at least one image")
     _check_stamp_args(scheme, excess_state_len, seed)
-    C = codec.cfg.xs[0]
-    for i, im in enumerate(images):
-        if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != C or im.shape[0] < 1 or im.shape[1] < 1:
-            raise ValueError(f"image {i}: expected an H x W x {C} uint8 array with H, W >= 1, got {im.dtype} {im.shape}")
-        if np.prod(block_grid(*im.shape[:2])) > MAX_BLOCKS:
-            raise ValueError(f"image {i} of {im.shape[0]} x {im.shape[1]} has more than {MAX_BLOCKS} blocks")
-    tiled = [extract_edge_blocks(im) for im in images]
-    total = sum(t[0].shape[0] for t in tiled)
+    blocks = _Blocks(codec, images, TILE_CODE, strict=True)
+    gh, gw = _grid(blocks.shapes, TILE_CODE)
+    total = int((gh * gw).sum())
     if total > MAX_ARCHIVE_BLOCKS:
         raise ValueError(f"the images hold {total} blocks, an archive at most {MAX_ARCHIVE_BLOCKS}")
     sizes = chain_sizes(total, chain_blocks)
     chains = list(zip(np.cumsum([0] + sizes[:-1]).tolist(), sizes))
-    blocks = np.concatenate([_blocks_to_model(t[0], False) for t in tiled])
     tail = _stamp_words(codec.fingerprint(), scheme, False, int(excess_state_len), int(seed)) if stamp else None
-    coded = _encode(codec, blocks, np.concatenate([t[1] for t in tiled]), chains, scheme, int(excess_state_len), int(seed),
+    coded = _encode(codec, blocks, _sequence_extents(blocks.shapes), chains, scheme, int(excess_state_len), int(seed),
                     words_per_block)
-    a = pack_archive(coded, [(t[2], t[3]) for t in tiled], int(excess_state_len), int(seed), scheme)
+    a = pack_archive(coded, blocks.shapes, int(excess_state_len), int(seed), scheme)
     return a if tail is None else np.concatenate([a, tail])
 
 
@@ -673,17 +807,18 @@ def plan_archive(archive, regions=None):
     return _plan(job, _all_images(job) if regions is None else regions)[1]
 
 
-def decompress_archive(codec, archive, regions=None):
+def decompress_archive(codec, archive, regions=None, as_tensors=False):
     """regions None -> every image of the archive, exactly as given; else a list of (i, y, x, h, w) over image i -> one HWC
     uint8 array per region, byte-identical to the crop of the full decode.  Each chain holding a wanted block is popped
     from its end down to the earliest wanted block in it (plan_archive).  Every chain popped down to its first block must
     come back to the seeded initial state it was coded from; otherwise ValueError naming the chain.  A stamped archive must
-    match the codec's fingerprint (ValueError naming every field that differs, before any decoding)."""
+    match the codec's fingerprint (ValueError naming every field that differs, before any decoding).  as_tensors=True:
+    contiguous torch.uint8 [h, w, C] CUDA tensors on the codec's device instead of numpy arrays."""
     job, n_init, seed, scheme, stamp = _archive_job(archive)
     regions = _all_images(job) if regions is None else regions
     _check_stamps(codec, [stamp], scheme, False, None, "archive")
     return _decode_regions(codec, job, regions, None, scheme, False, None,
-                           initial=[initial_words(n_init, seed=seed)] * len(job.cnb))
+                           initial=[initial_words(n_init, seed=seed)] * len(job.cnb), as_tensors=as_tensors)
 
 
 def _all_images(job):

@@ -121,7 +121,9 @@ class StreamSet:
 
     # -- fast packed path: one gather/scatter kernel + three memcpys, pinned staging buffers -------------------------
     @_on_own_device
-    def _staging(self, count):
+    def _staging(self, count, host=True):
+        """Device staging buffers for `count` streams, and with host=True their pinned host twins (pack_device alone needs
+        none: a worst-case pinned buffer of count * capacity words is costly to create)."""
         import torch
         st = getattr(self, "_stg", None)
         need = count * self.capacity
@@ -129,12 +131,14 @@ class StreamSet:
             st = dict(words_d=torch.empty(need, dtype=torch.int32, device="cuda"),
                       offs_d=torch.empty(count + 1, dtype=torch.int64, device="cuda"),
                       heads_d=torch.empty(count, dtype=torch.int64, device="cuda"),
-                      base_d=torch.empty(count, dtype=torch.int32, device="cuda"),
-                      base_h=torch.empty(count, dtype=torch.int32).pin_memory(),
-                      words_h=torch.empty(need, dtype=torch.int32).pin_memory(),
-                      offs_h=torch.empty(count + 1, dtype=torch.int64).pin_memory(),
-                      heads_h=torch.empty(count, dtype=torch.int64).pin_memory())
+                      base_d=torch.empty(count, dtype=torch.int32, device="cuda"))
             self._stg = st
+        if host and "words_h" not in st:
+            n = st["offs_d"].numel() - 1
+            st.update(base_h=torch.empty(n, dtype=torch.int32).pin_memory(),
+                      words_h=torch.empty(st["words_d"].numel(), dtype=torch.int32).pin_memory(),
+                      offs_h=torch.empty(n + 1, dtype=torch.int64).pin_memory(),
+                      heads_h=torch.empty(n, dtype=torch.int64).pin_memory())
         return st
 
     @_on_own_device
@@ -146,7 +150,7 @@ class StreamSet:
         demo_compress.py:137,160)."""
         from ._lib import cuda_stream_ptr
         count = self.n - first if count is None else count
-        st = self._staging(count)
+        st = self._staging(count, host=False)
         if trim:
             check(lib().bsw_streams_pack_trimmed(self._h, first, count, st["words_d"].data_ptr(), st["offs_d"].data_ptr(),
                                                  st["heads_d"].data_ptr(), st["base_d"].data_ptr(), cuda_stream_ptr()))

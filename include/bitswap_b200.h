@@ -443,6 +443,50 @@ typedef struct {
 /* The codec as it is now (the coder it was last set to).  Synchronises the first time the digests are computed. */
 int bsw_codec_fingerprint(bsw_codec *c, bsw_fingerprint *out, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Images in and out of the codec's block buffers (tiles.cu): byte copies on the device, so that images can enter and leave
+ * as device memory and a host image crosses PCIe once, whole.
+ *
+ * A set of images is one block sequence: image i's blocks in row-major order over its block grid, the images in turn.  The
+ * grid of an h x w image is floor(h/32) x floor(w/32) in BSW_TILE_CROP and BSW_TILE_QUIRK (the image cut down to multiples
+ * of 32, every block full) and ceil(h/32) x ceil(w/32) in BSW_TILE_CODE (partial blocks at the bottom and right edges, valid
+ * extent (vh, vw) = (min(32, h - 32 by), min(32, w - 32 bx)), as bsw_codec_encode_ext codes them).  A block is stored CHW,
+ * [C][32][32]; BSW_TILE_QUIRK stores the block's HWC bytes [32][32][C] flat in the same C*1024 bytes instead.
+ *
+ * The sequence is cut into chains: chain_blocks_host[c] (int64 >= 0) blocks each, in sequence order, covering it exactly.
+ * A block buffer is [steps][n_streams][C][32][32] uint8.  The tables are host memory, sized by images, chains and regions;
+ * they are validated on the host before anything is uploaded or launched (BSW_E_INVALID, nothing enqueued), then copied
+ * to the device in one transfer on `stream`.  The pixel memory behind a pointer cannot be checked: the caller guarantees
+ * that every element the view addresses is readable device memory.
+ * ---------------------------------------------------------------------------------------------- */
+#define BSW_TILE_CROP  0
+#define BSW_TILE_CODE  1
+#define BSW_TILE_QUIRK 2
+#define BSW_MAX_IMAGE_BLOCKS (1 << 20)   /* blocks per image either call accepts */
+typedef struct {
+    const uint8_t *pixels;   /* device: pixel (y, x) channel c is pixels[y * sy + x * sx + c * sc] */
+    int32_t h, w;            /* >= 1 each, at most BSW_MAX_IMAGE_BLOCKS blocks */
+    int64_t sy, sx, sc;      /* element strides, any value >= 0 (0 repeats a row, column or channel) */
+} bsw_image_view;
+/* The encoder's input: row (t, j) of blocks_dev (n_streams = n_chains) receives block t of the chain c with
+ * chain_stream_host[c] == j (a permutation of [0, n_chains)), for t < chain_blocks_host[c] <= steps; rows past a chain's
+ * end are not written.  Pixels outside a block's extent are edge-replicated.  BSW_TILE_CODE with extents_dev non-NULL
+ * also writes int16 extents_dev[t][j] = (vh, vw) for the same rows.  1 <= channels <= 4; an image may have no blocks (crop
+ * mode under 32 x 32), and if no image has any, nothing is enqueued. */
+int bsw_tile_blocks(const bsw_image_view *images_host, int n_images, int channels, int mode,
+                    const int64_t *chain_blocks_host, const int32_t *chain_stream_host, int n_chains, int64_t steps,
+                    uint8_t *blocks_dev, int16_t *extents_dev, void *stream);
+/* The decoder's output, cut: region r = regions_host[r] = (i, y, x, h, w) int32, inside image i (shapes_host[i] = (H, W),
+ * cropped to multiples of 32 outside BSW_TILE_CODE), is written to out_dev as contiguous HWC uint8, the regions in
+ * turn (region r starts at C times the pixels of the regions before it).  Block g of chain c (chain start s0, nb blocks)
+ * is read from step s0 + nb - 1 - g of stream chain_stream_host[c] (-1: the chain was not decoded): the layout a decoder
+ * that pops every chain from its end leaves.  Regions may share blocks and span blocks and chains; every block a region
+ * needs must lie in a decoded chain at a step below `steps`. */
+int bsw_untile_regions(const int32_t *shapes_host, int n_images, int channels, int mode,
+                       const int64_t *chain_blocks_host, const int32_t *chain_stream_host, int n_chains, int n_streams,
+                       int64_t steps, const uint8_t *blocks_dev, const int32_t *regions_host, int n_regions,
+                       uint8_t *out_dev, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
