@@ -160,6 +160,8 @@ def _set_argtypes(L):
         "bsw_codec_fingerprint": [P, P, P],
         "bsw_tile_blocks": [P, I, I, I, P, P, I, L64, P, P, P],
         "bsw_untile_regions": [P, I, I, I, P, P, I, I, L64, P, P, I, P, P],
+        "bsw_block_digests": [P, P, I, L64, P, P, I, P, P],
+        "bsw_block_digests_check": [P, P, I, L64, P, P, I, P, P, P],
     }
     for name, args in sig.items():
         fn = getattr(L, name, None)
@@ -178,7 +180,7 @@ EXPORTS = ["bsw_last_error", "bsw_version", "bsw_has_tensor_cores", "bsw_measure
            "bsw_codec_encode", "bsw_codec_decode", "bsw_codec_encode_ext", "bsw_codec_decode_ext", "bsw_codec_last_launches", "bsw_codec_profile", "bsw_codec_set_two_phase", "bsw_codec_set_dual_stream", "bsw_codec_set_coder",
            "bsw_discretize_reset", "bsw_discretize_sample", "bsw_discretize_fold", "bsw_discretize_edges",
            "bsw_bitstream_revision", "bsw_digest", "bsw_model_digest", "bsw_bins_digest", "bsw_codec_fingerprint",
-           "bsw_tile_blocks", "bsw_untile_regions"]
+           "bsw_tile_blocks", "bsw_untile_regions", "bsw_block_digests", "bsw_block_digests_check"]
 
 
 def device_index(device=None):

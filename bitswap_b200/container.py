@@ -50,6 +50,17 @@ model digest [4], bins digest [4]), then scheme, hwc_quirk, excess_state_len and
 reference layout has w and the archive its ARCHIVE_MARK, so a reader of the unstamped layouts refuses a stamped array.  The
 decoders compare a stamp with codec.fingerprint() and their own scheme, hwc_quirk and channels before any stream is
 created, and refuse it naming every field that differs; a stamped container also gets the archives' initial-state check.
+
+Checksums (opt-in: checksums=True): any of the three layouts may carry a 32-bit digest of every coded block's pixels,
+    [ inner array, byte-identical to the unchecked one | digest per block, in block-sequence order | nblocks, CHECK_VERSION,
+      CHECK_MARK ]
+the block sequence being the image's row-major blocks for a container and the archive's global sequence for an archive;
+a stamp, when there is one too, goes after this trailer.  The digest (bsw_block_digest, include/bitswap_b200.h) covers the
+block's valid extent as the coding buffer holds it and is seeded with the block's index in its sequence and its extent.
+The writers digest the tiled buffer on the device; the decoders digest every block they decode (including blocks popped
+on the way to a window) and compare on the device, then raise ValueError naming the first mismatching block after the
+stream flags.  CHECK_MARK >= 2^31 sits where the unchecked layouts have their last word, so a reader of those refuses a
+checked array.
 """
 import collections
 import numbers
@@ -71,6 +82,8 @@ MAX_INITIAL_WORDS = 1 << 24              # largest excess_state_len an archive m
 STAMP_MARK = 0x80535450                  # bit 31 | "STP": last word of a stamped container or archive
 STAMP_VERSION = 1
 _STAMP_NFIELDS = {1: 26}                 # per version: 14 fingerprint words, two 4-word digests, 4 coding arguments
+CHECK_MARK = 0x80434B53                  # bit 31 | "CKS": last word of a checked container or archive
+CHECK_VERSION = 1
 
 Stamp = collections.namedtuple("Stamp", "fingerprint scheme hwc_quirk excess_state_len seed")
 Stamp.__doc__ = """What a stamped container or archive records about its writer: the codec's Fingerprint, the scheme (BITSWAP /
@@ -156,6 +169,43 @@ def _check_stamps(codec, stamps, scheme, hwc_quirk, channels, what):
         if diff:
             raise ValueError(f"{what} {i} was written by a different codec or with other arguments; it cannot be decoded "
                              f"here: " + "; ".join(diff))
+
+
+def _check_words(digests):
+    """The check trailer appended to an array whose blocks have these digests (uint32, block-sequence order)."""
+    return np.concatenate([np.asarray(digests, dtype=np.uint32),
+                           np.array([len(digests), CHECK_VERSION, CHECK_MARK], dtype=np.uint32)])
+
+
+def _split_check(a):
+    """(inner array, digests uint32 [nblocks]) of a checked array, (a, None) of any other.  The trailer is checked here,
+    before anything is sized from it; that nblocks matches the inner header is the caller's check (_check_count)."""
+    if a.ndim != 1 or a.size < 3 or int(a[-1]) != CHECK_MARK:
+        return a, None
+    nblocks, version = int(a[-3]), int(a[-2])
+    if version != CHECK_VERSION:
+        raise ValueError(f"check trailer of unknown version {version} (this reader knows {CHECK_VERSION})")
+    if nblocks > MAX_ARCHIVE_BLOCKS:
+        raise ValueError(f"check trailer: {nblocks} blocks, more than any array holds ({MAX_ARCHIVE_BLOCKS})")
+    if a.size < nblocks + 4:
+        raise ValueError(f"checked array of {a.size} words cannot hold its {nblocks} digests and a checked array")
+    inner = a[:a.size - 3 - nblocks]
+    if int(inner[-1]) == CHECK_MARK:
+        raise ValueError("a check trailer inside a check trailer")
+    if int(inner[-1]) == STAMP_MARK:
+        raise ValueError("a stamp inside a check trailer (a stamp goes after the check trailer)")
+    return inner, a[inner.size:a.size - 3]
+
+
+def _check_count(digests, nblocks, what):
+    if digests is not None and digests.size != nblocks:
+        raise ValueError(f"{what}: the check trailer holds {digests.size} digests, the header {nblocks} blocks")
+
+
+# What a decode job verifies: its block sequence as the sequences the digests were computed over (offsets int64 [n + 1]:
+# a container's image each, or one for an archive), the stored digests over the job's sequence (expected uint32) and which
+# blocks have one (checked bool: an unchecked container's blocks have none); archive: how an error names the chain.
+_Checks = collections.namedtuple("_Checks", "offsets expected checked archive")
 
 
 def extract_blocks(arr, block_size=(32, 32)):
@@ -361,7 +411,7 @@ def _chain_runs(nb, chain_blocks):
 
 
 def compress_images(codec, images, excess_state_len=10000, seed=100, scheme=BITSWAP, hwc_quirk=False, words_per_block=1400,
-                    edges="crop", chain_blocks=None, stamp=False):
+                    edges="crop", chain_blocks=None, stamp=False, checksums=False):
     """images: list of HWC uint8 images -- numpy arrays, CPU tensors, or CUDA tensors of any strides on the codec's device
     -- or one [N, H, W, C] array or tensor.  Returns one container array per image (numpy uint32, the same bytes whatever
     the images were held in).  The images are tiled into blocks on the device; host images go up in one copy.
@@ -374,6 +424,9 @@ def compress_images(codec, images, excess_state_len=10000, seed=100, scheme=BITS
     ceil(n / L) chains of contiguous blocks (chain_sizes), which run side by side.  Fewer serial steps, more initial bits.
     stamp=True: every container is followed by a stamp of codec.fingerprint() and these arguments (module docstring),
     which decompress_images checks; the container before it is unchanged.
+    checksums=True: every container is followed by a 32-bit digest of each of its blocks' pixels (module docstring),
+    against which every decoder checks each block it decodes; the container before it is unchanged, and a stamp goes
+    after the digests.
     A CUDA image that is not a uint8 H x W x C tensor with the codec's C, is on another device, or is empty (under 32 x 32
     with edges="crop") is a ValueError before any device work."""
     if edges not in ("crop", "code"):
@@ -394,10 +447,16 @@ def compress_images(codec, images, excess_state_len=10000, seed=100, scheme=BITS
     per_image, sizes = _chain_runs(gh * gw, chain_blocks)
     chains = list(zip((np.cumsum(sizes) - sizes).tolist(), sizes.tolist()))
     extents = None if mode != TILE_CODE else _sequence_extents(blocks.shapes)
-    coded = _encode(codec, blocks, extents, chains, scheme, excess_state_len, seed, words_per_block)
+    ioff = np.concatenate([[0], np.cumsum(gh * gw)]).astype(np.int64)
+    if checksums:
+        coded, digests = _encode_checked(codec, blocks, extents, chains, scheme, excess_state_len, seed, words_per_block, ioff)
+    else:
+        coded = _encode(codec, blocks, extents, chains, scheme, excess_state_len, seed, words_per_block)
     out, k = [], 0
-    for K, (h, w) in zip(per_image.tolist(), hw.tolist()):
+    for i, (K, (h, w)) in enumerate(zip(per_image.tolist(), hw.tolist())):
         out.append(pack_container(coded[k:k + K], h, w))
+        if checksums:
+            out[-1] = np.concatenate([out[-1], _check_words(digests[ioff[i]:ioff[i + 1]])])
         if stamp:
             out[-1] = np.concatenate([out[-1], tail])
         k += K
@@ -408,12 +467,24 @@ def _encode(codec, blocks, extents, chains, scheme, excess_state_len, seed, word
     """Codes a block sequence (blocks: a _Blocks; extents int16 [n, 2] or None) as the chains (start, nblocks) given, each a
     run of it, from the seeded initial state.  Returns [(words above the lowest depth, head, nblocks)] in chain order.
     Streams hold the chains largest first, so the active streams at each step are a prefix."""
+    return _encode_checked(codec, blocks, extents, chains, scheme, excess_state_len, seed, words_per_block, None)[0]
+
+
+def _encode_checked(codec, blocks, extents, chains, scheme, excess_state_len, seed, words_per_block, seq_offsets):
+    """_encode's chains and the block digests: None when seq_offsets is None, else uint32 [blocks], the digest of every
+    block in sequence order as tiled, seeded over the sequences seq_offsets (int64) lays end to end (bsw_block_digests)."""
     cnb = np.array([nb for _, nb in chains], dtype=np.int64)
     order = np.argsort(-cnb, kind="stable")
     nblk = cnb[order]
     stream = np.empty(len(cnb), dtype=np.int32)
     stream[order] = np.arange(len(cnb))
     x, ext = _tile(codec, blocks, cnb, stream, int(nblk[0]), extents is not None and not (extents == 32).all())
+    digests = None
+    if seq_offsets is not None:
+        # slot [t, j] holds block t of the chain on stream j, at sequence index start + t
+        start = np.array([s for s, _ in chains], dtype=np.int64)[order]
+        t = np.arange(int(nblk[0]), dtype=np.int64)[:, None]
+        digests = _digest_blocks(codec, x, ext, np.where(t < nblk[None, :], start[None, :] + t, -1), seq_offsets)
     w, head = initial_words(excess_state_len, seed=seed)
     # capacity: `words_per_block` words per 32x32 block of the longest chain (1400 = 14.6 bits/dim; 8 bits/dim of raw pixels
     # is 768).  A chain that still overflows is retried with twice the room instead of failing after it was coded.
@@ -426,8 +497,24 @@ def _encode(codec, blocks, extents, chains, scheme, excess_state_len, seed, word
             if attempt == 3:
                 raise
             continue
-        return [(words[offs[j]:offs[j + 1]], int(heads[j]), nb) for j, nb in zip(stream.tolist(), cnb.tolist())]
+        coded = [(words[offs[j]:offs[j + 1]], int(heads[j]), nb) for j, nb in zip(stream.tolist(), cnb.tolist())]
+        return coded, None if digests is None else digests.cpu().numpy().view(np.uint32)
     raise AssertionError("unreachable")
+
+
+def _digest_blocks(codec, x, ext, block, seq_offsets):
+    """The digests of the blocks in x [step, stream, C, 32, 32] (extents ext [step, stream, 2] or None: full), on the
+    device, on the current stream (bsw_block_digests): an int32 CUDA tensor [total blocks], in sequence order.  block:
+    int64 [step, stream], each slot's block in the sequence (-1: none); seq_offsets: int64, the sequences' offsets."""
+    seq_offsets = np.ascontiguousarray(seq_offsets, dtype=np.int64)
+    block = np.ascontiguousarray(block, dtype=np.int64).reshape(-1)
+    out = torch.zeros(int(seq_offsets[-1]), dtype=torch.int32, device=x.device)
+    if block.size:
+        with on_device(codec.device):
+            check(lib().bsw_block_digests(x.data_ptr(), None if ext is None else ext.data_ptr(), x.shape[2], block.size,
+                                          block.ctypes.data, seq_offsets.ctypes.data, len(seq_offsets) - 1,
+                                          out.data_ptr(), cuda_stream_ptr()))
+    return out
 
 
 def _tile(codec, blocks, cnb, stream, steps, ragged):
@@ -483,16 +570,23 @@ def _check_header(nblocks, h, w, hwc_quirk):
 def unpack_container(c, hwc_quirk=False):
     """Inverse of pack_container: (words uint32, offsets int64 [K+1], heads uint64 [K], nblocks int64 [K], h, w), chain k's
     words being words[offsets[k]:offsets[k+1]].  Every field is checked here, before anything is sized from it: a truncated
-    or inconsistent container is a ValueError.  A stamped container is accepted: its stamp is checked and stripped."""
-    c = _split_stamp(np.asarray(c, dtype=np.uint32))[0]
+    or inconsistent container is a ValueError.  A stamped or checked container is accepted: its stamp and check trailer
+    are checked and stripped."""
+    return _unpack_container(c, hwc_quirk)[:-1]
+
+
+def _unpack_container(c, hwc_quirk):
+    """unpack_container's tuple and the container's block digests (None for an unchecked container)."""
+    c, digests = _split_check(_split_stamp(np.asarray(c, dtype=np.uint32))[0])
     if c.ndim != 1 or c.size < 5:
         raise ValueError(f"container too short ({c.size} words): needs at least head_lo, head_hi, nblocks, h, w")
     if int(c[-1]) != CHAIN_MARK:
         nblocks, h, w = int(c[-3]), int(c[-2]), int(c[-1])                                      # demo_decompress.py:216-219
         _check_header(nblocks, h, w, hwc_quirk)
+        _check_count(digests, nblocks, "container")
         head = (int(c[-4]) << 32) | int(c[-5])                                                  # :222
         return (c[:-5], np.array([0, c.size - 5], dtype=np.int64), np.array([head], dtype=np.uint64),
-                np.array([nblocks], dtype=np.int64), h, w)
+                np.array([nblocks], dtype=np.int64), h, w, digests)
     k, h, w = int(c[-4]), int(c[-3]), int(c[-2])
     if k < 2 or c.size < 4 * k + 4:
         raise ValueError(f"multi-chain container of {c.size} words cannot hold the table of its {k} chains")
@@ -501,13 +595,14 @@ def unpack_container(c, hwc_quirk=False):
     if (nblocks < 1).any():
         raise ValueError("multi-chain container: a chain with no blocks")
     _check_header(int(nblocks.sum()), h, w, hwc_quirk)                 # (so also K <= blocks, as each chain has one)
+    _check_count(digests, int(nblocks.sum()), "multi-chain container")
     body = c.size - 4 * k - 4
     if int(nwords.sum()) != body:
         raise ValueError(f"multi-chain container: the chains claim {int(nwords.sum())} words, the container holds {body}")
     offsets = np.zeros(k + 1, dtype=np.int64)
     np.cumsum(nwords, out=offsets[1:])
     heads = (table[:, 2].astype(np.uint64) << np.uint64(32)) | table[:, 1].astype(np.uint64)
-    return c[:body], offsets, heads, nblocks, h, w
+    return c[:body], offsets, heads, nblocks, h, w, digests
 
 
 RegionPlan = collections.namedtuple("RegionPlan", "first depth needed")
@@ -575,22 +670,28 @@ def plan_regions(containers, regions, hwc_quirk=False):
 
 
 def _stamped_job(codec, containers, channels, scheme, hwc_quirk):
-    """The decode job of a list of containers, every stamp checked against the codec and the arguments, and each chain's
+    """The decode job of a list of containers, every stamp checked against the codec and the arguments; each chain's
     seeded initial state (words, head) where its container is stamped (None where it is not; None alone when no
-    container is stamped)."""
+    container is stamped); and the job's _Checks (None when no container is checked)."""
     split = [_split_stamp(np.asarray(c, dtype=np.uint32)) for c in containers]
-    parsed = [unpack_container(inner, hwc_quirk) for inner, _ in split]
+    parsed = [_unpack_container(inner, hwc_quirk) for inner, _ in split]
     _check_stamps(codec, [st for _, st in split], scheme, hwc_quirk, channels, "container")
     states, initial = {}, []
     for (_, st), p in zip(split, parsed):
         if st is not None and (st.excess_state_len, st.seed) not in states:
             states[st.excess_state_len, st.seed] = initial_words(st.excess_state_len, seed=st.seed)
         initial += [None if st is None else states[st.excess_state_len, st.seed]] * len(p[3])
-    return _containers_job(parsed), initial if states else None
+    job = _containers_job(parsed)
+    checks = None
+    if any(p[6] is not None for p in parsed):
+        nb = np.diff(job.ioff)
+        checks = _Checks(job.ioff, np.concatenate([np.zeros(n, np.uint32) if p[6] is None else p[6] for p, n in zip(parsed, nb)]),
+                         np.repeat([p[6] is not None for p in parsed], nb), False)
+    return job, initial if states else None, checks
 
 
 def decompress_regions(codec, containers, regions, channels=3, scheme=BITSWAP, hwc_quirk=False, headroom_words=None,
-                       as_tensors=False):
+                       as_tensors=False, verify=True):
     """regions: list of (i, y, x, h, w) -> one HWC uint8 array per region, equal to decompress_images(...)[i][y:y+h, x:x+w].
     Only the chains holding a wanted block are imported, and each is popped only down to the earliest block any region on
     its container wants (plan_regions): a chain of n blocks whose earliest wanted block is j costs n - j block decodes.
@@ -598,26 +699,35 @@ def decompress_regions(codec, containers, regions, channels=3, scheme=BITSWAP, h
     A stamped container must match the codec's fingerprint, scheme, hwc_quirk and channels (ValueError naming every field
     that differs, before any decoding), and each of its chains popped down to its first block must come back to the
     stamp's initial state.
+    A checked container (compress_images(checksums=True)) has every block decoded here, including the blocks popped on
+    the way to a window, compared with its stored digest on the device; after the stream flags (IndexError,
+    OverflowError), a mismatch is a ValueError naming how many blocks differ and the first one's image, block row and
+    column, and chain.  verify=False skips that comparison.
     as_tensors=True: contiguous torch.uint8 [h, w, C] tensors on the codec's device instead, the same pixels; no pixel
     crosses PCIe.  Either way the regions are cut on the device and the decode is complete when this returns."""
-    job, initial = _stamped_job(codec, containers, channels, scheme, hwc_quirk)
-    return _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_words, initial, as_tensors)
+    job, initial, checks = _stamped_job(codec, containers, channels, scheme, hwc_quirk)
+    return _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_words, initial, as_tensors,
+                           checks if verify else None)
 
 
-def decompress_images(codec, containers, channels=3, scheme=BITSWAP, hwc_quirk=False, headroom_words=None, as_tensors=False):
+def decompress_images(codec, containers, channels=3, scheme=BITSWAP, hwc_quirk=False, headroom_words=None, as_tensors=False,
+                      verify=True):
     """Inverse of compress_images: list of container arrays -> list of HWC uint8 images (the cropped size for a crop-mode
     container, the full size for an edge-coded one: a header whose h or w is not a multiple of 32).  Single- and
-    multi-chain containers can be mixed in one call, and so can stamped and unstamped ones (see decompress_regions).
+    multi-chain containers can be mixed in one call, and so can stamped and unstamped, checked and unchecked ones (see
+    decompress_regions; verify=False skips the block digests).
     as_tensors=True: contiguous torch.uint8 [h, w, C] CUDA tensors on the codec's device instead of numpy arrays."""
-    job, initial = _stamped_job(codec, containers, channels, scheme, hwc_quirk)
+    job, initial, checks = _stamped_job(codec, containers, channels, scheme, hwc_quirk)
     return _decode_regions(codec, job, [(i, 0, 0, h, w) for i, (h, w) in enumerate(job.shapes)], channels, scheme,
-                           hwc_quirk, headroom_words, initial, as_tensors)
+                           hwc_quirk, headroom_words, initial, as_tensors, checks if verify else None)
 
 
-def _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_words, initial=None, as_tensors=False):
+def _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_words, initial=None, as_tensors=False,
+                   checks=None):
     """Decodes the job's regions.  channels None: the codec's.  initial: per chain, None or the seeded initial state
     (words, head) it started from; such a chain popped down to its first block must then hold its top words and head, or
-    ValueError.  as_tensors: CUDA tensors instead of numpy arrays."""
+    ValueError.  as_tensors: CUDA tensors instead of numpy arrays.  checks: None or the job's _Checks; every decoded block
+    that has a stored digest must then match it, or ValueError."""
     regions, plan = _plan(job, regions)
     if not regions:
         return []
@@ -650,7 +760,15 @@ def _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_w
     stream = np.full(len(cnb), -1, dtype=np.int32)
     stream[order] = np.arange(n)
     out = _untile(codec, job, regions, stream, dev, TILE_QUIRK if hwc_quirk else TILE_CODE)
+    if checks is not None:
+        # slot [s, j] holds block cend_j - 1 - s of the sequence for s < depth_j; blocks without a digest are skipped
+        g = (cstart + cnb)[order][None, :] - 1 - np.arange(int(depth[0]), dtype=np.int64)[:, None]
+        live = (g >= (cstart + cnb - plan.depth)[order][None, :])
+        block = np.where(live & checks.checked[np.where(live, g, 0)], g, -1)
+        result = _verify_blocks(codec, dev, ext, block, checks)
     ss.raise_on_error()                                                    # (synchronises the device)
+    if checks is not None:
+        _raise_on_mismatch(job, checks, *result.cpu().tolist())
     if initial is not None:
         _check_initial_state(ss, order, plan.first[order] == 0, initial)
     size = np.array([h * w * channels for _, _, _, h, w in regions], dtype=np.int64)
@@ -659,6 +777,34 @@ def _decode_regions(codec, job, regions, channels, scheme, hwc_quirk, headroom_w
         out = out.cpu().numpy()
     return [out[o:o + m].view(h, w, channels) if as_tensors else out[o:o + m].reshape(h, w, channels)
             for o, m, (_, _, _, h, w) in zip(start, size.tolist(), regions)]
+
+
+def _verify_blocks(codec, x, ext, block, checks):
+    """bsw_block_digests_check of the decoded blocks in x [step, stream, C, 32, 32] on the current stream: an int64 CUDA
+    tensor (blocks that differ from their stored digest, the lowest such index in the job's sequence)."""
+    block = np.ascontiguousarray(block, dtype=np.int64).reshape(-1)
+    offsets = np.ascontiguousarray(checks.offsets, dtype=np.int64)
+    expected = torch.from_numpy(np.ascontiguousarray(checks.expected, dtype=np.uint32).view(np.int32)).to(x.device)
+    result = torch.empty(2, dtype=torch.int64, device=x.device)
+    with on_device(codec.device):
+        check(lib().bsw_block_digests_check(x.data_ptr(), None if ext is None else ext.data_ptr(), x.shape[2], block.size,
+                                            block.ctypes.data, offsets.ctypes.data, len(offsets) - 1, expected.data_ptr(),
+                                            result.data_ptr(), cuda_stream_ptr()))
+    return result
+
+
+def _raise_on_mismatch(job, checks, bad, g):
+    """ValueError naming the first of `bad` decoded blocks whose digest differs (g: its index in the job's sequence)."""
+    if not bad:
+        return
+    i = int(np.searchsorted(job.ioff, g, side="right")) - 1
+    by, bx = divmod(g - int(job.ioff[i]), block_grid(*job.shapes[i])[1])
+    k = int(np.searchsorted(job.cstart, g, side="right")) - 1
+    where = f"chain {k} of the archive" if checks.archive else \
+        f"chain {k - int(np.searchsorted(job.cstart, job.ioff[i]))} of container {i}"
+    raise ValueError(f"{bad} decoded block{'s' if bad > 1 else ''} differ{'' if bad > 1 else 's'} from the stored digest: "
+                     f"the first is image {i}, block row {by}, column {bx}, in {where}.  The codec is not the encoder's "
+                     f"(coder, tc_precision, conv path, weights, bins or build), or the array is corrupt")
 
 
 def _decode_extents(codec, job, cend, depth):
@@ -718,13 +864,15 @@ def unpack_archive(a):
     """Inverse of pack_archive: (words uint32, offsets int64 [K+1], heads uint64 [K], nblocks int64 [K], shapes int64 [N, 2],
     excess_state_len, seed, scheme), chain k's words being words[offsets[k]:offsets[k+1]].  Every field is checked here,
     before anything is sized from it: a truncated or inconsistent archive is a ValueError.  A stamped archive is accepted:
-    its stamp is checked, must agree with the header's scheme and initial state, and is stripped."""
-    return _unpack_archive(a)[:-1]
+    its stamp is checked, must agree with the header's scheme and initial state, and is stripped; so is a checked
+    archive's check trailer."""
+    return _unpack_archive(a)[:-2]
 
 
 def _unpack_archive(a):
-    """unpack_archive's tuple and the archive's Stamp (or None)."""
+    """unpack_archive's tuple, the archive's Stamp (or None) and its block digests (or None)."""
     a, stamp = _split_stamp(np.asarray(a, dtype=np.uint32))
+    a, digests = _split_check(a)
     if a.ndim != 1 or a.size < 6 or int(a[-1]) != ARCHIVE_MARK:
         raise ValueError("not an archive: it must be a 1-D uint32 array ending in ARCHIVE_MARK")
     k, n, n_init, seed, scheme = (int(v) for v in a[-6:-1])
@@ -744,6 +892,7 @@ def _unpack_archive(a):
     if int(nblocks.sum()) != int(blocks.sum()) or int(blocks.sum()) > MAX_ARCHIVE_BLOCKS:
         raise ValueError(f"archive: the chains hold {int(nblocks.sum())} blocks, the images {int(blocks.sum())} "
                          f"(at most {MAX_ARCHIVE_BLOCKS})")
+    _check_count(digests, int(blocks.sum()), "archive")
     if int(nwords.sum()) != body:
         raise ValueError(f"archive: the chains claim {int(nwords.sum())} words, the archive holds {body}")
     if not 2 <= n_init <= MAX_INITIAL_WORDS:
@@ -758,20 +907,23 @@ def _unpack_archive(a):
     offsets = np.zeros(k + 1, dtype=np.int64)
     np.cumsum(nwords, out=offsets[1:])
     heads = (table[:, 2].astype(np.uint64) << np.uint64(32)) | table[:, 1].astype(np.uint64)
-    return a[:body], offsets, heads, nblocks, shapes, n_init, seed, scheme, stamp
+    return a[:body], offsets, heads, nblocks, shapes, n_init, seed, scheme, stamp, digests
 
 
 def _archive_job(a):
-    words, offsets, heads, nblocks, shapes, n_init, seed, scheme, stamp = _unpack_archive(a)
+    """The decode job of an archive, its header's initial state and scheme, its Stamp and its _Checks (or None)."""
+    words, offsets, heads, nblocks, shapes, n_init, seed, scheme, stamp, digests = _unpack_archive(a)
     ioff = np.zeros(len(shapes) + 1, dtype=np.int64)
     np.cumsum(-(-shapes[:, 0] // 32) * -(-shapes[:, 1] // 32), out=ioff[1:])
     job = _Job([words[offsets[k]:offsets[k + 1]] for k in range(len(heads))], heads, np.cumsum(nblocks) - nblocks, nblocks,
                [(int(h), int(w)) for h, w in shapes], ioff)
-    return job, n_init, seed, scheme, stamp
+    checks = None if digests is None else \
+        _Checks(np.array([0, ioff[-1]], dtype=np.int64), digests, np.ones(digests.size, dtype=bool), True)
+    return job, n_init, seed, scheme, stamp, checks
 
 
 def compress_archive(codec, images, chain_blocks=64, scheme=BITSWAP, excess_state_len=10000, seed=100, words_per_block=1400,
-                     stamp=False):
+                     stamp=False, checksums=False):
     """images: a sequence of HWC uint8 images of any sizes (H, W >= 1, C = the model's) -- numpy arrays, CPU tensors, or CUDA
     tensors of any strides on the codec's device -- or one [N, H, W, C] array or tensor -> one np.uint32 archive.
     Each image is tiled as compress_images(edges="code") tiles it; the row-major blocks of all images, in the order given,
@@ -779,7 +931,9 @@ def compress_archive(codec, images, chain_blocks=64, scheme=BITSWAP, excess_stat
     initial state.  A chain may start or end inside an image, so the initial words are paid once per chain, not once per
     image.  chain_blocks None: one chain over everything (the reference's experiment layout, cifar_compress.py).
     stamp=True: the archive is followed by a stamp of codec.fingerprint() and these arguments (module docstring), which
-    decompress_archive checks; the archive before it is unchanged."""
+    decompress_archive checks; the archive before it is unchanged.
+    checksums=True: the archive is followed by a 32-bit digest of each block's pixels, in the archive's block sequence
+    (module docstring), against which decompress_archive checks each block it decodes; a stamp goes after the digests."""
     chain_blocks = _check_chain_blocks(chain_blocks)
     if not (torch.is_tensor(images) or isinstance(images, np.ndarray)):
         images = list(images)
@@ -794,9 +948,14 @@ def compress_archive(codec, images, chain_blocks=64, scheme=BITSWAP, excess_stat
     sizes = chain_sizes(total, chain_blocks)
     chains = list(zip(np.cumsum([0] + sizes[:-1]).tolist(), sizes))
     tail = _stamp_words(codec.fingerprint(), scheme, False, int(excess_state_len), int(seed)) if stamp else None
-    coded = _encode(codec, blocks, _sequence_extents(blocks.shapes), chains, scheme, int(excess_state_len), int(seed),
-                    words_per_block)
+    args = (codec, blocks, _sequence_extents(blocks.shapes), chains, scheme, int(excess_state_len), int(seed), words_per_block)
+    if checksums:
+        coded, digests = _encode_checked(*args, np.array([0, total], dtype=np.int64))
+    else:
+        coded = _encode(*args)
     a = pack_archive(coded, blocks.shapes, int(excess_state_len), int(seed), scheme)
+    if checksums:
+        a = np.concatenate([a, _check_words(digests)])
     return a if tail is None else np.concatenate([a, tail])
 
 
@@ -807,18 +966,21 @@ def plan_archive(archive, regions=None):
     return _plan(job, _all_images(job) if regions is None else regions)[1]
 
 
-def decompress_archive(codec, archive, regions=None, as_tensors=False):
+def decompress_archive(codec, archive, regions=None, as_tensors=False, verify=True):
     """regions None -> every image of the archive, exactly as given; else a list of (i, y, x, h, w) over image i -> one HWC
     uint8 array per region, byte-identical to the crop of the full decode.  Each chain holding a wanted block is popped
     from its end down to the earliest wanted block in it (plan_archive).  Every chain popped down to its first block must
     come back to the seeded initial state it was coded from; otherwise ValueError naming the chain.  A stamped archive must
-    match the codec's fingerprint (ValueError naming every field that differs, before any decoding).  as_tensors=True:
-    contiguous torch.uint8 [h, w, C] CUDA tensors on the codec's device instead of numpy arrays."""
-    job, n_init, seed, scheme, stamp = _archive_job(archive)
+    match the codec's fingerprint (ValueError naming every field that differs, before any decoding).  Every block a
+    checked archive has decoded here must match its stored digest (ValueError naming the first that does not, after the
+    stream flags; verify=False skips it).  as_tensors=True: contiguous torch.uint8 [h, w, C] CUDA tensors on the codec's
+    device instead of numpy arrays."""
+    job, n_init, seed, scheme, stamp, checks = _archive_job(archive)
     regions = _all_images(job) if regions is None else regions
     _check_stamps(codec, [stamp], scheme, False, None, "archive")
     return _decode_regions(codec, job, regions, None, scheme, False, None,
-                           initial=[initial_words(n_init, seed=seed)] * len(job.cnb), as_tensors=as_tensors)
+                           initial=[initial_words(n_init, seed=seed)] * len(job.cnb), as_tensors=as_tensors,
+                           checks=checks if verify else None)
 
 
 def _all_images(job):

@@ -487,6 +487,41 @@ int bsw_untile_regions(const int32_t *shapes_host, int n_images, int channels, i
                        int64_t steps, const uint8_t *blocks_dev, const int32_t *regions_host, int n_regions,
                        uint8_t *out_dev, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Per-block pixel digests (checksums.cu): what a checked container or archive stores for every coded block, so that a
+ * decoder can tell a block it decoded wrong from one it decoded right.  They catch accidents (another coder, arithmetic,
+ * build or libm than the encoder's; a corrupt array), NOT tampering: nothing here is cryptographic.
+ *
+ * bsw_block_digest of one slot [C][32][32] of a block buffer (the layout of bsw_tile_blocks) that holds block i of its
+ * block sequence (i counted from the sequence's first block) with valid extent (vh, vw) ((32, 32) for a full block and
+ * for every BSW_TILE_QUIRK slot, whose C*1024 bytes are then covered in slot order), with integer operations only:
+ *   - s = mix64(((i << 16) | (vh << 8) | vw) ^ 0x424C4F434B534551)                       (i < 2^31, vh, vw in [0, 32])
+ *   - lane l = 0 .. 31 starts from a_l = lo32(mix64(s + l + 1)); if l < vw it takes the bytes x[c][r][l] for
+ *     c = 0 .. C-1, and in each c r = 0 .. vh-1, in that order:   a_l = rotl32(a_l ^ x, 13) * 0x9E3779B1  (mod 2^32);
+ *   - h = hi32(s), then for l = 0 .. 31 in order h = fmix32(h ^ a_l); the digest is h.
+ *   mix64 is the splitmix64 finaliser of bsw_digest; fmix32 is murmur3's (h ^= h >> 16; h *= 0x85EBCA6B; h ^= h >> 13;
+ *   h *= 0xC2B2AE35; h ^= h >> 16).  Every step is a bijection of the byte or word it takes, so one changed byte inside
+ *   the extent always changes the digest; bytes outside it are not read.  The seed makes a block decoded into another
+ *   place of the sequence, or with another extent, fail as well.
+ *
+ * A block buffer of n_slots slots (e.g. [steps][n_streams] flattened) and, per slot, block_host[q] (int64): the index of
+ * the block it holds in one block sequence made of n_seqs sequences laid end to end, sequence k holding blocks
+ * seq_offsets_host[k] .. seq_offsets_host[k + 1] (seq_offsets_host[0] = 0, non-decreasing, at most 2^31 - 1 in all), or
+ * -1 for a slot to skip.  A block is digested as block g - seq_offsets_host[k] of its own sequence k.  extents_dev: int16
+ * [n_slots][2] (vh, vw) on the device, or NULL for full blocks.  Validated on the host before anything is uploaded or
+ * launched (BSW_E_INVALID, nothing enqueued): null pointers, n_slots, n_seqs >= 1, 1 <= channels <= 4, the offsets, every
+ * block index in [-1, total) and no block in two slots.  Both calls are enqueued on `stream` and do not synchronise.
+ * bsw_block_digests: digests_dev[g] (uint32 [total]) receives the digest of every block g in a slot; other entries are
+ *   left alone.
+ * bsw_block_digests_check: compares each such digest with expected_dev[g] (uint32 [total]) and writes result_dev (int64
+ *   [2], device) = {blocks that differ, the lowest index g among them (INT64_MAX if none)}. */
+int bsw_block_digests(const uint8_t *blocks_dev, const int16_t *extents_dev, int channels, int64_t n_slots,
+                      const int64_t *block_host, const int64_t *seq_offsets_host, int n_seqs, uint32_t *digests_dev,
+                      void *stream);
+int bsw_block_digests_check(const uint8_t *blocks_dev, const int16_t *extents_dev, int channels, int64_t n_slots,
+                            const int64_t *block_host, const int64_t *seq_offsets_host, int n_seqs,
+                            const uint32_t *expected_dev, int64_t *result_dev, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
